@@ -1,5 +1,5 @@
 /*
- * urf.h — C-ABI of liburf_b200.so: the B200-native replacement for the per-scan road/curb classification path of
+ * urf.h — C-ABI of liburf_b200.so: the H100-native (sm_90a) replacement for the per-scan road/curb classification path of
  * jkk-research/urban_road_filter.
  *
  * Reference interface replaced (all paths relative to the reference repo root):

@@ -3,8 +3,11 @@
 urf_logic.cuh functions the kernels call, in the kernels' stage order) against the oracle port and, where it is built,
 against the unmodified reference (oracle/_ref), on seeded random parameter draws over the LidarFilters.cfg ranges and
 varied clouds (sensor layouts, flat worlds, quantised ranges = equal radii, random clouds). No GPU needed.
-usage: fuzz_model.py [first_seed] [count] [big]   -> one line per mismatch, a summary line at the end
-("big": whole OS1-64 / HDL-64E / OS2-128 scans instead of the small clouds, a few tenths of a second per case and side)"""
+usage: fuzz_model.py [first_seed] [count] [big] [--record]   -> one line per mismatch, a summary line at the end
+("big": whole OS1-64 / HDL-64E / OS2-128 scans instead of the small clouds, a few tenths of a second per case and side)
+Where the reference is not built, the small cases are checked against the sha256 of the reference's labels stored in
+tests/golden/ref/fuzz_labels.json; --record (reference built) adds the cases of this run to that file."""
+import json
 import os
 import sys
 import time
@@ -17,13 +20,19 @@ import numpy as np  # noqa: E402
 from oracle.pyoracle import PortOracle, RefOracle  # noqa: E402
 from urban_road_filter_b200 import FULL_ROI, make_params  # noqa: E402
 from urban_road_filter_b200.synth import make_scan, random_cloud  # noqa: E402
-from util import CpuModel, stage_diffs  # noqa: E402
+from util import REF_DIR, CpuModel, digest, stage_diffs  # noqa: E402
 
-first = int(sys.argv[1]) if len(sys.argv) > 1 else 0
-count = int(sys.argv[2]) if len(sys.argv) > 2 else 50
-big = len(sys.argv) > 3 and sys.argv[3] == "big"
+record = "--record" in sys.argv
+argv = [a for a in sys.argv if a != "--record"]
+first = int(argv[1]) if len(argv) > 1 else 0
+count = int(argv[2]) if len(argv) > 2 else 50
+big = len(argv) > 3 and argv[3] == "big"
 port, model = PortOracle(), CpuModel()
 ref = RefOracle() if RefOracle.available() else None
+DIGESTS = os.path.join(REF_DIR, "fuzz_labels.json")
+stored = {} if big or not os.path.exists(DIGESTS) else json.load(open(DIGESTS))   # seed -> sha256 of the labels, None: it crashed
+if record and (ref is None or big):
+    sys.exit("--record needs the reference built (oracle/_ref) and the small cases")
 bad = nref = nties = ncrash = 0
 road = curb = 0
 t0 = time.time()
@@ -94,5 +103,16 @@ for seed in range(first, first + count):
             if not np.array_equal(rl, np.asarray(m.label)):
                 bad += 1
                 print(f"seed {seed} kind {kind}: model vs REFERENCE labels differ at {int((rl != np.asarray(m.label)).sum())} points (flags {m.flags})", flush=True)
+        if record:
+            stored[str(seed)] = None if status != 0 else digest(rl)
+    elif ref is None and stored.get(str(seed)) is not None:
+        nref += 1
+        if digest(m.label) != stored[str(seed)]:
+            bad += 1
+            print(f"seed {seed} kind {kind}: model labels differ from the REFERENCE's (stored digest; flags {m.flags})", flush=True)
+if record:
+    with open(DIGESTS, "w") as f:
+        json.dump(dict(sorted(stored.items(), key=lambda kv: int(kv[0]))), f, indent=0)
+        f.write("\n")
 print(f"fuzz_model: seeds {first}..{first + count - 1}: {count} cases vs the port, {nref} of them also vs the unmodified reference, "
       f"{ncrash} reference crashes, {nties} with equal radii in a sector, {road} road / {curb} curb labels; mismatching cases {bad}; {time.time() - t0:.0f} s")

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Registers / spills / shared memory per kernel (ptxas -v) and the Blackwell/Hopper-class SASS mnemonics each kernel
 contains (cluster barriers UCGABAR_*, distributed-shared-memory mapping, warp REDUX, MATCH, 64-bit shared atomics).
-usage: python scripts/ptxas_table.py > profiles/r02_ptxas_sass_<version>.txt   (no GPU needed: nvcc cross-compiles)"""
+usage: python scripts/ptxas_table.py > ptxas_sass.txt   (no GPU needed: nvcc cross-compiles)"""
 import os, re, subprocess, sys, collections
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)

@@ -1,8 +1,11 @@
-"""Generates tests/golden/*.npz by running the UNMODIFIED reference (oracle/_ref/liburf_ref.so, built from
-/root/reference/src by `make -C oracle ref`) on seeded synthetic clouds. Run here, in the build container; the fixtures
-travel to the GPU box where /root/reference does not exist.
+"""Generates tests/golden/*.npz by running the UNMODIFIED reference (oracle/_ref/liburf_ref.so, built from the reference's
+sources by `make -C oracle ref REF=<reference checkout>`) on seeded synthetic clouds. The fixtures are committed, so the
+tests need neither the reference's sources nor its build.
 
-    python tests/golden/make_golden.py
+    python tests/golden/make_golden.py                 # everything but the C5 fixtures
+    python tests/golden/make_golden.py --only c5
+    python tests/golden/make_golden.py --ref-checks    # tests/golden/ref/: the reference's outputs for the random-parameter
+                                                       # draws of tests/test_oracle.py and the strips of tests/test_markers.py
 
 Each fixture holds: params (cfg overrides), the input cloud (or, for big clouds, the generator recipe + sha256 of the
 bytes it must produce), and what the reference published: per-point labels (recovered from the roi/road/curb clouds),
@@ -21,10 +24,12 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 from oracle.pyoracle import RefOracle  # noqa: E402
 from urban_road_filter_b200 import FULL_ROI, make_params  # noqa: E402
 from urban_road_filter_b200.synth import SHAPES, make_scan, random_cloud  # noqa: E402
+from util import MARKER_EPS, REF_DIR, cloud_digest, digest, random_param_case  # noqa: E402
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 
@@ -69,7 +74,32 @@ def strips_to_arrays(strips):
     return meta, pts.astype(np.float64)
 
 
+def ref_checks():
+    ref = RefOracle()
+    os.makedirs(REF_DIR, exist_ok=True)
+    draws = {}
+    for seed in range(6):
+        pts, prm = random_param_case(seed)
+        r = ref.run(pts, prm)
+        draws[str(seed)] = dict(cloud_sha256=cloud_digest(pts), published=r.published, label=digest(r.label),
+                                road_ids=digest(r.road_ids), curb_ids=digest(r.curb_ids))
+    with open(os.path.join(REF_DIR, "random_params.json"), "w") as f:
+        json.dump(draws, f, indent=1, sort_keys=True)
+        f.write("\n")
+    strips = {}
+    for seed in range(4):
+        pts = make_scan("C1", 20 + seed)
+        strips[f"s{seed}_cloud_sha256"] = cloud_digest(pts)
+        for k, eps in enumerate(MARKER_EPS):
+            r = ref.run(pts, make_params(poly_s_param=eps, **FULL_ROI), ghostcount=0)
+            strips[f"s{seed}_e{k}_published"] = np.int32(r.markers_published)
+            strips[f"s{seed}_e{k}_meta"], strips[f"s{seed}_e{k}_pts"] = strips_to_arrays(r.strips)
+    np.savez_compressed(os.path.join(REF_DIR, "marker_strips.npz"), **strips)
+
+
 def main():
+    if "--ref-checks" in sys.argv:
+        return ref_checks()
     only = sys.argv[sys.argv.index("--only") + 1] if "--only" in sys.argv else ""      # name prefix; default: everything but c5
     ref = RefOracle()
     env = dict(machine=platform.machine(), libc=" ".join(platform.libc_ver()), python=platform.python_version(),

@@ -74,8 +74,6 @@ def test_glue_publishes_what_the_reference_published(name, step):
     Velodyne-sized records."""
     lib = _lib()
     g = Golden(name)
-    if step and name.startswith(("c2", "c3", "c4")) and step == 32:
-        pytest.skip("one record size is enough for the large fixtures")
     label, emit, prob, counts, strips, _ = _run(lib, g, g.params(simple_poly_allow=0, poly_z_avg_allow=0), 0, step)
     assert bool(counts[0]) == g.published
     if not g.published:

@@ -2,11 +2,14 @@
 reference tree, so `simplify` is PARITY UNPINNED (DESIGN.md): the product states the published algorithm iteratively
 (urban_road_filter_b200/csrc/urf_markers.cpp), the reference build of the oracle states it recursively
 (oracle/shim/boost/geometry.hpp). These tests pin both to the algorithm's defining properties and to each other."""
+import os
+
 import numpy as np
 import pytest
 
-from oracle.pyoracle import RefOracle
+from oracle.pyoracle import PortOracle
 from urban_road_filter_b200 import api, make_params
+from util import MARKER_EPS, REF_DIR, Golden, cloud_digest
 
 
 def strip_points(vert_xy, eps, simplify=True):
@@ -77,23 +80,23 @@ def test_simplify_collinear_and_degenerate():
     assert len(strip_points(closed, 0.7)) == 3
 
 
-@pytest.mark.skipif(not RefOracle.available(), reason="oracle/_ref is built from /root/reference (this container only)")
 @pytest.mark.parametrize("seed", range(4))
 def test_iterative_and_recursive_statements_agree(seed):
     """The product (iterative) against the reference build, whose marker tail (the unmodified lidar_segmentation.cpp:369-602)
-    calls the shim's recursive statement: same strips for the same candidate vertices, at several tolerances."""
+    calls the shim's recursive statement: same strips for the same candidate vertices, at several tolerances. The
+    reference's strips are stored in tests/golden/ref/marker_strips.npz (tests/golden/make_golden.py --ref-checks)."""
     from urban_road_filter_b200 import FULL_ROI
     from urban_road_filter_b200.synth import make_scan
-    ref = RefOracle()
+    ref = np.load(os.path.join(REF_DIR, "marker_strips.npz"))
     pts = make_scan("C1", 20 + seed)
-    for eps in (0.05, 0.7, 3.0):
-        prm = make_params(poly_s_param=eps, **FULL_ROI)
-        r = ref.run(pts, prm, ghostcount=0)
-        if not r.markers_published:
+    assert cloud_digest(pts) == str(ref[f"s{seed}_cloud_sha256"]), "the synthetic generator no longer reproduces the stored input cloud"
+    for k, eps in enumerate(MARKER_EPS):
+        if not ref[f"s{seed}_e{k}_published"]:
             continue
-        from oracle.pyoracle import PortOracle
+        prm = make_params(poly_s_param=eps, **FULL_ROI)
         o = PortOracle().run(pts, prm)
         mine, _ = api.build_markers(prm, o.vert, 0)
-        assert len(mine) == len(r.strips)
-        for a, b in zip(mine, r.strips):
+        theirs = Golden._strips(ref[f"s{seed}_e{k}_meta"], ref[f"s{seed}_e{k}_pts"])
+        assert len(mine) == len(theirs)
+        for a, b in zip(mine, theirs):
             assert a[:3] == b[:3] and a[3].shape == b[3].shape and np.allclose(a[3], b[3], atol=1e-6)

@@ -83,11 +83,14 @@ def test_model_zero_elevation_quirk(both):
 
 def test_model_fuzz_short():
     """A short run of scripts/fuzz_model.py (random parameter draws x varied clouds; model vs port and vs the unmodified
-    reference where it is built). The long run (3000 cases, 0 mismatches) is recorded in DESIGN.md §2."""
+    reference, run where it is built, else its stored label digests). The long run (3000 cases, 0 mismatches) is recorded
+    in DESIGN.md §2."""
     import os
+    import re
     import subprocess
     import sys
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     out = subprocess.run([sys.executable, os.path.join(root, "scripts", "fuzz_model.py"), "0", "60"], capture_output=True, text=True, timeout=900)
     assert out.returncode == 0, out.stderr[-2000:]
     assert "mismatching cases 0;" in out.stdout, out.stdout[-2000:]
+    assert int(re.search(r"(\d+) of them also vs the unmodified reference", out.stdout).group(1)) >= 40, out.stdout[-2000:]

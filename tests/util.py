@@ -15,12 +15,38 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
 from oracle.pyoracle import OracleDebug  # noqa: E402
-from urban_road_filter_b200 import UrfParams, UrfResult, make_params  # noqa: E402
+from urban_road_filter_b200 import FULL_ROI, UrfParams, UrfResult, make_params  # noqa: E402
 from urban_road_filter_b200.ctypes_abi import URF_MAX_CHANNELS, URF_MAX_VERTS  # noqa: E402
 from urban_road_filter_b200.synth import make_scan, random_cloud  # noqa: E402
 
 GOLDEN_DIR = os.path.join(ROOT, "tests", "golden")
+REF_DIR = os.path.join(GOLDEN_DIR, "ref")    # what the unmodified reference returned for the tests that compare with it directly
 VERT_TOL = 1e-4     # metres: BASELINE.json north_star tolerance for curb-polyline vertices
+MARKER_EPS = (0.05, 0.7, 3.0)                 # poly_s_param values of the marker-tail comparison (tests/test_markers.py)
+
+
+def digest(a) -> str:
+    """sha256 of an int32 array: stands in for reference outputs too large to store."""
+    return hashlib.sha256(np.ascontiguousarray(a, np.int32).tobytes()).hexdigest()
+
+
+def cloud_digest(pts) -> str:
+    return hashlib.sha256(np.ascontiguousarray(pts, np.float32).tobytes()).hexdigest()
+
+
+def random_param_case(seed: int):
+    """Seeded random draw over the LidarFilters.cfg parameter ranges (cfg/LidarFilters.cfg:10-84) and its cloud."""
+    rng = np.random.default_rng(100 + seed)
+    pts = make_scan("C1", 10 + seed, order=("column", "ring")[seed % 2]) if seed % 3 else random_cloud(6000, seed, rings=12)
+    prm = make_params(
+        x_zero_method=int(rng.integers(0, 2)), z_zero_method=int(rng.integers(0, 2)), star_shaped_method=int(rng.integers(0, 2)),
+        blind_spots=int(rng.integers(0, 2)), xDirection=int(rng.integers(0, 3)), interval=float(rng.uniform(0.05, 0.5)),
+        curb_height=float(rng.uniform(0.01, 0.2)), curb_points=int(rng.integers(1, 12)), beamZone=float(rng.uniform(10, 100)),
+        cylinder_deg_x=float(rng.uniform(90, 180)), cylinder_deg_z=float(rng.uniform(90, 180)),
+        curb_slope_deg=float(rng.uniform(10, 90)), kdev_param=float(rng.uniform(0.5, 5)), kdist_param=float(rng.uniform(0.4, 10)),
+        starbeam_filter=int(rng.integers(0, 2)), dmin_param=int(rng.integers(3, 30)),
+        **(FULL_ROI if seed % 2 else dict(min_x=-20.0, max_x=40.0, min_y=-15.0, max_y=15.0, min_z=-3.0, max_z=1.0)))
+    return pts, prm
 
 
 _SCAN_CACHE: dict = {}

@@ -1,4 +1,4 @@
-"""Builds liburf_b200.so (nvcc, sm_100a) in-tree. nvcc cross-compiles without a GPU, so this runs on the CPU box too."""
+"""Builds liburf_b200.so (nvcc, sm_90a: H100) in-tree. nvcc cross-compiles without a GPU, so this runs on the CPU box too."""
 from __future__ import annotations
 
 import os
@@ -10,7 +10,7 @@ ROOT = os.path.dirname(PKG)
 CSRC = os.path.join(PKG, "csrc")
 LIB = os.path.join(PKG, "liburf_b200.so")
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-fmad=false",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-fmad=false",
               "-Xcompiler", "-fPIC"]
 SOURCES = ["urf_api.cu"]
 HOST_SOURCES = ["urf_markers.cpp", "urf_queue.cpp", "urf_mq.cpp"]
@@ -49,12 +49,12 @@ def build_lib(force: bool = False, verbose: bool = False) -> str:
         o = os.path.join(bdir, s + ".o")
         subprocess.run(["g++", "-std=c++17", "-O2", "-fPIC", "-pthread", "-c", os.path.join(CSRC, s), "-o", o], check=True)
         objs.append(o)
-    subprocess.run([_nvcc(), "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", LIB, *objs], check=True)
+    subprocess.run([_nvcc(), "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", LIB, *objs], check=True)
     return LIB
 
 
 def build_oracle() -> None:
-    """Test infrastructure: the CPU restatement always; the unmodified reference only where /root/reference exists."""
+    """Test infrastructure: the CPU restatement always; the unmodified reference only where its sources exist (oracle/Makefile REF)."""
     subprocess.run(["make", "-C", os.path.join(ROOT, "oracle"), "port"], check=True, stdout=subprocess.DEVNULL)
     subprocess.run(["make", "-C", os.path.join(ROOT, "oracle"), "ref"], check=True, stdout=subprocess.DEVNULL)
 

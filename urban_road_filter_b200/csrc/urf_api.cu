@@ -28,10 +28,10 @@ struct urf_ctx {
   // k_scatter and k_tab1: with `inner_fork` the ring detector runs on a side stream of the pipeline's stream (tuning option 11)
   cudaStream_t s_side[kGroups + 1] = {};
   cudaEvent_t ev_sfork[kGroups + 1] = {}, ev_sjoin[kGroups + 1] = {};
-  bool inner_fork = true;              // measured at C2 x 128: 1.240 -> 1.233 ms on two streams, 1.282 -> 1.263 on one
+  bool inner_fork = true;              // H100 (400 W), C2 x 128: 1.95 / 2.06 ms per step with, 2.11 / 1.99 without (within noise)
   int sort_variant = 16;               // widest single-warp network of k_star_sort_warp in elements per lane: 16 (64 registers, 32 warps/SM)
-                                       // or 32 (128 registers, 16 warps/SM; measured 2 % slower per step at C2 x 128) (tuning option 12)
-  int groups = 2;                                 // measured at C2 x 128: 1 stream 1.37 ms, 2 streams 1.31, 4 streams 1.34, 8 streams 1.40
+                                       // or 32 (128 registers, 16 warps/SM; H100, C2 x 128: 1.87 / 1.98 ms, within noise) (tuning option 12)
+  int groups = 2;                                 // H100 (400 W), C2 x 128, two runs: 1 stream 1.99 / 2.00 ms, 2 streams 1.95 / 2.06, 4 streams 2.11 / 2.02, 8 streams 2.07 / 2.14
   // device-resident batches as many small sub-batches: `sub` scans per sub-batch (0 = one sub-batch per stream), dealt
   // round-robin to the `groups` streams, the whole fork/join captured once as a CUDA graph (bgraph) and replayed; with
   // `slot_reuse` the sub-batches of a stream share one workspace slot (working set = groups * sub scans, L2-resident)
@@ -683,8 +683,8 @@ int process_batch_impl(urf_ctx* ctx, const void* const* data, const int* n, int 
   bufv.label8 = want_l8 ? ctx->label8 : nullptr;
   // Software pipeline over chunks of scans: H2D of chunk c+1 (s_in), kernels of chunk c (stream) and D2H of chunk c-1
   // (s_out) overlap; scans are independent, every chunk owns its slice of every buffer.
-  // Chunks of batch / 16 scans. (Measured and dropped: smaller chunks at both ends of the call — a shorter pipeline fill and
-  // drain on paper, 5 % slower in practice — and copies running only three chunks ahead of the launches.)
+  // Chunks of batch / 16 scans. (Tried and dropped: smaller chunks at both ends of the call — a shorter pipeline fill and
+  // drain on paper, slower in practice — and copies running only three chunks ahead of the launches.)
   std::vector<int> cb;                                        // chunk c = scans [cb[c], cb[c + 1])
   {
     const int chunk = batch >= 16 ? std::max(4, (batch + 15) / 16) : batch;

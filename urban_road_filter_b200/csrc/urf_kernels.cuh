@@ -1,4 +1,4 @@
-// urf_kernels.cuh — sm_100a kernels of the per-scan road/curb classification path (pipeline v2).
+// urf_kernels.cuh — sm_90a kernels of the per-scan road/curb classification path (pipeline v2).
 //
 // Every kernel takes the batch index from blockIdx.y (or blockIdx.x for one-CTA-per-scan kernels): a launch covers a
 // whole batch of scans laid out back to back with `S` points of stride. Everything that decides a label is computed by
@@ -1110,8 +1110,8 @@ __global__ void __launch_bounds__(kScanWarps * 32) k_star_scan(DevBuffers buf, D
   for (int o = 16; o > 0; o >>= 1) nmax = max(nmax, __shfl_xor_sync(0xffffffffu, nmax, o));
   for (int t0 = 0; t0 < nmax; t0 += 32) {
     // stage tile [t0, t0 + 32) of all 32 sector rows: 8 rows at a time so that the 16 loads of a group are in flight
-    // together (one L2 round trip per group instead of one per row). (Measured and dropped: 16 rows at a time with 8-byte
-    // loads and the predecessor taken from the left neighbour by shuffle — 0.102 instead of 0.068 ms at C2 x 128.)
+    // together (one L2 round trip per group instead of one per row). (Tried and dropped as slower: 16 rows at a time with
+    // 8-byte loads and the predecessor taken from the left neighbour by shuffle.)
     for (int q0 = 0; q0 < 32; q0 += 8) {
       float4 p[8], pp[8];
       bool ok[8];
@@ -1417,8 +1417,8 @@ __global__ void __launch_bounds__(256, MINB) k_ring_detect4(DevBuffers buf, DevP
 
 // ---------------------------------------------------------------------------------------------------------------------
 // blindSpots as tables (urf_logic.cuh: CurbView, window_blocked, build_T_row, covered_T). Three short kernels — a cluster
-// of eight CTAs per scan running the three phases behind cluster barriers was measured at 111 us against 71 us for the
-// three launches (C2 x 128: the 722 window tests of a scan want more than eight CTAs' worth of warps at once).
+// of eight CTAs per scan running the three phases behind cluster barriers was tried and was slower than the three
+// launches (C2 x 128: the 722 window tests of a scan want more than eight CTAs' worth of warps at once).
 // k_tab1: per scan — prefix counts of non-empty curb bins per ring, maxDistance / arc widths, q1..q4, reach := n_rings.
 __global__ void __launch_bounds__(256) k_tab1(DevBuffers buf, DevParams prm) {
   const int b = blockIdx.y;

@@ -1,5 +1,5 @@
 // urf_mq.cpp — ONE ingest stream over SEVERAL GPUs (include/urf.h urf_mq, BASELINE config 4: a continuous scan stream
-// sharded across the B200s of one box). Host code only.
+// sharded across the GPUs of one box). Host code only.
 //
 // The reference is a single subscriber with queue depth 1 (`nh->subscribe(params::topicName, 1, &Detector::filtered, this)`,
 // lidar_segmentation.cpp:53); the demo graph feeds four LiDAR topics (config/demo1.rviz:91,121,151,181). urf_mq keeps one
