@@ -9,7 +9,7 @@ from urban_road_filter_b200 import build
 src = os.path.join(build.CSRC, "urf_api.cu")
 out = subprocess.run([build._nvcc(), *build.NVCC_FLAGS, "-Xptxas=-v", "-c", src, "-o", "/tmp/urf_api_ptxas.o"], capture_output=True, text=True).stderr
 rows = []
-for m in re.finditer(r"Compiling entry function '(\S+)' for 'sm_100a'\n.*?\n\s+(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads\nptxas info\s+: Used (\d+) registers(?:, used (\d+) barriers)?(?:, (\d+) bytes cumulative stack size)?(?:, (\d+) bytes smem)?", out):
+for m in re.finditer(r"Compiling entry function '(\S+)' for 'sm_90a'\n.*?\n\s+(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads\nptxas info\s+: Used (\d+) registers(?:, used (\d+) barriers)?(?:, (\d+) bytes cumulative stack size)?(?:, (\d+) bytes smem)?", out):
     name = subprocess.run(["c++filt", m.group(1)], capture_output=True, text=True).stdout.strip().split("(")[0].replace("urf::", "")
     rows.append((name, int(m.group(5)), int(m.group(2)), int(m.group(3)), int(m.group(4)), int(m.group(8) or 0)))
 sass = subprocess.run(["cuobjdump", "-sass", build.LIB], capture_output=True, text=True).stdout

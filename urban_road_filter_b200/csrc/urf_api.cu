@@ -29,8 +29,7 @@ struct urf_ctx {
   cudaStream_t s_side[kGroups + 1] = {};
   cudaEvent_t ev_sfork[kGroups + 1] = {}, ev_sjoin[kGroups + 1] = {};
   bool inner_fork = true;              // H100 (400 W), C2 x 128: 1.95 / 2.06 ms per step with, 2.11 / 1.99 without (within noise)
-  int sort_variant = 16;               // widest single-warp network of k_star_sort_warp in elements per lane: 16 (64 registers, 32 warps/SM)
-                                       // or 32 (128 registers, 16 warps/SM; H100, C2 x 128: 1.87 / 1.98 ms, within noise) (tuning option 12)
+  int sort_ctas = 0;                   // resident CTAs of k_star_sort on the whole device (its grid: the warps walk the sectors)
   int groups = 2;                                 // H100 (400 W), C2 x 128, two runs: 1 stream 1.99 / 2.00 ms, 2 streams 1.95 / 2.06, 4 streams 2.11 / 2.02, 8 streams 2.07 / 2.14
   // device-resident batches as many small sub-batches: `sub` scans per sub-batch (0 = one sub-batch per stream), dealt
   // round-robin to the `groups` streams, the whole fork/join captured once as a CUDA graph (bgraph) and replayed; with
@@ -196,8 +195,12 @@ int launch_pipeline(urf_ctx* ctx, const DevBuffers& buf, int B, int S, bool want
   if (dp.star) {
     const int gbig = std::max(4, std::min(kSectKeys, 2048 / B));
     const dim3 gscan((kSectKeys + kScanWarps * 32 - 1) / (kScanWarps * 32), B);
-    if (ctx->sort_variant == 16) K("k_star_sort_warp", k_star_sort_warp<16><<<dim3(kSectKeys, B), 32, 0, st>>>(buf, dp, S));
-    else K("k_star_sort_warp", k_star_sort_warp<32><<<dim3(kSectKeys, B), 32, 0, st>>>(buf, dp, S));
+    // as many CTAs as can be resident at once, the sectors dealt out by a static stride: the sectors of a launch are of
+    // similar size (every scan of a batch comes from one sensor), so the shares are even; a work counter would cost one
+    // same-address atomic per sector (46 k per C2 launch). A CTA that starts late because the other stream or the ring
+    // detector holds SMs finishes its share late; the two-stream step times in DESIGN.md §6 include that.
+    const int gsort = std::min(ctx->sort_ctas, (B * kSectKeys + kSortWarps - 1) / kSortWarps);
+    K("k_star_sort", k_star_sort<<<gsort, kSortWarps * 32, kStarSortSmem, st>>>(buf, dp, S, B));
     K("k_star_sort_big", k_star_sort_big<<<dim3(gbig, B), 256, kStarCtaSmem, st>>>(buf, dp, S));
     K("k_star_scan", k_star_scan<<<gscan, kScanWarps * 32, 0, st>>>(buf, dp, S));
     if (dp.star_prefix)            // sectors whose edge search ran off the near-first prefix: full sort, search resumed
@@ -391,6 +394,13 @@ int urf_create(urf_ctx** out, int device, int max_points, int max_batch) {
     CKF(cudaMemcpyToSymbol(c_beam_yx, byx, sizeof(byx)));
     ctx->dp.Kfi = Kfi;
   }
+  CKF(cudaFuncSetAttribute(k_star_sort, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kStarSortSmem));
+  {
+    int sms = 0, per_sm = 0;
+    CKF(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ctx->device));
+    CKF(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_star_sort, kSortWarps * 32, kStarSortSmem));
+    ctx->sort_ctas = std::max(1, sms * per_sm);
+  }
   CKF(cudaFuncSetAttribute(k_star_sort_big, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kStarCtaSmem));
   CKF(cudaFuncSetAttribute(k_star_refine, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kStarCtaSmem));
   CKF(cudaFuncSetAttribute(k_sort_rings, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kRingSmemKeys * sizeof(unsigned long long))));
@@ -464,8 +474,8 @@ int urf_get_params(const urf_ctx* ctx, urf_params* p) {
 // 4 = near-first star sort (0/1, default 1); 5 = scans per sub-batch of a device-resident batch (0 = batch / streams);
 // 6 = replay the fork/join of a device-resident batch as one CUDA graph (0/1); 7 = sub-batches of a stream share one
 // workspace slot (0/1); 8 = ring detector variant; 9 = marker search variant; 10 = near-first pivot rank (3..28 of 32 samples);
-// 11 = ring detector on a side stream next to the star-shaped search (0/1, default 1); 12 = widest single-warp star sort
-// network in elements per lane (16 default, or 32)
+// 11 = ring detector on a side stream next to the star-shaped search (0/1, default 1); 12 = accepted and ignored (it chose
+// the widest single-warp star sort network; k_star_sort has one, 16 elements per lane, and wider sorts go to k_star_sort_big)
 int urf_set_option(urf_ctx* ctx, int option, int value) {
   if (!ctx) return URF_ERR_INVALID;
   CK(cudaSetDevice(ctx->device));
@@ -479,7 +489,7 @@ int urf_set_option(urf_ctx* ctx, int option, int value) {
   if (option == 7) { ctx->slot_reuse = value != 0; return URF_OK; }
   if (option == 8) { ctx->rd_variant = value; return URF_OK; }
   if (option == 9) { ctx->markers_variant = value; return URF_OK; }
-  if (option == 12) { ctx->sort_variant = value == 16 ? 16 : 32; return URF_OK; }
+  if (option == 12) return URF_OK;
   if (option == 11) { ctx->inner_fork = value != 0; return URF_OK; }
   if (option == 10) { ctx->dp.star_pivot = value < 3 ? 3 : (value > 28 ? 28 : value); return URF_OK; }
   if (option == 1) {                   // value = number of event slots (0 = off)
@@ -859,7 +869,8 @@ int urf_test_math(int device, int which, const float* a, const float* b, float* 
 
 // Copy a device-side intermediate of scan `b` of the last call into host memory (stage-level differential tests).
 //   what: 0 alpha_v[f32,n]  1 mark[u8,n] (all detectors)  2 ringid[i16,n]  3 sect[i16,n]  4 az[f32,n]  5 d2[f32,n]
-//         (4, 5: defined for ROI points only)  8 ScanTab (raw)
+//         (4, 5: defined for ROI points only)  8 ScanTab (raw)  9 star sort work lists [i32,2]: sectors handed to the
+//         eight-warp sort (nbig) and to the exact fallback (nslow)
 int urf_debug_fetch(urf_ctx* ctx, int b, int what, void* dst, size_t bytes) {
   if (!ctx || !dst || b < 0 || b >= ctx->last_B) return URF_ERR_INVALID;
   CK(cudaSetDevice(ctx->device));
@@ -874,6 +885,7 @@ int urf_debug_fetch(urf_ctx* ctx, int b, int what, void* dst, size_t bytes) {
     case 4: src = ctx->buf.az + off; break;
     case 5: src = ctx->buf.d2 + off; break;
     case 8: src = ctx->buf.tab + b; if (bytes > sizeof(ScanTab)) bytes = sizeof(ScanTab); break;
+    case 9: src = &ctx->buf.tab[b].nbig; if (bytes > 2 * sizeof(int)) bytes = 2 * sizeof(int); break;
     default: return URF_ERR_INVALID;
   }
   CK(cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost));

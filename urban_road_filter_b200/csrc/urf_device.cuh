@@ -75,7 +75,7 @@ struct ScanTab {
   unsigned long long cutbest[kDegBins];              // min (ring, azimuth bits, input index) over the bin's non-road points
   unsigned dmax[kDegBins];         // large scans (k_markers_grid): float bits of the farthest candidate road point
   unsigned long long best[kDegBins];                 // large scans: (ring, azimuth bits, input index) of the first candidate reaching dmax
-  // near-first star sort (k_star_sort_warp): only the points below a sampled pivot radius are sorted at first
+  // near-first star sort (k_star_sort): only the points below a sampled pivot radius are sorted at first
   int sorted_len[kSectKeys];       // length of the radius-sorted prefix of the sector in `ssorted` (== size when fully sorted)
   int nrefine, pad_;               // sectors whose edge search ran off the sorted prefix
   unsigned short refine[kSectKeys];

@@ -7,7 +7,7 @@
 //
 // Pipeline (DESIGN.md has the picture):
 //   k_reset -> k_points -> k_register -> k_assign -> k_scan_offsets (+ exact re-registration of refuted scans)
-//   -> k_scatter -> k_star_sort_warp (near-first) -> k_star_sort_big (large sectors, exact fallback) -> k_star_scan
+//   -> k_scatter -> k_star_sort (near-first) -> k_star_sort_big (large sectors, exact fallback) -> k_star_scan
 //   -> k_star_refine (sectors without an edge in their prefix: full sort, walk resumed)
 //   -> k_ring_detect -> k_tab1 -> k_reach -> k_tab2 -> k_label (input order) -> k_markers (cluster of 8 CTAs per scan)
 //   [-> k_sort_rings when the emission order is requested]
@@ -584,15 +584,17 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32) k_scatter(DevBuffers buf,
 // Register-resident bitonic network: thread t owns elements t*EPL .. t*EPL+EPL-1 (32-bit radius bits + the element's slot
 // in the unsorted sector as payload). Strides below EPL are register-only compare-exchanges, strides below 32*EPL go
 // through warp shuffles, larger strides (multi-warp CTAs only) exchange through shared memory. One warp sorts up to 1024
-// points (k_star_sort_warp, one 32-thread CTA per sector so that all control flow around the shuffles is provably
-// uniform), eight warps up to 8192 (k_star_sort_big / k_star_refine, work lists). Returns true when two points share a
+// points (k_star_sort: one sector per warp at a time, warp-uniform control flow around the shuffles; k_star_refine), eight
+// warps up to 8192 (k_star_sort_big / k_star_refine, work lists). Returns true when two points share a
 // radius: their order is what the reference's std::sort leaves (urf_stdsort.cuh), which the network does not see — such a
 // sector, like any sector beyond 8192 points, is redone by slow_sort_sector.
 constexpr int kWarpCap = 1024, kCtaCap = 8192;
 
-// LIST (single-warp only): the n elements to sort are given as (radius bits, slot in src) pairs in s_xk / s_xe instead of
-// being all of src[0 .. n) — the near-first prefix of k_star_sort_warp.
-template <int EPL, int WARPS, bool LIST = false>
+// LIST: the n elements to sort are given as (radius bits, slot in src) pairs in s_xk / s_xe instead of being all of
+// src[0 .. n) — the near-first prefix.
+// STAGED (k_star_sort: one warp, LIST, s_xk = the warp's key stage): s_xe == nullptr means that s_xk holds the radius bits
+// of all of src[0 .. n) in slot order; the records are gathered and stored through s_xk in sorted order (see below).
+template <int EPL, int WARPS, bool LIST = false, bool STAGED = false>
 __device__ __forceinline__ bool bitonic_sector(const float4* __restrict__ src, float4* __restrict__ dst, int n, int tid,
                                                unsigned* s_xk, unsigned* s_xe) {
   constexpr int THREADS = WARPS * 32;                // sorts up to THREADS * EPL elements
@@ -605,7 +607,7 @@ __device__ __forceinline__ bool bitonic_sector(const float4* __restrict__ src, f
     const int e = tid * EPL + r;
     key[r] = 0xffffffffu; el[r] = 0u;
     if (e < n) {
-      if (LIST) { key[r] = s_xk[e]; el[r] = s_xe[e]; }
+      if (LIST) { key[r] = s_xk[e]; el[r] = (STAGED && s_xe == nullptr) ? (unsigned)e : s_xe[e]; }
       else { key[r] = fbits(src[e].x); el[r] = (unsigned)e; }
     }
   }
@@ -669,13 +671,37 @@ __device__ __forceinline__ bool bitonic_sector(const float4* __restrict__ src, f
     if (lane == 0 && tid > 0) prev0 = s_xk[(tid >> 5) - 1];
   }
   bool tie = false;
+  if constexpr (STAGED) {
+    static_assert(!STAGED || (WARPS == 1 && LIST && EPL <= 16), "STAGED: single-warp list sorts of up to 16 elements per lane");
 #pragma unroll
-  for (int r = 0; r < EPL; r++) {
-    const int e = tid * EPL + r;
-    const unsigned prev = r > 0 ? key[r - 1] : prev0;
-    if (e < n) {
-      dst[e] = src[el[r]];
-      if (e > 0 && prev == key[r]) tie = true;
+    for (int r = 0; r < EPL; r++) {
+      const int e = tid * EPL + r;
+      const unsigned prev = r > 0 ? key[r - 1] : prev0;
+      if (e < n && e > 0 && prev == key[r]) tie = true;
+    }
+    // the list is in registers now: its buffer takes the slots in sorted order, so that consecutive lanes write consecutive
+    // records (a lane's own EPL records are EPL * 16 bytes apart in dst). Word r of lane t goes to t * EPL + (r ^ swz(t)):
+    // the XOR spreads the 32 lanes' words of one r over all 32 banks.
+    constexpr int TPW = 32 / EPL;                      // lanes per 32 consecutive elements
+    __syncwarp();
+#pragma unroll
+    for (int r = 0; r < EPL; r++) s_xk[tid * EPL + (r ^ ((tid / TPW) & (EPL - 1)))] = el[r];
+    __syncwarp();
+#pragma unroll
+    for (int r = 0; r < EPL; r++) {
+      const int e = r * 32 + tid, t = e / EPL;
+      if (e < n) dst[e] = src[s_xk[t * EPL + ((e & (EPL - 1)) ^ ((t / TPW) & (EPL - 1)))]];
+    }
+    __syncwarp();
+  } else {
+#pragma unroll
+    for (int r = 0; r < EPL; r++) {
+      const int e = tid * EPL + r;
+      const unsigned prev = r > 0 ? key[r - 1] : prev0;
+      if (e < n) {
+        dst[e] = src[el[r]];
+        if (e > 0 && prev == key[r]) tie = true;
+      }
     }
   }
   return tie;
@@ -689,31 +715,42 @@ __device__ __forceinline__ bool sort_sector_warp(const float4* __restrict__ src,
   return bitonic_sector<32, 1>(src, dst, n, lane, nullptr, nullptr);
 }
 
-// Near-first selection (see k_star_sort_warp): all radius loads of the sector are issued together, the pivot is the 18th
-// smallest of 32 evenly spaced samples, and the (radius bits, slot) pairs below the pivot are appended to the shared
-// lists in any order. Returns their number.
+// A near-first prefix of m of a sector's n points is worth sorting on its own (instead of the whole sector).
+__device__ __forceinline__ bool near_prefix(int m, int n) { return m >= 32 && 4 * m <= 3 * n; }
+
+// Near-first selection (see k_star_sort): the pivot is the 18th smallest of 32 evenly spaced samples of the sector's
+// radius bits kb[0 .. n); returns the number m of points below it. Only when that prefix is what k_star_sort will sort
+// (near_prefix(m, n) and m <= kNetCap) are its (radius bits, slot) pairs written, IN PLACE of the keys and in any order:
+// radius bits to kb[0 .. m), slots to kb[kNetCap .. kNetCap + m). Otherwise kb is left as it was (the whole sector is
+// sorted from it, or it goes to k_star_sort_big).
+constexpr int kNetCap = 512;                           // widest single-warp network of k_star_sort (16 elements per lane)
 template <int EPL>
-__device__ __forceinline__ int select_near(const float4* __restrict__ src, int n, int lane, unsigned* s_pk, unsigned* s_pe, int pivot_rank, int cap = kWarpCap) {
-  const unsigned mine = fbits(src[(int)(((unsigned)lane * (unsigned)n) >> 5)].x);
+__device__ __forceinline__ int select_near(unsigned* kb, int n, int lane, int pivot_rank) {
+  const unsigned mine = kb[(int)(((unsigned)lane * (unsigned)n) >> 5)];
   unsigned key[EPL];
 #pragma unroll
   for (int r = 0; r < EPL; r++) {
     const int e = r * 32 + lane;
-    key[r] = e < n ? fbits(src[e].x) : 0xffffffffu;
+    key[r] = e < n ? kb[e] : 0xffffffffu;
   }
   int rank = 0;                                        // ranks of the samples are a permutation (ties broken by lane)
 #pragma unroll
   for (int j = 0; j < 32; j++) { const unsigned o = __shfl_sync(0xffffffffu, mine, j); rank += (o < mine) || (o == mine && j < lane); }
   const unsigned pivot = __shfl_sync(0xffffffffu, mine, __ffs(__ballot_sync(0xffffffffu, rank == pivot_rank)) - 1);
+  int m = 0;                                           // padding keys are 0xffffffff: never below the pivot
+#pragma unroll
+  for (int r = 0; r < EPL; r++) m += __popc(__ballot_sync(0xffffffffu, key[r] < pivot));
+  if (!near_prefix(m, n) || m > kNetCap) return m;     // warp-uniform
+  __syncwarp();                                        // every lane holds its keys: the list may overwrite them
   const unsigned lt = (1u << lane) - 1u;
-  int m = 0;
+  int pos0 = 0;
 #pragma unroll
   for (int r = 0; r < EPL; r++) {
-    const bool sel = key[r] < pivot;                   // padding keys are 0xffffffff: never selected
+    const bool sel = key[r] < pivot;
     const unsigned bs = __ballot_sync(0xffffffffu, sel);
-    const int pos = m + __popc(bs & lt);
-    if (sel && pos < cap) { s_pk[pos] = key[r]; s_pe[pos] = (unsigned)(r * 32 + lane); }   // beyond cap: counted only
-    m += __popc(bs);
+    const int pos = pos0 + __popc(bs & lt);
+    if (sel) { kb[pos] = key[r]; kb[kNetCap + pos] = (unsigned)(r * 32 + lane); }
+    pos0 += __popc(bs);
   }
   __syncwarp();
   return m;
@@ -743,9 +780,6 @@ __device__ __forceinline__ int select_far(const float4* __restrict__ src, int n,
   return m;
 }
 
-// One 32-thread CTA per sector: sector index and size derive from blockIdx, so the compiler knows the control flow
-// around the shuffles is warp-uniform (no convergence barriers around every SHFL).
-//
 // Near-first sort. The edge search (k_star_scan) walks a sector outwards and stops at its first edge point, so the far
 // part of a sector is usually never looked at. Sectors above kPrefixMin points are therefore split at a pivot radius (the
 // 18th smallest of 32 evenly spaced samples): points below the pivot are compacted into shared memory and sorted (about
@@ -754,18 +788,21 @@ __device__ __forceinline__ int select_far(const float4* __restrict__ src, int n,
 // without an edge is put on tab.refine and redone in full (k_star_refine: full sort + star_resume_walk). Exact either
 // way: every point of the prefix is closer than every point behind it.
 constexpr int kPrefixMin = 128;
-// MAXEPL = 32: every sector of up to kWarpCap points is sorted here (128 registers, 16 warps per SM). MAXEPL = 16: sorts
-// of more than 512 elements go to k_star_sort_big's list instead, which leaves this kernel with the networks of up to 16
-// elements per lane (fewer registers, more resident warps to hide the shuffle latency). (Measured and dropped: a keys-only
-// network — one SHFL + two VIMNMX per remote compare-exchange instead of two SHFL, a compare and two selects — with the
-// payload recovered by a binary search of every key in the sorted keys: 30 % fewer instructions, but 0.7 % slower per step.)
-template <int MAXEPL>
-__global__ void __launch_bounds__(32, MAXEPL >= 32 ? 16 : 32) k_star_sort_warp(DevBuffers buf, DevParams prm, int S) {
-  constexpr int kList = 32 * MAXEPL;                                    // longest list this kernel sorts itself
-  __shared__ unsigned s_pk[kList], s_pe[kList];
-  const int b = blockIdx.y, s = blockIdx.x, lane = threadIdx.x;
+
+// 4-byte asynchronous global -> shared copies (cp.async): the copy needs no register, and the warp goes on working while
+// it is in flight
+__device__ __forceinline__ void cp_async4(unsigned* s, const float* g) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;\n" ::"r"((unsigned)__cvta_generic_to_shared(s)), "l"(g) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N) : "memory"); }
+
+// One sector of k_star_sort, by one warp; kb[0 .. n) holds its radius bits (slot order). Sectors of more than kWarpCap
+// points, and sorts wider than kNetCap elements, go to k_star_sort_big's lists; equal radii to the exact fallback.
+__device__ __forceinline__ void star_sort_sector(const DevBuffers& buf, const DevParams& prm, int S, int b, int s, int base, int n,
+                                                 unsigned* kb, int lane) {
   ScanTab& tab = buf.tab[b];
-  const int base = tab.sect_start[s], n = tab.sect_start[s + 1] - base;
   if (lane == 0) tab.sorted_len[s] = n;
   if (n <= 0) return;
   const float4* src = buf.spt + (size_t)b * S + base;
@@ -778,31 +815,76 @@ __global__ void __launch_bounds__(32, MAXEPL >= 32 ? 16 : 32) k_star_sort_warp(D
     }
     return;
   }
-  bool tie;
   int m = 0;
   if (prm.star_prefix && n > kPrefixMin) {
-    if (n <= 256) m = select_near<8>(src, n, lane, s_pk, s_pe, prm.star_pivot, kList);
-    else if (n <= 512) m = select_near<16>(src, n, lane, s_pk, s_pe, prm.star_pivot, kList);
-    else m = select_near<32>(src, n, lane, s_pk, s_pe, prm.star_pivot, kList);
+    if (n <= 256) m = select_near<8>(kb, n, lane, prm.star_pivot);
+    else if (n <= 512) m = select_near<16>(kb, n, lane, prm.star_pivot);
+    else m = select_near<32>(kb, n, lane, prm.star_pivot);
   }
-  const bool near = m >= 32 && 4 * m <= 3 * n;                          // worth it: sort the near part only
-  if (MAXEPL < 32 && (near ? m : n) > 32 * MAXEPL) {                    // a wide network: eight warps do it (k_star_sort_big)
+  const bool near = near_prefix(m, n);                                  // worth it: sort the near part only
+  const int len = near ? m : n;
+  if (len > kNetCap) {                                                  // a wide network: eight warps do it (k_star_sort_big)
     if (lane == 0) tab.biglist[atomicAdd(&tab.nbig, 1)] = (unsigned short)s;
     return;
   }
-  if (near) {
-    if (m <= 128) tie = bitonic_sector<4, 1, true>(src, dst, m, lane, s_pk, s_pe);
-    else if (m <= 256) tie = bitonic_sector<8, 1, true>(src, dst, m, lane, s_pk, s_pe);
-    else if (MAXEPL >= 32 && m > 512) tie = bitonic_sector<32, 1, true>(src, dst, m, lane, s_pk, s_pe);
-    else tie = bitonic_sector<16, 1, true>(src, dst, m, lane, s_pk, s_pe);
-    if (lane == 0) tab.sorted_len[s] = m;
-  } else {
-    if (n <= 128) tie = bitonic_sector<4, 1>(src, dst, n, lane, nullptr, nullptr);
-    else if (n <= 256) tie = bitonic_sector<8, 1>(src, dst, n, lane, nullptr, nullptr);
-    else if (MAXEPL >= 32 && n > 512) tie = bitonic_sector<32, 1>(src, dst, n, lane, nullptr, nullptr);
-    else tie = bitonic_sector<16, 1>(src, dst, n, lane, nullptr, nullptr);
-  }
+  unsigned* pe = near ? kb + kNetCap : nullptr;                         // whole sector: the keys in kb are in slot order
+  bool tie;
+  if (len <= 128) tie = bitonic_sector<4, 1, true, true>(src, dst, len, lane, kb, pe);
+  else if (len <= 256) tie = bitonic_sector<8, 1, true, true>(src, dst, len, lane, kb, pe);
+  else tie = bitonic_sector<16, 1, true, true>(src, dst, len, lane, kb, pe);
+  if (near && lane == 0) tab.sorted_len[s] = m;
   if (__any_sync(0xffffffffu, tie) && lane == 0) tab.slowlist[atomicAdd(&tab.nslow, 1)] = (unsigned short)s;   // sets F_TIE_SECTOR there
+}
+
+// k_star_sort: the radius sort of the sectors of a batch. Every warp walks the flat (scan, sector) index q = warp,
+// warp + W, ... (W = warps in the grid; the loop counter is warp-uniform, so the shuffle network needs no convergence
+// barriers) and keeps the next sector's memory traffic in flight while it sorts the current one: the radius bits of the
+// next sector are copied into the warp's other shared-memory stage with cp.async (4 bytes of every 16-byte spt record;
+// the records' lines are then in L2 for the gather of the sorted prefix), and the offsets of the sector after that are
+// loaded into registers. A one-warp CTA per sector (the previous form) exposed the offset load, the key loads and the
+// record gather one after the other on every sector, with at most 32 warps per SM (the resident-CTA limit) to cover them.
+// (Measured and dropped before: a keys-only network — one SHFL + two VIMNMX per remote compare-exchange instead of two
+// SHFL, a compare and two selects — with the payload recovered by a binary search of every key in the sorted keys: 30 %
+// fewer instructions, but 0.7 % slower per step.)
+constexpr int kSortWarps = 8;                                                              // warps per CTA
+constexpr size_t kStarSortSmem = (size_t)kSortWarps * 2 * kWarpCap * sizeof(unsigned);    // 64 KB: two key stages per warp
+__global__ void __launch_bounds__(kSortWarps * 32, 3) k_star_sort(DevBuffers buf, DevParams prm, int S, int B) {
+  extern __shared__ unsigned s_dyn[];
+  const int lane = lane_id(), warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0);
+  unsigned* const stage = s_dyn + (size_t)warp * 2 * kWarpCap;
+  const int Q = B * kSectKeys, W = gridDim.x * kSortWarps;
+  // (base, size) of sector q: lanes 0 and 1 load the two offsets, the shuffles hand them to the warp
+  auto offsets = [&](int q, int& base, int& n) {
+    int v = 0;
+    if (q < Q && lane < 2) { const int b = q / kSectKeys; v = buf.tab[b].sect_start[q - b * kSectKeys + lane]; }
+    base = __shfl_sync(0xffffffffu, v, 0);
+    n = __shfl_sync(0xffffffffu, v, 1) - base;
+  };
+  // radius bits of sector q into stage kb (one commit group per call, empty when there is nothing to stage)
+  auto stage_keys = [&](int q, int base, int n, unsigned* kb) {
+    if (q < Q && n > 1 && n <= kWarpCap) {
+      const float4* src = buf.spt + (size_t)(q / kSectKeys) * S + base;
+      for (int e = lane; e < n; e += 32) cp_async4(kb + e, &src[e].x);
+    }
+    cp_async_commit();
+  };
+  int q = blockIdx.x * kSortWarps + warp;
+  int base, n, nbase, nn;
+  offsets(q, base, n);
+  stage_keys(q, base, n, stage);
+  offsets(q + W, nbase, nn);
+  for (int it = 0; q < Q; q += W, it ^= 1) {
+    stage_keys(q + W, nbase, nn, stage + (it ^ 1) * kWarpCap);          // that stage's last reader finished (__syncwarp below)
+    int base2, n2;
+    offsets(q + 2 * W, base2, n2);
+    cp_async_wait<1>();                                                 // this lane's copies of sector q have landed ...
+    __syncwarp();                                                       // ... and every other lane's
+    const int b = q / kSectKeys;
+    star_sort_sector(buf, prm, S, b, q - b * kSectKeys, base, n, stage + it * kWarpCap, lane);
+    __syncwarp();
+    base = nbase; n = nn; nbase = base2; nn = n2;
+  }
+  cp_async_wait<0>();
 }
 
 // Exact fallback sort of one sector by all threads of the CTA (bitonic; shared memory up to `cap` keys, global scratch
@@ -841,7 +923,7 @@ __device__ void slow_sort_sector(const DevBuffers& buf, int b, int S, int base, 
   __syncthreads();
 }
 
-// Near-first selection for the eight-warp sort (see k_star_sort_warp): pivot = the 144th smallest of 256 evenly spaced
+// Near-first selection for the eight-warp sort (see k_star_sort): pivot = the 144th smallest of 256 evenly spaced
 // samples (56 %), the (radius bits, slot) pairs below it appended to the shared lists in any order. Returns their number.
 template <int EPL>
 __device__ __forceinline__ int select_near_cta(const float4* __restrict__ src, int n, int tid, unsigned* s_pk, unsigned* s_pe, unsigned* s_misc, int pivot_rank) {
@@ -885,7 +967,7 @@ __device__ __forceinline__ bool sort_sector_cta(const float4* __restrict__ src, 
   return bitonic_sector<32, 8, LIST>(src, dst, n, tid, s_xk, s_xe);
 }
 
-// k_star_sort_big: the sectors k_star_sort_warp handed over. tab.biglist (1025 .. kCtaCap points): eight-warp register
+// k_star_sort_big: the sectors k_star_sort handed over. tab.biglist (1025 .. kCtaCap points): eight-warp register
 // network, near-first like the single-warp sort (only the points below a sampled pivot radius are sorted, sorted_len tells
 // k_star_scan how far it may walk), redone at once in full by the exact fallback when it meets equal radii; tab.slowlist
 // (larger sectors, and sectors in which the single-warp sort met equal radii): exact fallback, whole sector.
