@@ -166,7 +166,7 @@ int launch_pipeline(urf_ctx* ctx, const DevBuffers& buf, int B, int S, bool want
   K("k_register", k_register<<<B, 256, 0, st>>>(buf, dp, S));
   K("k_assign", k_assign<<<gchunk, kWarpsPerBlock * 32, 0, st>>>(buf, dp, S, T));
   K("k_scan_offsets", k_scan_offsets<<<B, 1024, 0, st>>>(buf, dp, S, T));   // + exact re-registration of refuted scans
-  K("k_scatter", k_scatter<<<gchunk, kWarpsPerBlock * 32, 0, st>>>(buf, dp, S, T));   // 64 registers, 4 CTAs/SM (48 / 40 registers spill: measured slower)
+  K("k_scatter", k_scatter<<<dim3((T + kScatterWarps - 1) / kScatterWarps, B), kScatterWarps * 32, kScatterSmem, st>>>(buf, dp, S, T));
   // the ring detector next to the star-shaped search: both only read what k_scatter left and add curb hits (idempotent
   // marks, atomic min / max aggregates); k_tab1 is the first reader of the aggregates
   const bool fork = ctx->inner_fork && dp.star && !ctx->profile;
@@ -210,7 +210,7 @@ int launch_pipeline(urf_ctx* ctx, const DevBuffers& buf, int B, int S, bool want
   K("k_tab1", k_tab1<<<dim3((dp.channels + 7) / 8, B), 256, 0, st>>>(buf, dp));
   K("k_reach", k_reach<<<dim3((2 * kDegBins + 7) / 8, B), 256, 0, st>>>(buf, dp));
   K("k_tab2", k_tab2<<<dim3((dp.channels + kTab2Rings - 1) / kTab2Rings, B), kTab2Rings * 64, 0, st>>>(buf, dp));
-  K("k_label", k_label<<<gpts, 256, 0, st>>>(buf, dp, S));
+  K("k_label", k_label<<<dim3((S + kLabelThreads * kLabelGroups - 1) / (kLabelThreads * kLabelGroups), B), kLabelThreads, 0, st>>>(buf, dp, S));
   if (ctx->markers_variant == 2 || (ctx->markers_variant == 1 && S > kMarkSingleMax)) {   // large scans: a grid of CTAs per scan, three launches
     const dim3 gm(std::max(1, std::min(64, S / 16384)), B);
     K("k_markers_grid1", k_markers_grid<1><<<gm, kMarkGridThreads, 0, st>>>(buf, S));
@@ -403,6 +403,8 @@ int urf_create(urf_ctx** out, int device, int max_points, int max_batch) {
   }
   CKF(cudaFuncSetAttribute(k_star_sort_big, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kStarCtaSmem));
   CKF(cudaFuncSetAttribute(k_star_refine, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kStarCtaSmem));
+  CKF(cudaFuncSetAttribute(k_scatter, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kScatterSmem));
+  CKF(cudaFuncSetAttribute(k_scatter, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));   // four CTAs per SM
   CKF(cudaFuncSetAttribute(k_sort_rings, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kRingSmemKeys * sizeof(unsigned long long))));
   urf_default_params(&ctx->params);
   const char* fe = std::getenv("URF_FORCE_EXACT_REGISTRATION");
