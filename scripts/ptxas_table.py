@@ -1,8 +1,7 @@
 #!/usr/bin/env python
-"""Registers / spills / shared memory per kernel (ptxas -v) and the Blackwell/Hopper-class SASS mnemonics each kernel
-contains (cluster barriers UCGABAR_*, distributed-shared-memory mapping, warp REDUX, MATCH, 64-bit shared atomics, bulk
-asynchronous copies UBLKCP and the mbarrier operations SYNCS they complete on). The SASS is read from the object file the
-script compiles, so the table needs no prior build of the library.
+"""Registers / spills / shared memory per kernel (ptxas -v) and the Hopper-class SASS mnemonics each kernel contains (warp
+REDUX, MATCH, 64-bit shared atomics, bulk asynchronous copies UBLKCP and the mbarrier operations SYNCS they complete on).
+The SASS is read from the object file the script compiles, so the table needs no prior build of the library.
 usage: python scripts/ptxas_table.py > ptxas_sass.txt   (no GPU needed: nvcc cross-compiles)"""
 import os, re, subprocess, sys, collections, tempfile
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -26,7 +25,7 @@ for line in sass.splitlines():
     m = re.match(r"\s+/\*[0-9a-f]+\*/\s+(?:@!?U?P\d+\s+)?([A-Z0-9_.]+)", line)
     if m and cur:
         op = m.group(1)
-        for tag in ("UCGABAR_ARV", "UCGABAR_WAIT", "REDUX", "MATCH", "ATOMS", "ATOM", "RED", "SHFL", "DSQRT", "MUFU.RSQ64H", "DFMA", "DMUL", "DADD", "LDL", "STL", "BAR.SYNC", "VOTE", "UBLKCP", "SYNCS"):
+        for tag in ("REDUX", "MATCH", "ATOMS", "ATOM", "RED", "SHFL", "DSQRT", "MUFU.RSQ64H", "DFMA", "DMUL", "DADD", "LDL", "STL", "BAR.SYNC", "VOTE", "UBLKCP", "SYNCS"):
             if op.startswith(tag):
                 per[cur][tag] += 1
                 break
@@ -37,7 +36,6 @@ for name, regs, stack, sst, sld, smem in sorted(rows):
     c = per.get(name, {})
     notes = ", ".join(f"{k} {v}" for k, v in sorted(c.items()) if k != "total" and k not in ("DFMA", "DMUL", "DADD") and v)
     print(f"{name:28s} {regs:4d} {stack:5d} {sst:8d} {sld:8d} {smem:7d} {c.get('total', 0):6d}  {notes}")
-print("\nUCGABAR_ARV / UCGABAR_WAIT = thread-block-cluster barrier (cluster.sync); ATOM on generic addresses in k_markers target the")
-print("shared memory of the cluster's first CTA (distributed shared memory, cluster.map_shared_rank); REDUX = warp-wide integer reduce;")
-print("MATCH = __match_any_sync; UBLKCP = cp.async.bulk (k_scatter stages each warp's 8 KB of input records with one), SYNCS = the")
-print("mbarrier init / expect-tx / wait it completes on. No tensor-core instructions: the path has no dense contraction.")
+print("\nREDUX = warp-wide integer reduce; MATCH = __match_any_sync; UBLKCP = cp.async.bulk (k_scatter stages each warp's")
+print("8 KB of input records with one), SYNCS = the mbarrier init / expect-tx / wait it completes on. No tensor-core")
+print("instructions: the path has no dense contraction.")

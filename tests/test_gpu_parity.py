@@ -522,13 +522,10 @@ def test_gpu_packed_clouds_match_oracle(det, port, shape, step, offs):
         assert r.label is None and (r.n_road, r.n_curb) == (len(exp["road"]), len(exp["curb"]))
 
 
-SORT_WIDTH_DEFAULT = 16
-
-
 @pytest.mark.parametrize("variant", ["scan", "flat", "half_flat"])
 @pytest.mark.parametrize("shape", ["C2", "C4"])
 def test_gpu_near_first_star_sort(det, port, shape, variant):
-    """k_star_sort_warp sorts only the points below a sampled pivot radius and k_star_scan redoes (tab.refine) the sectors
+    """k_star_sort sorts only the points below a sampled pivot radius and k_star_scan redoes (tab.refine) the sectors
     whose edge search runs off that prefix. A flat world has no edge at all (every sector is refined), a half-flat one
     mixes both paths; each must give the oracle's result, and the same result as whole-sector sorting (option 4 = 0)."""
     sh = SHAPES[shape]
@@ -544,14 +541,28 @@ def test_gpu_near_first_star_sort(det, port, shape, variant):
     if variant == "flat":
         assert int((np.asarray(o.star_mark) == 2).sum()) == 0
     res = {}
-    for mode, width in ((1, 16), (0, 16), (1, 32), (0, 32)):   # option 12: widest single-warp network (wider sorts: k_star_sort_big)
+    for mode in (1, 0):
         det.set_option(4, mode)
-        det.set_option(12, width)
         r = det.filtered(pts)
-        assert stage_diffs(o, GpuDebug(det, r, n), n) == [], f"star_prefix={mode} width={width}"
-        res[mode, width] = r
+        assert stage_diffs(o, GpuDebug(det, r, n), n) == [], f"star_prefix={mode}"
+        res[mode] = r
     det.set_option(4, 1)
-    det.set_option(12, SORT_WIDTH_DEFAULT)
-    for k in res:
-        np.testing.assert_array_equal(res[k].label, res[1, 32].label)
-        np.testing.assert_array_equal(res[k].vert, res[1, 32].vert)
+    np.testing.assert_array_equal(res[0].label, res[1].label)
+    np.testing.assert_array_equal(res[0].vert, res[1].vert)
+
+
+def test_gpu_retired_options_are_ignored(det):
+    """Options 5-9, 11 and 12 of urf_set_option once selected scheduling and kernel variants; they are accepted and change
+    nothing: same labels, emission order and vertices, byte for byte, and the same kernel launches as with no option set."""
+    pts = make_scan("C1", 3)
+    det.set_params(make_params(**FULL_ROI))
+    base = det.filtered(pts)
+    launches = det.last_launch_count()
+    for option, values in ((5, (1, 2)), (6, (1,)), (7, (1,)), (8, (4, 5, 6, 45)), (9, (0, 2)), (11, (0,)), (12, (32,))):
+        for v in values:
+            det.set_option(option, v)
+            r = det.filtered(pts)
+            assert r.label.tobytes() == base.label.tobytes(), (option, v)
+            assert r.order.tobytes() == base.order.tobytes(), (option, v)
+            assert r.vert.tobytes() == base.vert.tobytes(), (option, v)
+            assert det.last_launch_count() == launches, (option, v)

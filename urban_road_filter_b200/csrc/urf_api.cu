@@ -25,22 +25,12 @@ struct urf_ctx {
   cudaStream_t s_grp[kGroups] = {};               // independent, so their (short, partly latency-bound) kernels overlap
   cudaEvent_t ev_fork = nullptr, ev_join[kGroups] = {};
   // inside one pipeline the star-shaped search (four kernels) and the ring detector (one kernel) are independent between
-  // k_scatter and k_tab1: with `inner_fork` the ring detector runs on a side stream of the pipeline's stream (tuning option 11)
+  // k_scatter and k_tab1: the ring detector runs on a side stream of the pipeline's stream
+  // (H100 (400 W), C2 x 128: 1.95 / 2.06 ms per step with, 2.11 / 1.99 without (within noise))
   cudaStream_t s_side[kGroups + 1] = {};
   cudaEvent_t ev_sfork[kGroups + 1] = {}, ev_sjoin[kGroups + 1] = {};
-  bool inner_fork = true;              // H100 (400 W), C2 x 128: 1.95 / 2.06 ms per step with, 2.11 / 1.99 without (within noise)
   int sort_ctas = 0;                   // resident CTAs of k_star_sort on the whole device (its grid: the warps walk the sectors)
   int groups = 2;                                 // H100 (400 W), C2 x 128, two runs: 1 stream 1.99 / 2.00 ms, 2 streams 1.95 / 2.06, 4 streams 2.11 / 2.02, 8 streams 2.07 / 2.14
-  // device-resident batches as many small sub-batches: `sub` scans per sub-batch (0 = one sub-batch per stream), dealt
-  // round-robin to the `groups` streams, the whole fork/join captured once as a CUDA graph (bgraph) and replayed; with
-  // `slot_reuse` the sub-batches of a stream share one workspace slot (working set = groups * sub scans, L2-resident)
-  int sub = 0;
-  int markers_variant = 1;             // 0: cluster of eight CTAs per scan (k_markers), 1: one CTA per scan (k_markers1) (tuning option 9)
-  int rd_variant = 46;                 // 4 / 45 / 46: k_ring_detect4 (four positions per thread; default curb_points only) at 4 / 5 / 6 CTAs per SM;
-                                       // 8 / 6 / 5: k_ring_detect (one position per thread) (tuning option 8)
-  bool slot_reuse = false, batch_graph = false;
-  cudaGraphExec_t bexec = nullptr;
-  struct { int B = -1, S = -1, sub = -1, G = -1, order = -1; bool reuse = false; const void* in = nullptr; void* label = nullptr; void* orderp = nullptr; unsigned long long version = 0; int launches = 0; } bkey;
   // CUDA graph of the kernel sequence for small host-buffer batches (launch latency dominates there); re-captured when
   // the shape, the parameters or an option change
   bool use_graph = true;
@@ -115,25 +105,23 @@ __global__ void k_ring32(DevBuffers buf, int* dst, int S) {
   if (i < buf.n[b]) dst[(size_t)b * S + i] = max((int)buf.ringid[(size_t)b * S + i], -1);
 }
 
-// View of `buf` for a sub-batch: what belongs to a scan for good (input, labels, point count, results, emission order) is
-// advanced by b0 scans, the workspace arrays by w0 scans (S points of stride, T histogram rows per scan). w0 == b0 gives
-// every scan its own workspace; sub-batches that run one after the other on one stream may share a slot (w0 = slot * sub).
-DevBuffers slot_view(const DevBuffers& a, int b0, int w0, int S, int T, int channels) {
+// View of `buf` for the sub-batch that starts at scan b0: every per-scan array is advanced by b0 scans (S points of
+// stride, T histogram rows per scan), so each scan keeps its own slice of the input, the outputs and the workspace.
+DevBuffers offset_view(const DevBuffers& a, int b0, int S, int T, int channels) {
   DevBuffers v = a;
-  const size_t o = (size_t)b0 * S, w = (size_t)w0 * S;
+  const size_t o = (size_t)b0 * S;
   v.in += o; v.label += o; v.order += o; v.n += b0; v.out += b0;
   if (v.label8) v.label8 += o;
-  v.alpha_v += w; v.mark += w; v.ringid += w; v.sect += w; v.bpt += w; v.spt += w; v.ssorted += w;
-  v.az += w; v.d2 += w; v.baz += w; v.roadlist += w; v.roadcnt += (size_t)w0 * ((S + 31) >> 5); v.sortbuf += 2 * w;
-  v.Tf += (size_t)w0 * channels * kTStride; v.Tb += (size_t)w0 * channels * kTStride;
-  v.lut += (size_t)w0 * (kElevBins + 1); v.firstidx += (size_t)w0 * (kElevBins + 1);
-  v.hist += (size_t)w0 * T * kRingKeys;
-  v.cmin += (size_t)w0 * channels * kDegBins; v.cmax += (size_t)w0 * channels * kDegBins;
-  v.ne += (size_t)w0 * channels * (kDegBins + 1);
-  v.tab += w0;
+  v.alpha_v += o; v.mark += o; v.ringid += o; v.sect += o; v.bpt += o; v.spt += o; v.ssorted += o;
+  v.az += o; v.d2 += o; v.baz += o; v.roadlist += o; v.roadcnt += (size_t)b0 * ((S + 31) >> 5); v.sortbuf += 2 * o;
+  v.Tf += (size_t)b0 * channels * kTStride; v.Tb += (size_t)b0 * channels * kTStride;
+  v.lut += (size_t)b0 * (kElevBins + 1); v.firstidx += (size_t)b0 * (kElevBins + 1);
+  v.hist += (size_t)b0 * T * kRingKeys;
+  v.cmin += (size_t)b0 * channels * kDegBins; v.cmax += (size_t)b0 * channels * kDegBins;
+  v.ne += (size_t)b0 * channels * (kDegBins + 1);
+  v.tab += b0;
   return v;
 }
-DevBuffers offset_view(const DevBuffers& a, int b0, int S, int T, int channels) { return slot_view(a, b0, b0, S, T, channels); }
 
 constexpr int kMaxKernels = 32;
 constexpr int kMarkSingleMax = 300000;   // scans above this many points take the multi-CTA marker search
@@ -168,8 +156,9 @@ int launch_pipeline(urf_ctx* ctx, const DevBuffers& buf, int B, int S, bool want
   K("k_scan_offsets", k_scan_offsets<<<B, 1024, 0, st>>>(buf, dp, S, T));   // + exact re-registration of refuted scans
   K("k_scatter", k_scatter<<<dim3((T + kScatterWarps - 1) / kScatterWarps, B), kScatterWarps * 32, kScatterSmem, st>>>(buf, dp, S, T));
   // the ring detector next to the star-shaped search: both only read what k_scatter left and add curb hits (idempotent
-  // marks, atomic min / max aggregates); k_tab1 is the first reader of the aggregates
-  const bool fork = ctx->inner_fork && dp.star && !ctx->profile;
+  // marks, atomic min / max aggregates); k_tab1 is the first reader of the aggregates. Per-kernel timing keeps every
+  // kernel on `st`, where K records its events, and without the star-shaped search there is nothing to overlap.
+  const bool fork = dp.star && !ctx->profile;
   cudaStream_t st_ring = st;
   int side = urf_ctx::kGroups;
   if (fork) {
@@ -178,19 +167,9 @@ int launch_pipeline(urf_ctx* ctx, const DevBuffers& buf, int B, int S, bool want
     CK(cudaEventRecord(ctx->ev_sfork[side], st));
     CK(cudaStreamWaitEvent(st_ring, ctx->ev_sfork[side], 0));
   }
-  const dim3 gtile((S + kTile4 - 1) / kTile4, B);
-  {
-    cudaStream_t st_main = st;
-    st = st_ring;
-    if (ctx->rd_variant == 4 && dp.curbPoints == 5)        // four positions per thread (default curb_points only)
-      K("k_ring_detect4", k_ring_detect4<4><<<gtile, 256, 0, st>>>(buf, dp, S));
-    else if (ctx->rd_variant == 45 && dp.curbPoints == 5) K("k_ring_detect4", k_ring_detect4<5><<<gtile, 256, 0, st>>>(buf, dp, S));
-    else if (ctx->rd_variant == 46 && dp.curbPoints == 5) K("k_ring_detect4", k_ring_detect4<6><<<gtile, 256, 0, st>>>(buf, dp, S));
-    else if (ctx->rd_variant == 6) K("k_ring_detect", k_ring_detect<6><<<gpts, 256, 0, st>>>(buf, dp, S));
-    else if (ctx->rd_variant == 5) K("k_ring_detect", k_ring_detect<5><<<gpts, 256, 0, st>>>(buf, dp, S));
-    else K("k_ring_detect", k_ring_detect<8><<<gpts, 256, 0, st>>>(buf, dp, S));   // 8 CTAs/SM (32 registers)
-    st = st_main;
-  }
+  if (dp.curbPoints == 5)              // four positions per thread (default curb_points only)
+    K("k_ring_detect4", k_ring_detect4<<<dim3((S + kTile4 - 1) / kTile4, B), 256, 0, st_ring>>>(buf, dp, S));
+  else K("k_ring_detect", k_ring_detect<<<gpts, 256, 0, st_ring>>>(buf, dp, S));
   if (fork) CK(cudaEventRecord(ctx->ev_sjoin[side], st_ring));
   if (dp.star) {
     const int gbig = std::max(4, std::min(kSectKeys, 2048 / B));
@@ -211,13 +190,12 @@ int launch_pipeline(urf_ctx* ctx, const DevBuffers& buf, int B, int S, bool want
   K("k_reach", k_reach<<<dim3((2 * kDegBins + 7) / 8, B), 256, 0, st>>>(buf, dp));
   K("k_tab2", k_tab2<<<dim3((dp.channels + kTab2Rings - 1) / kTab2Rings, B), kTab2Rings * 64, 0, st>>>(buf, dp));
   K("k_label", k_label<<<dim3((S + kLabelThreads * kLabelGroups - 1) / (kLabelThreads * kLabelGroups), B), kLabelThreads, 0, st>>>(buf, dp, S));
-  if (ctx->markers_variant == 2 || (ctx->markers_variant == 1 && S > kMarkSingleMax)) {   // large scans: a grid of CTAs per scan, three launches
+  if (S > kMarkSingleMax) {            // large scans: a grid of CTAs per scan, three launches
     const dim3 gm(std::max(1, std::min(64, S / 16384)), B);
     K("k_markers_grid1", k_markers_grid<1><<<gm, kMarkGridThreads, 0, st>>>(buf, S));
     K("k_markers_grid2", k_markers_grid<2><<<gm, kMarkGridThreads, 0, st>>>(buf, S));
     K("k_verts", k_verts<<<B, 384, 0, st>>>(buf, S));
-  } else if (ctx->markers_variant == 1) K("k_markers1", k_markers1<<<dim3(1, B), kMark1Threads, 0, st>>>(buf, S));   // one CTA per scan
-  else K("k_markers", k_markers<<<dim3(kMarkCtas, B), kMarkThreads, 0, st>>>(buf, S));              // cluster of kMarkCtas CTAs per scan
+  } else K("k_markers1", k_markers1<<<dim3(1, B), kMark1Threads, 0, st>>>(buf, S));   // one CTA per scan
   if (want_order) K("k_sort_rings", k_sort_rings<<<dim3(dp.channels, B), kSortThreads, kRingSmemKeys * sizeof(unsigned long long), st>>>(buf, S));
 #undef K
   if (last) CK(cudaEventRecord(ctx->ev1, st));
@@ -429,7 +407,6 @@ void urf_destroy(urf_ctx* ctx) {
   if (ctx->h_out) cudaFreeHost(ctx->h_out);
   if (ctx->h_packtot) cudaFreeHost(ctx->h_packtot);
   if (ctx->gexec) cudaGraphExecDestroy(ctx->gexec);
-  if (ctx->bexec) cudaGraphExecDestroy(ctx->bexec);
   for (cudaEvent_t e : ctx->kev) cudaEventDestroy(e);
   for (cudaEvent_t e : ctx->ev_in) cudaEventDestroy(e);
   for (cudaEvent_t e : ctx->ev_comp) cudaEventDestroy(e);
@@ -473,11 +450,10 @@ int urf_get_params(const urf_ctx* ctx, urf_params* p) {
 
 // test/diagnostic options: 0 = force exact ring registration (0/1); 1 = per-kernel CUDA-event timing (slots, 0 = off);
 // 2 = number of compute streams a device-resident batch is spread over (1..4); 3 = CUDA graph for small batches (0/1);
-// 4 = near-first star sort (0/1, default 1); 5 = scans per sub-batch of a device-resident batch (0 = batch / streams);
-// 6 = replay the fork/join of a device-resident batch as one CUDA graph (0/1); 7 = sub-batches of a stream share one
-// workspace slot (0/1); 8 = ring detector variant; 9 = marker search variant; 10 = near-first pivot rank (3..28 of 32 samples);
-// 11 = ring detector on a side stream next to the star-shaped search (0/1, default 1); 12 = accepted and ignored (it chose
-// the widest single-warp star sort network; k_star_sort has one, 16 elements per lane, and wider sorts go to k_star_sort_big)
+// 4 = near-first star sort (0/1, default 1); 10 = near-first pivot rank (3..28 of 32 samples).
+// 5, 6, 7, 8, 9, 11 and 12 are retired numbers, accepted and ignored: they selected scheduling and kernel variants
+// (sub-batch size, batch graph, shared workspace slots, ring detector and marker search variants, ring detector on the
+// pipeline's own stream, star sort network width) that measured no better than the defaults, which are all that is left.
 int urf_set_option(urf_ctx* ctx, int option, int value) {
   if (!ctx) return URF_ERR_INVALID;
   CK(cudaSetDevice(ctx->device));
@@ -486,13 +462,7 @@ int urf_set_option(urf_ctx* ctx, int option, int value) {
   if (option == 4) { ctx->dp.star_prefix = value != 0; ctx->version++; return URF_OK; }
   if (option == 3) { ctx->use_graph = value != 0; return URF_OK; }
   if (option == 2) { ctx->groups = value < 1 ? 1 : (value > urf_ctx::kGroups ? urf_ctx::kGroups : value); return URF_OK; }
-  if (option == 5) { ctx->sub = value < 0 ? 0 : value; return URF_OK; }
-  if (option == 6) { ctx->batch_graph = value != 0; return URF_OK; }
-  if (option == 7) { ctx->slot_reuse = value != 0; return URF_OK; }
-  if (option == 8) { ctx->rd_variant = value; return URF_OK; }
-  if (option == 9) { ctx->markers_variant = value; return URF_OK; }
-  if (option == 12) return URF_OK;
-  if (option == 11) { ctx->inner_fork = value != 0; return URF_OK; }
+  if ((option >= 5 && option <= 9) || option == 11 || option == 12) return URF_OK;
   if (option == 10) { ctx->dp.star_pivot = value < 3 ? 3 : (value > 28 ? 28 : value); return URF_OK; }
   if (option == 1) {                   // value = number of event slots (0 = off)
     CK(cudaStreamSynchronize(ctx->stream));               // events of the previous setting may still be pending
@@ -568,56 +538,27 @@ int urf_enqueue_batch_device_ex(urf_ctx* ctx, const float* d_xyzi, int stride_po
   if (want_order) bufv.order = d_order;
   int rc = URF_OK;
   const int T = (stride_points + kChunk - 1) / kChunk;
-  int sub = ctx->sub > 0 ? std::min(ctx->sub, batch) : (batch + ctx->groups - 1) / ctx->groups;
-  const int nsub = (batch + sub - 1) / sub;
-  const int G = (ctx->profile || batch < 2 * ctx->groups) ? 1 : std::min(ctx->groups, nsub);   // per-kernel event timing needs one stream
+  const int G = (ctx->profile || batch < 2 * ctx->groups) ? 1 : ctx->groups;   // per-kernel event timing needs one stream
   if (G == 1) rc = launch_pipeline(ctx, bufv, batch, stride_points, want_order);
   else {
-    // fork: the ctx stream hands sub-batches to the group streams (round-robin) and joins them again, so callers still see
-    // ONE stream. Scans are independent: a stream works through its sub-batches one after the other.
-    const bool reuse = ctx->slot_reuse;
-    auto fork_join = [&]() -> int {
-      CK(cudaEventRecord(ctx->ev_fork, ctx->stream));
-      int launches = 0;
-      for (int g = 0; g < G; g++) CK(cudaStreamWaitEvent(ctx->s_grp[g], ctx->ev_fork, 0));
-      for (int j = 0; j < nsub; j++) {
-        const int g = j % G, b0 = j * sub, nb = std::min(sub, batch - b0);
-        const int r = launch_pipeline(ctx, slot_view(bufv, b0, reuse ? g * sub : b0, stride_points, T, ctx->dp.channels), nb, stride_points,
-                                      want_order, false, false, ctx->s_grp[g]);
-        if (r != URF_OK) return r;
-        launches += ctx->launches;
-      }
-      for (int g = 0; g < G; g++) {
-        CK(cudaEventRecord(ctx->ev_join[g], ctx->s_grp[g]));
-        CK(cudaStreamWaitEvent(ctx->stream, ctx->ev_join[g], 0));
-      }
-      ctx->launches = launches;
-      return URF_OK;
-    };
+    // fork: the ctx stream hands one of G near-equal sub-batches (scans [ceil(g * batch / G), ceil((g + 1) * batch / G)))
+    // to each group stream and joins them again, so callers still see ONE stream. Scans are independent.
     CK(cudaEventRecord(ctx->ev0, ctx->stream));
-    if (!ctx->batch_graph) rc = fork_join();
-    else {
-      auto& k = ctx->bkey;
-      if (!ctx->bexec || k.B != batch || k.S != stride_points || k.sub != sub || k.G != G || k.order != (int)want_order || k.reuse != reuse ||
-          k.in != (const void*)d_xyzi || k.label != (void*)d_label || k.orderp != (void*)d_order || k.version != ctx->version) {
-        if (ctx->bexec) { cudaGraphExecDestroy(ctx->bexec); ctx->bexec = nullptr; }
-        cudaGraph_t graph = nullptr;
-        CK(cudaStreamBeginCapture(ctx->stream, cudaStreamCaptureModeThreadLocal));
-        rc = fork_join();
-        const cudaError_t e = cudaStreamEndCapture(ctx->stream, &graph);
-        if (rc != URF_OK || e != cudaSuccess || !graph) {
-          if (graph) cudaGraphDestroy(graph);
-          if (rc == URF_OK) { ctx->err = std::string("batch graph capture: ") + cudaGetErrorString(e); rc = URF_ERR_CUDA; }
-        } else {
-          const cudaError_t ei = cudaGraphInstantiate(&ctx->bexec, graph, 0);
-          cudaGraphDestroy(graph);
-          if (ei != cudaSuccess) { ctx->bexec = nullptr; ctx->err = cudaGetErrorString(ei); rc = URF_ERR_CUDA; }
-          else { k.B = batch; k.S = stride_points; k.sub = sub; k.G = G; k.order = (int)want_order; k.reuse = reuse; k.in = d_xyzi; k.label = d_label; k.orderp = d_order;
-                 k.version = ctx->version; k.launches = ctx->launches; }
-        }
-      }
-      if (rc == URF_OK) { CK(cudaGraphLaunch(ctx->bexec, ctx->stream)); ctx->launches = ctx->bkey.launches; }
+    CK(cudaEventRecord(ctx->ev_fork, ctx->stream));
+    for (int g = 0; g < G; g++) CK(cudaStreamWaitEvent(ctx->s_grp[g], ctx->ev_fork, 0));
+    int launches = 0;
+    for (int g = 0; g < G; g++) {
+      const int b0 = (g * batch + G - 1) / G, b1 = ((g + 1) * batch + G - 1) / G;
+      rc = launch_pipeline(ctx, offset_view(bufv, b0, stride_points, T, ctx->dp.channels), b1 - b0, stride_points, want_order, false, false,
+                           ctx->s_grp[g]);
+      if (rc != URF_OK) return rc;
+      launches += ctx->launches;
     }
+    for (int g = 0; g < G; g++) {
+      CK(cudaEventRecord(ctx->ev_join[g], ctx->s_grp[g]));
+      CK(cudaStreamWaitEvent(ctx->stream, ctx->ev_join[g], 0));
+    }
+    ctx->launches = launches;
     CK(cudaEventRecord(ctx->ev1, ctx->stream));
   }
   ctx->last_B = batch; ctx->last_S = stride_points;
