@@ -12,7 +12,7 @@ from urban_road_filter_b200 import FULL_ROI, make_params
 from urban_road_filter_b200 import api
 from urban_road_filter_b200.synth import SHAPES, make_scan, random_cloud
 
-from util import Golden, assert_matches_golden, golden_names, stage_diffs
+from util import Golden, assert_matches_golden, cloud2_records, golden_names, stage_diffs
 
 pytestmark = pytest.mark.gpu
 
@@ -442,7 +442,7 @@ def test_gpu_lean_and_batched_record_entries(port):
                     assert stage_diffs(o, r, c.shape[0]) == []
                 else:
                     assert np.all(r.label == -1)
-        recs = [_cloud2_records(c, 22, 0, 4, 8, 12, seed=i).reshape(-1) for i, c in enumerate(clouds)]     # Velodyne-like, unaligned
+        recs = [cloud2_records(c, 22, 0, 4, 8, 12, seed=i).reshape(-1) for i, c in enumerate(clouds)]     # Velodyne-like, unaligned
         rs = d.filtered_batch_records(recs, 22, 0, 4, 8, 12, want_order=True, label8=True)
         for o, r, c in zip(exp, rs, clouds):
             assert o.status == r.status
@@ -455,15 +455,6 @@ def test_gpu_lean_and_batched_record_entries(port):
             assert stage_diffs(o, r, c.shape[0]) == []
     finally:
         d.close()
-
-
-def _cloud2_records(pts, step, ox, oy, oz, oi, seed=0):
-    n = pts.shape[0]
-    rec = np.random.default_rng(seed).integers(0, 256, (n, step), dtype=np.uint8)     # garbage in the other fields
-    for k, off in enumerate((ox, oy, oz, oi)):
-        if off >= 0:
-            rec[:, off: off + 4] = pts[:, k: k + 1].copy().view(np.uint8)
-    return rec.reshape(-1)
 
 
 def _expect_records(pts, ids, with_intensity=True):
@@ -485,7 +476,7 @@ def test_gpu_packed_clouds_match_reference_goldens(det, det_big, name):
     if n > det.max_points:
         det = det_big()                                                   # the C5 fixtures (1,048,576 points)
     det.set_params(g.params())
-    raw = _cloud2_records(pts, 48, 0, 4, 8, 16, seed=n)                 # Ouster-like 48-byte records, intensity at 16
+    raw = cloud2_records(pts, 48, 0, 4, 8, 16, seed=n)                 # Ouster-like 48-byte records, intensity at 16
     r, cl = det.filtered_cloud2_packed(raw, n, 48, 0, 4, 8, 16, want_labels=True)
     if not g.published:
         assert r.status == 1 and all(len(v) == 0 for v in cl.values())
@@ -506,7 +497,7 @@ def test_gpu_packed_clouds_match_oracle(det, port, shape, step, offs):
     n = pts.shape[0]
     for prm in (make_params(), make_params(**FULL_ROI)):
         det.set_params(prm)
-        raw = _cloud2_records(pts, step, *offs, seed=step)
+        raw = cloud2_records(pts, step, *offs, seed=step)
         r, cl = det.filtered_cloud2_packed(raw, n, step, *offs)
         o = port.run(pts, prm)
         assert r.status == o.status == 0

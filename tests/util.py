@@ -146,6 +146,17 @@ def feq(a: np.ndarray, b: np.ndarray) -> bool:
     return a.shape == b.shape and np.array_equal(a.view(np.uint32), b.view(np.uint32))
 
 
+def cloud2_records(pts, step, ox, oy, oz, oi, seed=0):
+    """PointCloud2 record bytes of an (N, 4) cloud: x / y / z / intensity as float32 at the given byte offsets (oi < 0:
+    none), seeded garbage in the other bytes of each `step`-byte record."""
+    n = pts.shape[0]
+    rec = np.random.default_rng(seed).integers(0, 256, (n, step), dtype=np.uint8)     # garbage in the other fields
+    for k, off in enumerate((ox, oy, oz, oi)):
+        if off >= 0:
+            rec[:, off: off + 4] = pts[:, k: k + 1].copy().view(np.uint8)
+    return rec.reshape(-1)
+
+
 class ModelResult:
     pass
 

@@ -133,6 +133,19 @@ class ScanResult:
         return self.order[lab == (1 if which == "road" else 2)]
 
 
+def _scan_result(res: UrfResult, label, ring=None, order=None, ring_start=None) -> ScanResult:
+    """ScanResult of a filled urf_result: `label` and `ring` as given, `order` / `ring_start` (the caller's whole buffers, or
+    None) cut to n_order / n_rings + 1 entries and copied, the vertices copied."""
+    r = ScanResult()
+    for f in ("status", "n_in", "n_roi", "n_rings", "n_order", "n_road", "n_curb", "n_vert", "flags"):
+        setattr(r, f, int(getattr(res, f)))
+    r.label, r.ring = label, ring
+    r.order = None if order is None else order[: r.n_order].copy()
+    r.ring_start = None if ring_start is None else ring_start[: r.n_rings + 1].copy()
+    r.vert = np.ctypeslib.as_array(res.vert).reshape(URF_MAX_VERTS, 4)[: r.n_vert].copy()
+    return r
+
+
 def build_markers(prm: UrfParams, vert: np.ndarray, ghostcount: int = 0):
     """Marker tail (lidar_segmentation.cpp:371-598). Returns (strips, ghostcount'): strips = [(id, action, red, xyz[n,3])]."""
     lib = load_library()
@@ -211,16 +224,8 @@ class Detector:
         out = []
         for b, a in enumerate(arrs):
             lab, ring, order, rs = keep[b]
-            r = ScanResult()
             n = a.shape[0]
-            for f in ("status", "n_in", "n_roi", "n_rings", "n_order", "n_road", "n_curb", "n_vert", "flags"):
-                setattr(r, f, int(getattr(res[b], f)))
-            r.label = lab[:n]
-            r.ring = ring[:n] if want_ring else None
-            r.order = order[: r.n_order].copy() if want_order else None
-            r.ring_start = rs[: r.n_rings + 1].copy()
-            r.vert = np.ctypeslib.as_array(res[b].vert).reshape(URF_MAX_VERTS, 4)[: r.n_vert].copy()
-            out.append(r)
+            out.append(_scan_result(res[b], lab[:n], ring[:n] if want_ring else None, order, rs))
         return out
 
     def filtered_batch_records(self, records, point_step: int, off_x: int, off_y: int, off_z: int, off_intensity: int = -1,
@@ -257,15 +262,7 @@ class Detector:
         out = []
         for b, n in enumerate(ns):
             lab, order, rs = keep[b]
-            r = ScanResult()
-            for f in ("status", "n_in", "n_roi", "n_rings", "n_order", "n_road", "n_curb", "n_vert", "flags"):
-                setattr(r, f, int(getattr(res[b], f)))
-            r.label = lab[:n].astype(np.int32)
-            r.ring = None
-            r.order = order[: r.n_order].copy() if want_order else None
-            r.ring_start = rs[: r.n_rings + 1].copy()
-            r.vert = np.ctypeslib.as_array(res[b].vert).reshape(URF_MAX_VERTS, 4)[: r.n_vert].copy()
-            out.append(r)
+            out.append(_scan_result(res[b], lab[:n].astype(np.int32), None, order, rs))
         return out
 
     def filtered_cloud2(self, data: bytes | np.ndarray, n_points: int, point_step: int, off_x: int, off_y: int, off_z: int) -> ScanResult:
@@ -279,13 +276,7 @@ class Detector:
         res.order = order.ctypes.data_as(C.POINTER(C.c_int32)); res.ring_start = rs.ctypes.data_as(C.POINTER(C.c_int32))
         self._check(self.lib.urf_process_cloud2(self._ctx, raw.ctypes.data, n_points, point_step, off_x, off_y, off_z, C.byref(res)),
                     "urf_process_cloud2")
-        r = ScanResult()
-        for f in ("status", "n_in", "n_roi", "n_rings", "n_order", "n_road", "n_curb", "n_vert", "flags"):
-            setattr(r, f, int(getattr(res, f)))
-        r.label, r.ring, r.order = lab[:n_points], ring[:n_points], order[: r.n_order].copy()
-        r.ring_start = rs[: r.n_rings + 1].copy()
-        r.vert = np.ctypeslib.as_array(res.vert).reshape(URF_MAX_VERTS, 4)[: r.n_vert].copy()
-        return r
+        return _scan_result(res, lab[:n_points], ring[:n_points], order, rs)
 
     def filtered_cloud2_packed(self, data, n_points: int, point_step: int, off_x: int, off_y: int, off_z: int,
                                off_intensity: int = -1, want_labels: bool = False):
@@ -307,14 +298,7 @@ class Detector:
             res.label = lab.ctypes.data_as(C.POINTER(C.c_int32)); res.order = order.ctypes.data_as(C.POINTER(C.c_int32))
         self._check(self.lib.urf_process_cloud2_packed(self._ctx, raw.ctypes.data, n_points, point_step, off_x, off_y, off_z,
                                                        off_intensity, C.byref(res), C.byref(cl)), "urf_process_cloud2_packed")
-        r = ScanResult()
-        for f in ("status", "n_in", "n_roi", "n_rings", "n_order", "n_road", "n_curb", "n_vert", "flags"):
-            setattr(r, f, int(getattr(res, f)))
-        r.label = lab[:n_points] if want_labels else None
-        r.order = order[: r.n_order].copy() if want_labels else None
-        r.ring = None
-        r.ring_start = rs[: r.n_rings + 1].copy()
-        r.vert = np.ctypeslib.as_array(res.vert).reshape(URF_MAX_VERTS, 4)[: r.n_vert].copy()
+        r = _scan_result(res, lab[:n_points] if want_labels else None, None, order, rs)
         counts = dict(road=cl.n_road, curb=cl.n_curb, roi=cl.n_roi, road_probably=cl.n_road_probably)
         return r, {k: bufs[k][: counts[k]] for k in bufs}
 
@@ -402,13 +386,7 @@ class MultiGpuQueue:
         if rc != URF_OK:
             raise UrfError(rc, "urf_mq_next")
         self._keep.pop(tag.value, None)
-        r = ScanResult()
-        for f in ("status", "n_in", "n_roi", "n_rings", "n_order", "n_road", "n_curb", "n_vert", "flags"):
-            setattr(r, f, int(getattr(res, f)))
-        r.label = lab[: r.n_in].copy()
-        r.ring = r.order = r.ring_start = None
-        r.vert = np.ctypeslib.as_array(res.vert).reshape(URF_MAX_VERTS, 4)[: r.n_vert].copy()
-        return tag.value, r
+        return tag.value, _scan_result(res, lab[: res.n_in].copy())
 
     def stats(self) -> dict:
         st = UrfMqStats()
@@ -467,13 +445,7 @@ class ScanQueue:
             return None
         if rc != URF_OK:
             raise UrfError(rc, "urf_queue_next")
-        r = ScanResult()
-        for f in ("status", "n_in", "n_roi", "n_rings", "n_order", "n_road", "n_curb", "n_vert", "flags"):
-            setattr(r, f, int(getattr(res, f)))
-        r.label = lab[: r.n_in].copy()
-        r.ring = r.order = r.ring_start = None
-        r.vert = np.ctypeslib.as_array(res.vert).reshape(URF_MAX_VERTS, 4)[: r.n_vert].copy()
-        return int(tag.value), r
+        return int(tag.value), _scan_result(res, lab[: res.n_in].copy())
 
     def stats(self) -> dict:
         st = UrfQueueStats()

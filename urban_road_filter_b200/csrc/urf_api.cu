@@ -41,9 +41,10 @@ struct urf_ctx {
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   DevBuffers buf{};
   float4* own_in = nullptr;
-  unsigned char* raw = nullptr;        // PointCloud2 staging: max_points * URF_MAX_POINT_STEP bytes (urf_process_cloud2)
-  unsigned char* rawb = nullptr;       // batched record staging (urf_process_cloud2_batch / _xyz): P * rawb_step bytes, first use
-  int rawb_step = 0;
+  // record staging of the PointCloud2 / packed-xyz entry points: max_points * URF_MAX_POINT_STEP bytes from urf_create, so
+  // single scans never allocate; re-allocated at P * step bytes by the first batch that needs more
+  unsigned char* rawb = nullptr;
+  size_t rawb_bytes = 0;
   signed char* label8 = nullptr;       // int8 labels (P bytes), allocated when a caller first asks for them
   int* own_label = nullptr;
   float4* pack = nullptr;              // packed output clouds (urf_process_cloud2_packed): 3 * max_points 32-byte records, allocated on first use
@@ -77,13 +78,17 @@ struct urf_ctx {
 
 namespace {
 
+// URF code of a CUDA status; the text of a failed call is kept for urf_last_cuda_error
+int cuda_rc(urf_ctx* ctx, cudaError_t e, const char* call) {
+  if (e == cudaSuccess) return URF_OK;
+  ctx->err = std::string(call) + ": " + cudaGetErrorString(e);
+  return e == cudaErrorMemoryAllocation ? URF_ERR_NOMEM : URF_ERR_CUDA;
+}
+
 #define CK(call)                                                                                   \
   do {                                                                                             \
-    cudaError_t e_ = (call);                                                                       \
-    if (e_ != cudaSuccess) {                                                                       \
-      ctx->err = std::string(#call) + ": " + cudaGetErrorString(e_);                               \
-      return e_ == cudaErrorMemoryAllocation ? URF_ERR_NOMEM : URF_ERR_CUDA;                        \
-    }                                                                                              \
+    const int rc_ = cuda_rc(ctx, (call), #call);                                                   \
+    if (rc_ != URF_OK) return rc_;                                                                 \
   } while (0)
 
 template <class T> int dalloc(urf_ctx* ctx, T** p, size_t count) {
@@ -127,11 +132,12 @@ constexpr int kMaxKernels = 32;
 constexpr int kMarkSingleMax = 300000;   // scans above this many points take the multi-CTA marker search
 thread_local std::string g_create_err;
 
-int launch_pipeline(urf_ctx* ctx, const DevBuffers& buf, int B, int S, bool want_order, bool first = true, bool last = true,
-                    cudaStream_t st_override = nullptr) {
+// Enqueues the kernel sequence for B scans of stride S from `buf` on the stream of `group` (0 .. kGroups-1: a group
+// stream, kGroups: the context's own stream) and stores the number of kernels launched in *launched.
+int launch_pipeline(urf_ctx* ctx, const DevBuffers& buf, int B, int S, bool want_order, int group, int* launched) {
   DevParams dp = ctx->dp;
   dp.want_order = want_order ? 1 : 0;
-  cudaStream_t st = st_override ? st_override : ctx->stream;
+  cudaStream_t st = group < urf_ctx::kGroups ? ctx->s_grp[group] : ctx->stream;
   const int T = (S + kChunk - 1) / kChunk;
   if (T > ctx->Tmax) return URF_ERR_CAPACITY;
   int L = 0;
@@ -148,7 +154,6 @@ int launch_pipeline(urf_ctx* ctx, const DevBuffers& buf, int B, int S, bool want
     __VA_ARGS__;                                                                             \
     L++;                                                                                     \
   } while (0)
-  if (first) CK(cudaEventRecord(ctx->ev0, st));
   K("k_reset", k_reset<<<dim3(8, B), 256, 0, st>>>(buf, dp));
   K("k_points", k_points<<<gpts, 256, 0, st>>>(buf, dp, S));
   K("k_register", k_register<<<B, 256, 0, st>>>(buf, dp, S));
@@ -159,18 +164,15 @@ int launch_pipeline(urf_ctx* ctx, const DevBuffers& buf, int B, int S, bool want
   // marks, atomic min / max aggregates); k_tab1 is the first reader of the aggregates. Per-kernel timing keeps every
   // kernel on `st`, where K records its events, and without the star-shaped search there is nothing to overlap.
   const bool fork = dp.star && !ctx->profile;
-  cudaStream_t st_ring = st;
-  int side = urf_ctx::kGroups;
+  cudaStream_t st_ring = fork ? ctx->s_side[group] : st;
   if (fork) {
-    for (int g = 0; g < urf_ctx::kGroups; g++) if (st == ctx->s_grp[g]) side = g;
-    st_ring = ctx->s_side[side];
-    CK(cudaEventRecord(ctx->ev_sfork[side], st));
-    CK(cudaStreamWaitEvent(st_ring, ctx->ev_sfork[side], 0));
+    CK(cudaEventRecord(ctx->ev_sfork[group], st));
+    CK(cudaStreamWaitEvent(st_ring, ctx->ev_sfork[group], 0));
   }
   if (dp.curbPoints == 5)              // four positions per thread (default curb_points only)
     K("k_ring_detect4", k_ring_detect4<<<dim3((S + kTile4 - 1) / kTile4, B), 256, 0, st_ring>>>(buf, dp, S));
   else K("k_ring_detect", k_ring_detect<<<gpts, 256, 0, st_ring>>>(buf, dp, S));
-  if (fork) CK(cudaEventRecord(ctx->ev_sjoin[side], st_ring));
+  if (fork) CK(cudaEventRecord(ctx->ev_sjoin[group], st_ring));
   if (dp.star) {
     const int gbig = std::max(4, std::min(kSectKeys, 2048 / B));
     const dim3 gscan((kSectKeys + kScanWarps * 32 - 1) / (kScanWarps * 32), B);
@@ -185,7 +187,7 @@ int launch_pipeline(urf_ctx* ctx, const DevBuffers& buf, int B, int S, bool want
     if (dp.star_prefix)            // sectors whose edge search ran off the near-first prefix: full sort, search resumed
       K("k_star_refine", k_star_refine<<<dim3(std::max(8, std::min(kSectKeys / 8, 8192 / B)), B), 256, kStarCtaSmem, st>>>(buf, dp, S));
   }
-  if (fork) CK(cudaStreamWaitEvent(st, ctx->ev_sjoin[side], 0));
+  if (fork) CK(cudaStreamWaitEvent(st, ctx->ev_sjoin[group], 0));
   K("k_tab1", k_tab1<<<dim3((dp.channels + 7) / 8, B), 256, 0, st>>>(buf, dp));
   K("k_reach", k_reach<<<dim3((2 * kDegBins + 7) / 8, B), 256, 0, st>>>(buf, dp));
   K("k_tab2", k_tab2<<<dim3((dp.channels + kTab2Rings - 1) / kTab2Rings, B), kTab2Rings * 64, 0, st>>>(buf, dp));
@@ -198,56 +200,49 @@ int launch_pipeline(urf_ctx* ctx, const DevBuffers& buf, int B, int S, bool want
   } else K("k_markers1", k_markers1<<<dim3(1, B), kMark1Threads, 0, st>>>(buf, S));   // one CTA per scan
   if (want_order) K("k_sort_rings", k_sort_rings<<<dim3(dp.channels, B), kSortThreads, kRingSmemKeys * sizeof(unsigned long long), st>>>(buf, S));
 #undef K
-  if (last) CK(cudaEventRecord(ctx->ev1, st));
   if (ctx->profile) {
     CK(cudaEventRecord(ctx->kev[(size_t)ctx->kslot * (kMaxKernels + 1) + kMaxKernels], st));
     ctx->kcounts[ctx->kslot] = ctx->kcount;
     ctx->kslot = (ctx->kslot + 1) % ctx->kslots;
   }
   CK(cudaGetLastError());
-  ctx->launches = (first || st_override) ? L : ctx->launches + L;
-  ctx->timing_valid = true;
+  *launched = L;
   return URF_OK;
 }
 
-// Small batches: replay the whole kernel sequence as one CUDA graph (buf must be ctx->buf itself: constant pointers).
-int launch_pipeline_graphed(urf_ctx* ctx, int B, int S, bool want_order) {
-  if (!ctx->use_graph || ctx->profile) return launch_pipeline(ctx, ctx->buf, B, S, want_order);
-  cudaStream_t st = ctx->stream;
-  if (!ctx->gexec || ctx->g_B != B || ctx->g_S != S || ctx->g_order != (int)want_order || ctx->g_version != ctx->version) {
-    if (ctx->gexec) { cudaGraphExecDestroy(ctx->gexec); ctx->gexec = nullptr; }
-    cudaGraph_t graph = nullptr;
-    CK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-    ctx->launches = 0;
-    const int rc = launch_pipeline(ctx, ctx->buf, B, S, want_order, false, false);
-    const cudaError_t e = cudaStreamEndCapture(st, &graph);
-    if (rc != URF_OK || e != cudaSuccess || !graph) { if (graph) cudaGraphDestroy(graph); ctx->err = "graph capture failed"; return rc != URF_OK ? rc : URF_ERR_CUDA; }
-    const cudaError_t ei = cudaGraphInstantiate(&ctx->gexec, graph, 0);
-    cudaGraphDestroy(graph);
-    if (ei != cudaSuccess) { ctx->gexec = nullptr; ctx->err = cudaGetErrorString(ei); return URF_ERR_CUDA; }
-    ctx->g_B = B; ctx->g_S = S; ctx->g_order = (int)want_order; ctx->g_version = ctx->version; ctx->g_launches = ctx->launches;
-  }
-  CK(cudaEventRecord(ctx->ev0, st));
-  CK(cudaGraphLaunch(ctx->gexec, st));
-  CK(cudaEventRecord(ctx->ev1, st));
-  ctx->launches = ctx->g_launches;
-  ctx->timing_valid = true;
+// Small host-buffer batches replay the kernel sequence as one CUDA graph (launch latency dominates there). Makes
+// ctx->gexec the graph of this shape, captured from ctx->buf itself (the graph keeps its pointers) and re-captured when
+// the shape, the parameters or an option change.
+int update_graph(urf_ctx* ctx, int B, int S, bool want_order) {
+  if (ctx->gexec && ctx->g_B == B && ctx->g_S == S && ctx->g_order == (int)want_order && ctx->g_version == ctx->version) return URF_OK;
+  if (ctx->gexec) { cudaGraphExecDestroy(ctx->gexec); ctx->gexec = nullptr; }
+  cudaGraph_t graph = nullptr;
+  CK(cudaStreamBeginCapture(ctx->stream, cudaStreamCaptureModeThreadLocal));
+  int L = 0;
+  const int rc = launch_pipeline(ctx, ctx->buf, B, S, want_order, urf_ctx::kGroups, &L);
+  const cudaError_t e = cudaStreamEndCapture(ctx->stream, &graph);
+  if (rc != URF_OK || e != cudaSuccess || !graph) { if (graph) cudaGraphDestroy(graph); ctx->err = "graph capture failed"; return rc != URF_OK ? rc : URF_ERR_CUDA; }
+  const cudaError_t ei = cudaGraphInstantiate(&ctx->gexec, graph, 0);
+  cudaGraphDestroy(graph);
+  if (ei != cudaSuccess) { ctx->gexec = nullptr; ctx->err = cudaGetErrorString(ei); return URF_ERR_CUDA; }
+  ctx->g_B = B; ctx->g_S = S; ctx->g_order = (int)want_order; ctx->g_version = ctx->version; ctx->g_launches = L;
   return URF_OK;
 }
 
-void fill_result(const ScanOut& o, urf_result* r) {
+// with_ring_start = false leaves the caller's ring_start untouched
+void fill_result(const ScanOut& o, urf_result* r, bool with_ring_start) {
   r->n_in = o.n_in; r->n_roi = o.n_roi;
   r->flags = o.flags & F_PUBLIC_MASK; r->reserved = 0;
   if (o.n_roi < 30) {                       // lidar_segmentation.cpp:124-126
     r->status = URF_TOO_FEW_POINTS;
     r->n_rings = 0; r->n_order = 0; r->n_road = 0; r->n_curb = 0; r->n_vert = 0;
-    if (r->ring_start) for (int k = 0; k <= URF_MAX_CHANNELS; k++) r->ring_start[k] = 0;
+    if (with_ring_start && r->ring_start) for (int k = 0; k <= URF_MAX_CHANNELS; k++) r->ring_start[k] = 0;
     return;
   }
   r->status = URF_OK;
   r->n_rings = o.n_rings; r->n_order = o.n_order; r->n_road = o.n_road; r->n_curb = o.n_curb; r->n_vert = o.n_vert;
   std::memcpy(r->vert, o.vert, sizeof(float) * 4 * (size_t)o.n_vert);
-  if (r->ring_start) std::memcpy(r->ring_start, o.ring_start, sizeof(int) * (URF_MAX_CHANNELS + 1));
+  if (with_ring_start && r->ring_start) std::memcpy(r->ring_start, o.ring_start, sizeof(int) * (URF_MAX_CHANNELS + 1));
 }
 
 }  // namespace
@@ -326,7 +321,8 @@ int urf_create(urf_ctx** out, int device, int max_points, int max_batch) {
   const size_t P = ctx->P;
   DevBuffers& b = ctx->buf;
   TRY(dalloc(ctx, &ctx->own_in, P));
-  TRY(dalloc(ctx, &ctx->raw, (size_t)ctx->max_points * URF_MAX_POINT_STEP));
+  ctx->rawb_bytes = (size_t)ctx->max_points * URF_MAX_POINT_STEP;
+  TRY(dalloc(ctx, &ctx->rawb, ctx->rawb_bytes));
   TRY(dalloc(ctx, &b.alpha_v, P));
   TRY(dalloc(ctx, &b.mark, P));
   TRY(dalloc(ctx, &b.ringid, P));
@@ -536,33 +532,35 @@ int urf_enqueue_batch_device_ex(urf_ctx* ctx, const float* d_xyzi, int stride_po
   bufv.in = reinterpret_cast<float4*>(const_cast<float*>(d_xyzi));
   bufv.label = d_label;
   if (want_order) bufv.order = d_order;
-  int rc = URF_OK;
   const int T = (stride_points + kChunk - 1) / kChunk;
   const int G = (ctx->profile || batch < 2 * ctx->groups) ? 1 : ctx->groups;   // per-kernel event timing needs one stream
-  if (G == 1) rc = launch_pipeline(ctx, bufv, batch, stride_points, want_order);
-  else {
+  int launches = 0;
+  CK(cudaEventRecord(ctx->ev0, ctx->stream));
+  if (G == 1) {
+    const int rc = launch_pipeline(ctx, bufv, batch, stride_points, want_order, urf_ctx::kGroups, &launches);
+    if (rc != URF_OK) return rc;
+  } else {
     // fork: the ctx stream hands one of G near-equal sub-batches (scans [ceil(g * batch / G), ceil((g + 1) * batch / G)))
     // to each group stream and joins them again, so callers still see ONE stream. Scans are independent.
-    CK(cudaEventRecord(ctx->ev0, ctx->stream));
     CK(cudaEventRecord(ctx->ev_fork, ctx->stream));
     for (int g = 0; g < G; g++) CK(cudaStreamWaitEvent(ctx->s_grp[g], ctx->ev_fork, 0));
-    int launches = 0;
     for (int g = 0; g < G; g++) {
       const int b0 = (g * batch + G - 1) / G, b1 = ((g + 1) * batch + G - 1) / G;
-      rc = launch_pipeline(ctx, offset_view(bufv, b0, stride_points, T, ctx->dp.channels), b1 - b0, stride_points, want_order, false, false,
-                           ctx->s_grp[g]);
+      int L = 0;
+      const int rc = launch_pipeline(ctx, offset_view(bufv, b0, stride_points, T, ctx->dp.channels), b1 - b0, stride_points, want_order, g, &L);
       if (rc != URF_OK) return rc;
-      launches += ctx->launches;
+      launches += L;
     }
     for (int g = 0; g < G; g++) {
       CK(cudaEventRecord(ctx->ev_join[g], ctx->s_grp[g]));
       CK(cudaStreamWaitEvent(ctx->stream, ctx->ev_join[g], 0));
     }
-    ctx->launches = launches;
-    CK(cudaEventRecord(ctx->ev1, ctx->stream));
   }
+  CK(cudaEventRecord(ctx->ev1, ctx->stream));
+  ctx->launches = launches;
+  ctx->timing_valid = true;
   ctx->last_B = batch; ctx->last_S = stride_points;
-  return rc;
+  return URF_OK;
 }
 
 int urf_enqueue_batch_device(urf_ctx* ctx, const float* d_xyzi, int stride_points, const int* n, int batch, int32_t* d_label) {
@@ -575,13 +573,7 @@ int urf_finish_batch_device(urf_ctx* ctx, urf_result* outs) {
   const int B = ctx->last_B;
   if (outs) CK(cudaMemcpyAsync(ctx->h_out, ctx->buf.out, sizeof(ScanOut) * B, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  if (outs) for (int b = 0; b < B; b++) {
-    urf_result tmp = outs[b];
-    tmp.ring_start = nullptr;
-    fill_result(ctx->h_out[b], &tmp);
-    tmp.label = outs[b].label; tmp.ring = outs[b].ring; tmp.order = outs[b].order; tmp.ring_start = outs[b].ring_start;
-    outs[b] = tmp;
-  }
+  if (outs) for (int b = 0; b < B; b++) fill_result(ctx->h_out[b], &outs[b], false);
   return URF_OK;
 }
 
@@ -597,8 +589,9 @@ namespace {
 // are copied straight into the input buffer; step > 0: data[b] holds n[b] records of `step` bytes with FLOAT32 x / y / z /
 // intensity at the given byte offsets (oi < 0: none) — the raw bytes cross PCIe and are unpacked on the device.
 // label8 (or NULL): per scan an int8 HOST buffer for the labels (one byte per point instead of four).
+// clouds (or NULL, batch == 1 only): the four published clouds of the scan, packed on the device.
 int process_batch_impl(urf_ctx* ctx, const void* const* data, const int* n, int batch, int step, int ox, int oy, int oz, int oi,
-                       urf_result* outs, int8_t* const* label8) {
+                       urf_result* outs, int8_t* const* label8, urf_clouds* clouds) {
   if (!ctx || !data || !n || !outs || batch < 1) return URF_ERR_INVALID;
   if (batch > ctx->max_batch) return URF_ERR_CAPACITY;
   if (step != 0) {
@@ -608,7 +601,7 @@ int process_batch_impl(urf_ctx* ctx, const void* const* data, const int* n, int 
   }
   CK(cudaSetDevice(ctx->device));
   int nmax = 1;
-  bool want_order = false, want_ring = false, want_l8 = false;
+  bool want_order = clouds != nullptr, want_ring = false, want_l8 = false;
   for (int b = 0; b < batch; b++) {
     if (n[b] < 0 || (n[b] > 0 && !data[b])) return URF_ERR_INVALID;
     if (n[b] > ctx->max_points) return URF_ERR_CAPACITY;
@@ -618,19 +611,28 @@ int process_batch_impl(urf_ctx* ctx, const void* const* data, const int* n, int 
     want_l8 |= label8 && label8[b];
     ctx->h_n[b] = n[b];
   }
-  if (step != 0 && (!ctx->rawb || ctx->rawb_step < step)) {      // first use (or a wider record than before): P * step bytes
+  const int S = ((nmax + 255) / 256) * 256;
+  const int T = (S + kChunk - 1) / kChunk;
+  if ((size_t)batch * S * step > ctx->rawb_bytes) {            // records of a batch beyond the staging buffer: P * step bytes
     CK(cudaStreamSynchronize(ctx->stream));
     if (ctx->rawb) { cudaFree(ctx->rawb); ctx->allocs.erase(std::find(ctx->allocs.begin(), ctx->allocs.end(), (void*)ctx->rawb)); ctx->rawb = nullptr; }
+    ctx->rawb_bytes = 0;
     const int rc = dalloc(ctx, &ctx->rawb, ctx->P * (size_t)step);
     if (rc != URF_OK) return rc;
-    ctx->rawb_step = step;
+    ctx->rawb_bytes = ctx->P * (size_t)step;
   }
   if (want_l8 && !ctx->label8) {
     const int rc = dalloc(ctx, &ctx->label8, ctx->P);
     if (rc != URF_OK) return rc;
   }
-  const int S = ((nmax + 255) / 256) * 256;
-  const int T = (S + kChunk - 1) / kChunk;
+  if (clouds && !ctx->pack) {                                  // first packed call: 96 bytes per point of capacity
+    const int tiles = (std::max(ctx->max_points, 1) + kPackTile - 1) / kPackTile;
+    int rc = dalloc(ctx, &ctx->pack, (size_t)6 * ctx->max_points);
+    if (rc == URF_OK) rc = dalloc(ctx, &ctx->packcnt, (size_t)3 * tiles);
+    if (rc == URF_OK) rc = dalloc(ctx, &ctx->packtot, 4);
+    if (rc != URF_OK) { ctx->pack = nullptr; return rc; }
+    CK(cudaMallocHost((void**)&ctx->h_packtot, sizeof(int) * 4));
+  }
   cudaStream_t st = ctx->stream;
   DevBuffers bufv = ctx->buf;
   bufv.label8 = want_l8 ? ctx->label8 : nullptr;
@@ -652,7 +654,11 @@ int process_batch_impl(urf_ctx* ctx, const void* const* data, const int* n, int 
     ctx->ev_in.push_back(a); ctx->ev_comp.push_back(c);
   }
   int* ring32 = reinterpret_cast<int*>(ctx->buf.sortbuf);     // free once the sorts of a chunk are done (chunk-private slice)
-  const bool graphed = nchunks == 1 && batch <= 8 && !want_l8;
+  const bool graphed = nchunks == 1 && batch <= 8 && !want_l8 && ctx->use_graph && !ctx->profile;
+  if (graphed) {
+    const int rc = update_graph(ctx, batch, S, want_order);
+    if (rc != URF_OK) return rc;
+  }
   // every host-to-device copy of the call is queued first (the copies depend on nothing): the copy engine then never waits
   // for this thread to get through a chunk's kernel launches and result copies
   for (int c = 0; c < nchunks; c++) {
@@ -665,6 +671,7 @@ int process_batch_impl(urf_ctx* ctx, const void* const* data, const int* n, int 
     }
     CK(cudaEventRecord(ctx->ev_in[c], ctx->s_in));
   }
+  int launches = 0;
   for (int c = 0; c < nchunks; c++) {
     const int b0 = cb[c], nb = cb[c + 1] - b0;
     CK(cudaStreamWaitEvent(st, ctx->ev_in[c], 0));
@@ -672,12 +679,27 @@ int process_batch_impl(urf_ctx* ctx, const void* const* data, const int* n, int 
       k_unpack_cloud2_batch<<<dim3((S + 255) / 256, nb), 256, 0, st>>>(ctx->rawb + (size_t)b0 * S * step, ctx->own_in + (size_t)b0 * S, ctx->buf.n + b0, S,
                                                                           step, ox, oy, oz, oi);
     const DevBuffers view = offset_view(bufv, b0, S, T, ctx->dp.channels);
-    int rc = graphed ? launch_pipeline_graphed(ctx, nb, S, want_order) : launch_pipeline(ctx, view, nb, S, want_order, c == 0, c == nchunks - 1);
+    // ev0 / ev1 bracket the kernels of the whole call: before the first chunk's pipeline, after the last one's
+    int L = graphed ? ctx->g_launches : 0;
+    int rc = c == 0 ? cuda_rc(ctx, cudaEventRecord(ctx->ev0, st), "cudaEventRecord(ev0)") : URF_OK;
+    if (rc == URF_OK)
+      rc = graphed ? cuda_rc(ctx, cudaGraphLaunch(ctx->gexec, st), "cudaGraphLaunch") : launch_pipeline(ctx, view, nb, S, want_order, urf_ctx::kGroups, &L);
+    if (rc == URF_OK && c == nchunks - 1) rc = cuda_rc(ctx, cudaEventRecord(ctx->ev1, st), "cudaEventRecord(ev1)");
     if (rc != URF_OK) {                                 // nothing of this call may still be writing into the caller's buffers
       cudaStreamSynchronize(ctx->s_in); cudaStreamSynchronize(st); cudaStreamSynchronize(ctx->s_out);
       return rc;
     }
+    launches += L;
     if (want_ring) k_ring32<<<dim3((S + 255) / 256, nb), 256, 0, st>>>(view, ring32 + (size_t)b0 * S * 4, S);
+    if (clouds) {                                       // batch == 1: pack scan 0, sizes to the host with the results
+      const int nt = (std::max(n[0], 1) + kPackTile - 1) / kPackTile;
+      k_pack_count<<<nt, 256, 0, st>>>(ctx->buf, ctx->packcnt, nt);
+      k_pack_scan<<<1, 1024, 0, st>>>(ctx->buf, ctx->packcnt, nt, ctx->packtot);
+      k_pack_write<<<nt, 256, 0, st>>>(ctx->buf, ctx->packcnt, nt, ctx->packtot, ctx->pack, ctx->pack + 2 * (size_t)ctx->max_points,
+                                       ctx->pack + 4 * (size_t)ctx->max_points);
+      launches += 3;
+      CK(cudaMemcpyAsync(ctx->h_packtot, ctx->packtot, sizeof(int) * 4, cudaMemcpyDeviceToHost, st));
+    }
     CK(cudaEventRecord(ctx->ev_comp[c], st));
     CK(cudaStreamWaitEvent(ctx->s_out, ctx->ev_comp[c], 0));
     CK(cudaMemcpyAsync(ctx->h_out + b0, ctx->buf.out + b0, sizeof(ScanOut) * nb, cudaMemcpyDeviceToHost, ctx->s_out));
@@ -691,79 +713,9 @@ int process_batch_impl(urf_ctx* ctx, const void* const* data, const int* n, int 
   }
   CK(cudaStreamSynchronize(ctx->s_out));
   CK(cudaStreamSynchronize(st));
-  ctx->last_B = batch; ctx->last_S = S;
-  for (int b = 0; b < batch; b++) {
-    fill_result(ctx->h_out[b], &outs[b]);
-    if (outs[b].status == URF_TOO_FEW_POINTS && outs[b].ring) for (int i = 0; i < n[b]; i++) outs[b].ring[i] = -1;
-  }
-  return URF_OK;
-}
-}  // namespace
-
-int urf_process_batch(urf_ctx* ctx, const float* const* xyzi, const int* n, int batch, urf_result* outs) {
-  return process_batch_impl(ctx, reinterpret_cast<const void* const*>(xyzi), n, batch, 0, 0, 0, 0, -1, outs, nullptr);
-}
-
-int urf_process_batch_xyz(urf_ctx* ctx, const float* const* xyz, const int* n, int batch, urf_result* outs, int8_t* const* label8) {
-  return process_batch_impl(ctx, reinterpret_cast<const void* const*>(xyz), n, batch, 12, 0, 4, 8, -1, outs, label8);
-}
-
-int urf_process_cloud2_batch(urf_ctx* ctx, const void* const* data, const int* n_points, int batch, int point_step, int off_x, int off_y,
-                             int off_z, int off_intensity, urf_result* outs, int8_t* const* label8) {
-  if (point_step == 0) return URF_ERR_INVALID;
-  return process_batch_impl(ctx, data, n_points, batch, point_step, off_x, off_y, off_z, off_intensity, outs, label8);
-}
-
-namespace {
-// Shared body of urf_process_cloud2 / urf_process_cloud2_packed: H2D of the raw records, unpack, pipeline, optional pack.
-int process_cloud2(urf_ctx* ctx, const void* data, int n, int point_step, int off_x, int off_y, int off_z, int off_i,
-                   urf_result* out, urf_clouds* clouds) {
-  if (!ctx || !out || n < 0 || (n > 0 && !data)) return URF_ERR_INVALID;
-  if (point_step < 12 || point_step > URF_MAX_POINT_STEP) return URF_ERR_INVALID;
-  for (int o : {off_x, off_y, off_z}) if (o < 0 || o + 4 > point_step) return URF_ERR_INVALID;
-  if (off_i >= 0 && off_i + 4 > point_step) return URF_ERR_INVALID;
-  if (n > ctx->max_points) return URF_ERR_CAPACITY;
-  CK(cudaSetDevice(ctx->device));
-  const int tiles = (std::max(ctx->max_points, 1) + kPackTile - 1) / kPackTile;
-  if (clouds && !ctx->pack) {                                // first packed call: 96 bytes per point of capacity
-    int rc = dalloc(ctx, &ctx->pack, (size_t)6 * ctx->max_points);
-    if (rc == URF_OK) rc = dalloc(ctx, &ctx->packcnt, (size_t)3 * tiles);
-    if (rc == URF_OK) rc = dalloc(ctx, &ctx->packtot, 4);
-    if (rc != URF_OK) { ctx->pack = nullptr; return rc; }
-    CK(cudaMallocHost((void**)&ctx->h_packtot, sizeof(int) * 4));
-  }
-  const int S = ((std::max(n, 1) + 255) / 256) * 256;
-  cudaStream_t st = ctx->stream;
-  ctx->h_n[0] = n;
-  CK(cudaMemcpyAsync(ctx->buf.n, ctx->h_n, sizeof(int), cudaMemcpyHostToDevice, st));
-  if (n > 0) {
-    CK(cudaMemcpyAsync(ctx->raw, data, (size_t)n * point_step, cudaMemcpyHostToDevice, st));
-    k_unpack_cloud2<<<(n + 255) / 256, 256, 0, st>>>(ctx->raw, ctx->own_in, n, point_step, off_x, off_y, off_z, off_i);
-  }
-  const bool want_order = out->order != nullptr || clouds != nullptr;
-  int rc = launch_pipeline_graphed(ctx, 1, S, want_order);
-  if (rc != URF_OK) return rc;
-  int* ring32 = reinterpret_cast<int*>(ctx->buf.sortbuf);
-  if (out->ring) k_ring32<<<dim3((S + 255) / 256, 1), 256, 0, st>>>(ctx->buf, ring32, S);
-  float4 *d_rc = nullptr, *d_roi = nullptr, *d_prob = nullptr;
-  if (clouds) {
-    const int nt = (std::max(n, 1) + kPackTile - 1) / kPackTile;
-    d_rc = ctx->pack; d_roi = ctx->pack + 2 * (size_t)ctx->max_points; d_prob = ctx->pack + 4 * (size_t)ctx->max_points;
-    k_pack_count<<<nt, 256, 0, st>>>(ctx->buf, ctx->packcnt, nt);
-    k_pack_scan<<<1, 1024, 0, st>>>(ctx->buf, ctx->packcnt, nt, ctx->packtot);
-    k_pack_write<<<nt, 256, 0, st>>>(ctx->buf, ctx->packcnt, nt, ctx->packtot, d_rc, d_roi, d_prob);
-    ctx->launches += 3;
-    CK(cudaMemcpyAsync(ctx->h_packtot, ctx->packtot, sizeof(int) * 4, cudaMemcpyDeviceToHost, st));
-  }
-  CK(cudaMemcpyAsync(ctx->h_out, ctx->buf.out, sizeof(ScanOut), cudaMemcpyDeviceToHost, st));
-  if (n > 0) {
-    if (out->label) CK(cudaMemcpyAsync(out->label, ctx->own_label, sizeof(int) * (size_t)n, cudaMemcpyDeviceToHost, st));
-    if (out->ring) CK(cudaMemcpyAsync(out->ring, ring32, sizeof(int) * (size_t)n, cudaMemcpyDeviceToHost, st));
-    if (out->order) CK(cudaMemcpyAsync(out->order, ctx->buf.order, sizeof(int) * (size_t)n, cudaMemcpyDeviceToHost, st));
-  }
-  CK(cudaStreamSynchronize(st));
   if (clouds) {                                              // sizes are known now: copy exactly the records that exist
     const int* t = ctx->h_packtot;
+    const float4 *d_rc = ctx->pack, *d_roi = ctx->pack + 2 * (size_t)ctx->max_points, *d_prob = ctx->pack + 4 * (size_t)ctx->max_points;
     clouds->n_road = t[0]; clouds->n_curb = t[1]; clouds->n_roi = t[2]; clouds->n_road_probably = t[3];
     const size_t rec = sizeof(urf_point_xyzi);
     if (clouds->road && t[0] > 0) CK(cudaMemcpyAsync(clouds->road, d_rc, rec * t[0], cudaMemcpyDeviceToHost, st));
@@ -772,21 +724,41 @@ int process_cloud2(urf_ctx* ctx, const void* data, int n, int point_step, int of
     if (clouds->road_probably && t[3] > 0) CK(cudaMemcpyAsync(clouds->road_probably, d_prob, rec * t[3], cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
   }
-  ctx->last_B = 1; ctx->last_S = S;
-  fill_result(ctx->h_out[0], out);
-  if (out->status == URF_TOO_FEW_POINTS && out->ring) for (int i = 0; i < n; i++) out->ring[i] = -1;
+  ctx->launches = launches;
+  ctx->timing_valid = true;
+  ctx->last_B = batch; ctx->last_S = S;
+  for (int b = 0; b < batch; b++) {
+    fill_result(ctx->h_out[b], &outs[b], true);
+    if (outs[b].status == URF_TOO_FEW_POINTS && outs[b].ring) for (int i = 0; i < n[b]; i++) outs[b].ring[i] = -1;
+  }
   return URF_OK;
 }
 }  // namespace
 
+int urf_process_batch(urf_ctx* ctx, const float* const* xyzi, const int* n, int batch, urf_result* outs) {
+  return process_batch_impl(ctx, reinterpret_cast<const void* const*>(xyzi), n, batch, 0, 0, 0, 0, -1, outs, nullptr, nullptr);
+}
+
+int urf_process_batch_xyz(urf_ctx* ctx, const float* const* xyz, const int* n, int batch, urf_result* outs, int8_t* const* label8) {
+  return process_batch_impl(ctx, reinterpret_cast<const void* const*>(xyz), n, batch, 12, 0, 4, 8, -1, outs, label8, nullptr);
+}
+
+// the record entry points reject point_step 0 themselves: the body reads step 0 as float4 input
+int urf_process_cloud2_batch(urf_ctx* ctx, const void* const* data, const int* n_points, int batch, int point_step, int off_x, int off_y,
+                             int off_z, int off_intensity, urf_result* outs, int8_t* const* label8) {
+  if (point_step == 0) return URF_ERR_INVALID;
+  return process_batch_impl(ctx, data, n_points, batch, point_step, off_x, off_y, off_z, off_intensity, outs, label8, nullptr);
+}
+
 int urf_process_cloud2(urf_ctx* ctx, const void* data, int n, int point_step, int off_x, int off_y, int off_z, urf_result* out) {
-  return process_cloud2(ctx, data, n, point_step, off_x, off_y, off_z, -1, out, nullptr);
+  if (point_step == 0) return URF_ERR_INVALID;
+  return process_batch_impl(ctx, &data, &n, 1, point_step, off_x, off_y, off_z, -1, out, nullptr, nullptr);
 }
 
 int urf_process_cloud2_packed(urf_ctx* ctx, const void* data, int n, int point_step, int off_x, int off_y, int off_z,
                               int off_intensity, urf_result* out, urf_clouds* clouds) {
-  if (!clouds) return URF_ERR_INVALID;
-  return process_cloud2(ctx, data, n, point_step, off_x, off_y, off_z, off_intensity, out, clouds);
+  if (!clouds || point_step == 0) return URF_ERR_INVALID;
+  return process_batch_impl(ctx, &data, &n, 1, point_step, off_x, off_y, off_z, off_intensity, out, nullptr, clouds);
 }
 
 int urf_process(urf_ctx* ctx, const float* xyzi, int n, urf_result* out) {

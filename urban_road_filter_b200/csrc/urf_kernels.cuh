@@ -12,7 +12,7 @@
 //   -> k_ring_detect -> k_tab1 -> k_reach -> k_tab2 -> k_label (input order) -> k_markers1 (one CTA per scan; scans
 //   above 300,000 points: k_markers_grid<1> -> k_markers_grid<2> -> k_verts)
 //   [-> k_sort_rings when the emission order is requested]
-//   PointCloud2 entry points: k_unpack_cloud2 in front, k_pack_count -> k_pack_scan -> k_pack_write behind
+//   PointCloud2 entry points: k_unpack_cloud2_batch in front, k_pack_count -> k_pack_scan -> k_pack_write behind
 #pragma once
 #include <type_traits>
 
@@ -1976,22 +1976,14 @@ __global__ void __launch_bounds__(kSortThreads) k_sort_rings(DevBuffers buf, int
   if (tie) atomicOr(&out.flags, F_TIE_AZIMUTH);
 }
 
-// k_unpack_cloud2: PointCloud2 record -> (x, y, z, intensity) float4 (SURVEY.md §8 f1). Byte-wise loads when a field is
-// not 4-byte aligned (Velodyne's 22-byte records). off_i < 0: no intensity field, 0 is stored.
+// k_unpack_cloud2_batch: PointCloud2 record -> (x, y, z, intensity) float4 (SURVEY.md §8 f1) for a batch: scan
+// b = blockIdx.y, its records at raw + b * S * point_step, its points at dst + b * S. Byte-wise loads when a field is not
+// 4-byte aligned (Velodyne's 22-byte records). off_i < 0: no intensity field, 0 is stored.
 __device__ __forceinline__ float load_f32_unaligned(const unsigned char* p) {
   if ((reinterpret_cast<size_t>(p) & 3) == 0) return *reinterpret_cast<const float*>(p);
   const unsigned v = (unsigned)p[0] | ((unsigned)p[1] << 8) | ((unsigned)p[2] << 16) | ((unsigned)p[3] << 24);
   return __uint_as_float(v);
 }
-__global__ void __launch_bounds__(256) k_unpack_cloud2(const unsigned char* __restrict__ raw, float4* __restrict__ dst, int n,
-                                                        int point_step, int off_x, int off_y, int off_z, int off_i) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const unsigned char* rec = raw + (size_t)i * point_step;
-  dst[i] = make_float4(load_f32_unaligned(rec + off_x), load_f32_unaligned(rec + off_y), load_f32_unaligned(rec + off_z),
-                       off_i >= 0 ? load_f32_unaligned(rec + off_i) : 0.f);
-}
-// the same for a batch: scan b = blockIdx.y, its records at raw + b * S * point_step, its points at dst + b * S
 __global__ void __launch_bounds__(256) k_unpack_cloud2_batch(const unsigned char* __restrict__ raw, float4* __restrict__ dst,
                                                               const int* __restrict__ n, int S, int point_step, int off_x, int off_y,
                                                               int off_z, int off_i) {
