@@ -58,11 +58,11 @@ def kernel_bytes(c: dict, batch: int) -> dict:
         "k_register": ((ELEV_BINS + 1) * (4 + 2) + RING_KEYS * 12, "first-index bins, lookup table, ring tables"),
         "k_assign": (N * (4 + 2) + hist, "alpha 4 + ringid 2 per point, histogram rows"),
         "k_scan_offsets": (2 * hist, "histogram rows read and rewritten"),
-        "k_scatter": (N * (2 + 2 + 16) + O * 16 + R * 16 + hist,
-                      "ringid 2 + sect 2 + in 16 per point, bpt 16 per ring point, spt 16 per sector point, histogram rows"),
-        "k_star_sort": (R * (4 + 16 + 16), "radius key 4 + record gather 16 + ssorted 16 per sector point (whole sectors)"),
+        "k_scatter": (N * (2 + 2 + 16) + O * 16 + R * 12 + hist,
+                      "ringid 2 + sect 2 + in 16 per point, bpt 16 per ring point, sr + sz + sidx 12 per sector point, histogram rows"),
+        "k_star_sort": (R * (4 + 4 + 8 + 4), "sr 4 + sz gather 4 + ssrz 8 + ssl 4 per sector point (whole sectors)"),
         "k_star_sort_big": (0, "work list only (empty at the bench shapes)"),
-        "k_star_scan": (R * 16, "ssorted 16 per sector point (whole sectors)"),
+        "k_star_scan": (R * 8, "ssrz 8 per sector point (whole sectors)"),
         "k_star_refine": (0, "work list only"),
         "k_ring_detect4": (O * 16 + O * 1, "bpt 16 + mark 1 per ring point"),
         "k_tab1": (C * DEG_BINS * 8 * 2, "curb bins read, non-empty prefix counts"),

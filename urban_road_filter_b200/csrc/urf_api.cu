@@ -117,7 +117,8 @@ DevBuffers offset_view(const DevBuffers& a, int b0, int S, int T, int channels) 
   const size_t o = (size_t)b0 * S;
   v.in += o; v.label += o; v.order += o; v.n += b0; v.out += b0;
   if (v.label8) v.label8 += o;
-  v.alpha_v += o; v.mark += o; v.ringid += o; v.sect += o; v.bpt += o; v.spt += o; v.ssorted += o;
+  v.alpha_v += o; v.mark += o; v.ringid += o; v.sect += o; v.bpt += o;
+  v.sr += o; v.sz += o; v.sidx += o; v.ssrz += o; v.ssl += o;
   v.az += o; v.d2 += o; v.baz += o; v.roadlist += o; v.roadcnt += (size_t)b0 * ((S + 31) >> 5); v.sortbuf += 2 * o;
   v.Tf += (size_t)b0 * channels * kTStride; v.Tb += (size_t)b0 * channels * kTStride;
   v.lut += (size_t)b0 * (kElevBins + 1); v.firstidx += (size_t)b0 * (kElevBins + 1);
@@ -329,8 +330,11 @@ int urf_create(urf_ctx** out, int device, int max_points, int max_batch) {
   TRY(dalloc(ctx, &b.sect, P));
   TRY(dalloc(ctx, &ctx->own_label, P));
   TRY(dalloc(ctx, &b.bpt, P));
-  TRY(dalloc(ctx, &b.spt, P));
-  TRY(dalloc(ctx, &b.ssorted, P));
+  TRY(dalloc(ctx, &b.sr, P));
+  TRY(dalloc(ctx, &b.sz, P));
+  TRY(dalloc(ctx, &b.sidx, P));
+  TRY(dalloc(ctx, &b.ssrz, P));
+  TRY(dalloc(ctx, &b.ssl, P));
   TRY(dalloc(ctx, &b.az, P));
   TRY(dalloc(ctx, &b.d2, P));
   TRY(dalloc(ctx, &b.baz, P));
@@ -785,7 +789,8 @@ int urf_test_math(int device, int which, const float* a, const float* b, float* 
 // Copy a device-side intermediate of scan `b` of the last call into host memory (stage-level differential tests).
 //   what: 0 alpha_v[f32,n]  1 mark[u8,n] (all detectors)  2 ringid[i16,n]  3 sect[i16,n]  4 az[f32,n]  5 d2[f32,n]
 //         (4, 5: defined for ROI points only)  8 ScanTab (raw)  9 star sort work lists [i32,2]: sectors handed to the
-//         eight-warp sort (nbig) and to the exact fallback (nslow)
+//         eight-warp sort (nbig) and to the exact fallback (nslow)  10 sectors completed by k_star_refine [i32,1]
+//         (nrefine: their edge search ran off the near-first prefix)
 int urf_debug_fetch(urf_ctx* ctx, int b, int what, void* dst, size_t bytes) {
   if (!ctx || !dst || b < 0 || b >= ctx->last_B) return URF_ERR_INVALID;
   CK(cudaSetDevice(ctx->device));
@@ -801,6 +806,7 @@ int urf_debug_fetch(urf_ctx* ctx, int b, int what, void* dst, size_t bytes) {
     case 5: src = ctx->buf.d2 + off; break;
     case 8: src = ctx->buf.tab + b; if (bytes > sizeof(ScanTab)) bytes = sizeof(ScanTab); break;
     case 9: src = &ctx->buf.tab[b].nbig; if (bytes > 2 * sizeof(int)) bytes = 2 * sizeof(int); break;
+    case 10: src = &ctx->buf.tab[b].nrefine; if (bytes > sizeof(int)) bytes = sizeof(int); break;
     default: return URF_ERR_INVALID;
   }
   CK(cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost));

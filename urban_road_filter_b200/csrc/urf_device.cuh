@@ -76,7 +76,7 @@ struct ScanTab {
   unsigned dmax[kDegBins];         // large scans (k_markers_grid): float bits of the farthest candidate road point
   unsigned long long best[kDegBins];                 // large scans: (ring, azimuth bits, input index) of the first candidate reaching dmax
   // near-first star sort (k_star_sort): only the points below a sampled pivot radius are sorted at first
-  int sorted_len[kSectKeys];       // length of the radius-sorted prefix of the sector in `ssorted` (== size when fully sorted)
+  int sorted_len[kSectKeys];       // length of the radius-sorted prefix of the sector in `ssrz` (== size when fully sorted)
   int nrefine, pad_;               // sectors whose edge search ran off the sorted prefix
   unsigned short refine[kSectKeys];
   float resume[kSectKeys][4];      // per refine entry: running mean, deviation, NaN count of the walk over the prefix, its length
@@ -92,8 +92,14 @@ struct DevBuffers {
   int* label;            // [P]   output labels, input order
   signed char* label8;   // [P] or NULL: the same labels as one byte per point (callers that ask for int8 labels)
   float4* bpt;           // [P]   ring buckets (ring-major, input order inside a ring): x, y, z, input index bits
-  float4* spt;           // [P]   sector buckets (unordered inside a sector): r, z, input index bits, -
-  float4* ssorted;       // [P]   sector buckets sorted by r
+  // sector buckets (unordered inside a sector), in sector-slot order: planar radius (the sort key), height, input index
+  float* sr;             // [P]
+  float* sz;             // [P]
+  unsigned* sidx;        // [P]
+  // sector buckets sorted by r: (r, z), all the edge search reads, and per sorted position the sector slot the point came
+  // from (network sorts) or its input index | 0x80000000 (exact fallback); star_input_index resolves either
+  float2* ssrz;          // [P]
+  unsigned* ssl;         // [P]
   float* az;             // [P]   azimuth per input point (ROI points only)
   float* d2;             // [P]   planar range per input point (ROI points only)
   uint2* baz;            // [P]   (azimuth bits, input index) per bucket position (written by k_scatter only when the emission order is wanted)
