@@ -236,7 +236,11 @@ void urf_pinned_free(void* p);
  * anyone else until urf_queue_destroy returns.
  */
 typedef struct urf_queue urf_queue;
-enum { URF_QUEUE_BLOCK = 0, URF_QUEUE_DROP_OLDEST = 1 };
+/* policy of urf_queue_create*: BLOCK or DROP_OLDEST, optionally OR-ed with URF_QUEUE_LABEL8 — int8 label slots (max_points
+ * bytes per slot instead of 4 * max_points; the worker fetches one-byte labels from the device, the int32 label copy is not
+ * issued). On such a queue urf_queue_next widens the labels into the caller's int32 buffer, urf_queue_next_view returns
+ * URF_ERR_INVALID (there is no int32 array to point at) and urf_queue_next_batch lends int8_t views. */
+enum { URF_QUEUE_BLOCK = 0, URF_QUEUE_DROP_OLDEST = 1, URF_QUEUE_LABEL8 = 2 };
 enum { URF_ERR_TIMEOUT = -6, URF_ERR_CLOSED = -7 };
 typedef struct urf_queue_stats {
   uint64_t submitted, processed, dropped, delivered, batches;
@@ -258,6 +262,18 @@ int urf_queue_next(urf_queue* q, uint64_t* tag, urf_result* out, int timeout_ms)
  * (NULL for a failed scan); the slot stays reserved until the consumer's next urf_queue_next / _next_view call on this queue
  * or urf_queue_release_view. out->label is ignored. One consumer thread at a time may hold a view. */
 int urf_queue_next_view(urf_queue* q, uint64_t* tag, urf_result* out, const int32_t** label_view, int timeout_ms);
+/* Batched delivery: one wake-up and one lock round for every scan that is ready, instead of one per scan. Waits up to
+ * timeout_ms (< 0: forever) until the oldest live scan is done, then lends out the run of consecutive finished scans that
+ * starts with it, in submission order, at most max_results of them (it never skips a scan that is not done yet; dropped
+ * scans are skipped as by urf_queue_next). Returns how many it lent (>= 1), or URF_ERR_TIMEOUT / URF_ERR_CLOSED as
+ * urf_queue_next. For scan j: tags[j], rcs[j] (URF_OK, or the error code of the batch the scan failed in), outs[j] (counts,
+ * flags and the n_vert vertices; pointer members set to NULL) and label_views[j], which points at the n_in labels inside
+ * the queue's slot — int8_t with URF_QUEUE_LABEL8, int32_t otherwise — or is NULL for a failed scan. tags, rcs and
+ * label_views may be NULL. Every lent slot stays reserved until the consumer's next urf_queue_next* call on this queue or
+ * urf_queue_release_view, so the views stay valid until then. */
+int urf_queue_next_batch(urf_queue* q, int max_results, uint64_t* tags, int32_t* rcs, urf_result* outs, const void** label_views,
+                         int timeout_ms);
+/* Gives back every slot lent by urf_queue_next_view / urf_queue_next_batch. */
 void urf_queue_release_view(urf_queue* q);
 int urf_queue_get_stats(urf_queue* q, urf_queue_stats* st);
 /* Stop accepting scans: blocked and later urf_queue_submit calls return URF_ERR_CLOSED; the worker still finishes what
@@ -280,7 +296,8 @@ int urf_queue_create_cloud2(urf_queue** out, urf_ctx* ctx, int max_points, int s
 int urf_queue_submit_cloud2(urf_queue* q, const void* data, int n_points, uint64_t tag, int timeout_ms);
 
 /* Test hook: the same queue around a caller-supplied batch function with urf_process_batch's signature (`user` is passed
- * as its ctx argument) and malloc'ed instead of pinned staging — the queue mechanics can then be exercised without a GPU. */
+ * as its ctx argument) and malloc'ed instead of pinned staging — the queue mechanics can then be exercised without a GPU.
+ * With URF_QUEUE_LABEL8 the function still writes int32 labels (outs[b].label); the queue narrows them into its int8 slots. */
 typedef int (*urf_queue_process_fn)(void* user, const float* const* xyzi, const int* n, int batch, urf_result* outs);
 int urf_queue_create_with(urf_queue** out, urf_queue_process_fn fn, void* user, int max_points, int slots, int max_batch,
                           int policy);
@@ -308,12 +325,22 @@ int urf_mq_submit(urf_mq* mq, const float* xyzi, int n, uint64_t tag, int timeou
 int urf_mq_submit_ref(urf_mq* mq, const float* xyzi, int n, uint64_t tag, int timeout_ms);
 int urf_mq_next(urf_mq* mq, uint64_t* tag, urf_result* out, int timeout_ms);
 int urf_mq_next_view(urf_mq* mq, uint64_t* tag, urf_result* out, const int32_t** label_view, int timeout_ms);   /* see urf_queue_next_view */
+/* urf_queue_next_batch over all devices: lends the run of finished scans at the front of the global order (one call may
+ * take scans from several devices, in the global order), at most max_results of them. Every lent slot, on whichever device,
+ * stays reserved until the consumer's next urf_mq_next* call. The mq lock is taken twice per call, whatever the count. */
+int urf_mq_next_batch(urf_mq* mq, int max_results, uint64_t* tags, int32_t* rcs, urf_result* outs, const void** label_views,
+                      int timeout_ms);
+/* urf_mq_create with int8 label slots on every device (URF_QUEUE_LABEL8; urf_mq_next_view then returns URF_ERR_INVALID). */
+int urf_mq_create_label8(urf_mq** out, const int* devices, int n_devices, int max_points, int slots_per_device, int max_batch,
+                         const urf_params* params /* or NULL: cfg defaults */);
 int urf_mq_get_stats(urf_mq* mq, urf_mq_stats* st);
 void urf_mq_close(urf_mq* mq);
 void urf_mq_destroy(urf_mq* mq);
 /* Test hook: N stand-in devices around a caller-supplied batch function (users[j] is passed to it for device j). */
 int urf_mq_create_with(urf_mq** out, urf_queue_process_fn fn, void* const* users, int n_devices, int max_points,
                        int slots_per_device, int max_batch);
+int urf_mq_create_with_label8(urf_mq** out, urf_queue_process_fn fn, void* const* users, int n_devices, int max_points,
+                              int slots_per_device, int max_batch);
 
 const char* urf_strerror(int code);
 /* Text of the last failed CUDA call of `ctx`; with ctx == NULL: why this thread's last urf_create failed. */

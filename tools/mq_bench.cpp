@@ -3,7 +3,12 @@
 // producer threads and one consumer, once with copying submits (memcpy into the device queue's pinned slot) and once by
 // reference (scans already in pinned memory, no host copy). Prints one JSON line per mode: scans/s and the host-side
 // limiter it points at. Host tool: links liburf_b200.so, no CUDA code of its own.
-//   usage: mq_bench <scans.bin> <points per scan> <n_scans_in_file> <n_devices> <producers> <total scans> <slots> <max_batch> [full_roi channels interval]
+//   usage: mq_bench <scans.bin> <points per scan> <n_scans_in_file> <n_devices> <producers> <total scans> <slots> <max_batch>
+//          [full_roi channels interval [modes max_results]]
+// modes: comma-separated subset of 0 (copying submit), 1 (by reference), 2 (by reference, labels viewed in place with
+// urf_mq_next_view), 3 (by reference, int8 label slots, results taken with urf_mq_next_batch, up to max_results per call);
+// default 0,1,2.
+#include <algorithm>
 #include <atomic>
 #include <chrono>
 #include <cstdio>
@@ -20,6 +25,9 @@ int main(int argc, char** argv) {
             mb = atoi(argv[8]);
   const int full_roi = argc > 9 ? atoi(argv[9]) : 1, channels = argc > 10 ? atoi(argv[10]) : 64;
   const double interval = argc > 11 ? atof(argv[11]) : 0.18;
+  std::vector<int> modes = {0, 1, 2};
+  if (argc > 12) { modes.clear(); for (const char* c = argv[12]; *c; c++) if (*c >= '0' && *c <= '3') modes.push_back(*c - '0'); }
+  const int max_results = argc > 13 ? atoi(argv[13]) : 64;
   const size_t bytes = (size_t)n * 16;
   std::vector<float*> pinned(K);
   FILE* f = fopen(path, "rb");
@@ -37,9 +45,10 @@ int main(int argc, char** argv) {
   if (full_roi) { prm.min_x = prm.min_y = prm.min_z = -200; prm.max_x = prm.max_y = prm.max_z = 200; }
   std::vector<int> devs(D);
   for (int d = 0; d < D; d++) devs[d] = d;
-  for (int mode = 0; mode < 3; mode++) {                          // 0: copying submit, 1: by reference (pinned), 2: 1 + labels viewed in place
+  for (int mode : modes) {                                        // 0: copying submit, 1: by reference (pinned), 2: 1 + labels viewed in place,
+                                                                  // 3: 1 + int8 slots delivered in runs (urf_mq_next_batch)
     urf_mq* mq = nullptr;
-    int rc = urf_mq_create(&mq, devs.data(), D, n, slots, mb, &prm);
+    int rc = mode == 3 ? urf_mq_create_label8(&mq, devs.data(), D, n, slots, mb, &prm) : urf_mq_create(&mq, devs.data(), D, n, slots, mb, &prm);
     if (rc != URF_OK) { fprintf(stderr, "urf_mq_create: %s (%s)\n", urf_strerror(rc), urf_last_cuda_error(nullptr)); return 1; }
     std::vector<int32_t> lab(n);
     std::atomic<long> road{0};
@@ -54,6 +63,22 @@ int main(int argc, char** argv) {
         }
       });
       std::thread cons([&] {
+        if (mode == 3) {
+          std::vector<uint64_t> tags(max_results);
+          std::vector<int32_t> rcs(max_results);
+          std::vector<urf_result> outs(max_results);
+          std::vector<const void*> views(max_results);
+          for (int i = 0; i < count;) {
+            const int k = urf_mq_next_batch(mq, std::min(max_results, count - i), tags.data(), rcs.data(), outs.data(), views.data(), -1);
+            if (k < 1) { fprintf(stderr, "next_batch: %s\n", urf_strerror(k)); exit(1); }
+            for (int j = 0; j < k; j++) {
+              if (rcs[j] != URF_OK) { fprintf(stderr, "next_batch: %s\n", urf_strerror(rcs[j])); exit(1); }
+              if (timed) road += outs[j].n_road;
+            }
+            i += k;
+          }
+          return;
+        }
         for (int i = 0; i < count; i++) {
           urf_result res; memset(&res, 0, sizeof(res)); res.label = lab.data();
           uint64_t tag;
@@ -75,7 +100,7 @@ int main(int argc, char** argv) {
     for (int d = 0; d < D; d++) { largest = st.largest_batch[d] > largest ? st.largest_batch[d] : largest; mn = st.submitted[d] < mn ? st.submitted[d] : mn; mx = st.submitted[d] > mx ? st.submitted[d] : mx; }
     printf("{\"mq_bench\": \"%s\", \"devices\": %d, \"producers\": %d, \"points_per_scan\": %d, \"scans\": %d, \"seconds\": %.4f, \"scans_per_sec\": %.1f, "
            "\"mpoints_per_sec\": %.1f, \"h2d_gb_per_sec\": %.2f, \"largest_batch\": %d, \"per_device_min_max\": [%llu, %llu], \"road_points\": %ld}\n",
-           mode == 2 ? "by_reference_pinned_labels_viewed_in_place" : mode ? "by_reference_pinned" : "copying_submit", D, P, n, total, s, total / s, total / s * n / 1e6, total / s * bytes / 1e9, largest, mn, mx,
+           mode == 3 ? "by_reference_pinned_label8_next_batch" : mode == 2 ? "by_reference_pinned_labels_viewed_in_place" : mode ? "by_reference_pinned" : "copying_submit", D, P, n, total, s, total / s, total / s * n / 1e6, total / s * bytes / 1e9, largest, mn, mx,
            road.load());
     fflush(stdout);
     urf_mq_destroy(mq);

@@ -10,12 +10,12 @@ import os
 import numpy as np
 
 from .ctypes_abi import (UrfMqStats, QUEUE_PROCESS_FN, URF_ERR_CLOSED, URF_ERR_TIMEOUT, URF_MAX_CHANNELS, URF_MAX_VERTS, URF_OK, URF_QUEUE_BLOCK,
-                         URF_QUEUE_DROP_OLDEST, URF_TOO_FEW_POINTS, UrfClouds, UrfParams, UrfQueueStats, UrfResult, UrfStrip,
-                         make_params)
+                         URF_QUEUE_DROP_OLDEST, URF_QUEUE_LABEL8, URF_TOO_FEW_POINTS, UrfClouds, UrfParams, UrfQueueStats, UrfResult,
+                         UrfStrip, make_params)
 
 LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "liburf_b200.so")
 
-EXPORTS = ["urf_queue_next_view", "urf_queue_release_view", "urf_mq_next_view", "urf_queue_submit_ref", "urf_queue_create_cloud2", "urf_queue_submit_cloud2", "urf_mq_create", "urf_mq_create_with",
+EXPORTS = ["urf_queue_next_batch", "urf_mq_next_batch", "urf_mq_create_label8", "urf_mq_create_with_label8", "urf_queue_next_view", "urf_queue_release_view", "urf_mq_next_view", "urf_queue_submit_ref", "urf_queue_create_cloud2", "urf_queue_submit_cloud2", "urf_mq_create", "urf_mq_create_with",
            "urf_mq_set_params", "urf_mq_submit", "urf_mq_submit_ref", "urf_mq_next", "urf_mq_get_stats", "urf_mq_close", "urf_mq_destroy",
            "urf_process_cloud2", "urf_process_cloud2_packed", "urf_pinned_alloc", "urf_pinned_free", "urf_queue_create",
            "urf_queue_create_with", "urf_queue_submit", "urf_queue_next", "urf_queue_get_stats", "urf_queue_close", "urf_queue_destroy",
@@ -94,6 +94,15 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
     lib.urf_mq_submit_ref.argtypes = [vp, vp, ip, C.c_uint64, ip]
     lib.urf_mq_next.argtypes = [vp, C.POINTER(C.c_uint64), C.POINTER(UrfResult), ip]
     lib.urf_mq_get_stats.argtypes = [vp, C.POINTER(UrfMqStats)]
+    lib.urf_mq_create_label8.argtypes = [C.POINTER(vp), C.POINTER(ip), ip, ip, ip, ip, C.POINTER(UrfParams)]
+    lib.urf_mq_create_with_label8.argtypes = [C.POINTER(vp), QUEUE_PROCESS_FN, C.POINTER(vp), ip, ip, ip, ip]
+    batch_args = [vp, ip, C.POINTER(C.c_uint64), C.POINTER(C.c_int32), C.POINTER(UrfResult), C.POINTER(vp), ip]
+    lib.urf_queue_next_batch.argtypes = batch_args
+    lib.urf_queue_next_view.argtypes = [vp, C.POINTER(C.c_uint64), C.POINTER(UrfResult), C.POINTER(vp), ip]
+    lib.urf_mq_next_view.argtypes = [vp, C.POINTER(C.c_uint64), C.POINTER(UrfResult), C.POINTER(vp), ip]
+    lib.urf_queue_release_view.argtypes = [vp]
+    lib.urf_queue_release_view.restype = None
+    lib.urf_mq_next_batch.argtypes = batch_args
     lib.urf_mq_close.argtypes = [vp]
     lib.urf_mq_close.restype = None
     lib.urf_mq_destroy.argtypes = [vp]
@@ -335,25 +344,73 @@ class Detector:
         return a[:count]
 
 
+class _BatchBuffers:
+    """Output arrays of urf_queue_next_batch / urf_mq_next_batch for up to `cap` scans, reused between calls."""
+
+    def __init__(self, cap: int):
+        self.cap = cap
+        self.tags = (C.c_uint64 * cap)()
+        self.rcs = (C.c_int32 * cap)()
+        self.outs = (UrfResult * cap)()
+        self.views = (C.c_void_p * cap)()
+
+    def results(self, k: int, label8: bool, copy: bool) -> list:
+        """(tag, ScanResult) of the k scans handed out. Labels are numpy views of the lent slots (int8 or int32) unless
+        `copy`; a scan whose batch failed has status = its (negative) error code and label None."""
+        ct = C.c_int8 if label8 else C.c_int32
+        out = []
+        for j in range(k):
+            res, rc = self.outs[j], int(self.rcs[j])
+            lab = None
+            if rc == URF_OK:
+                n = int(res.n_in)
+                lab = (np.ctypeslib.as_array(C.cast(self.views[j], C.POINTER(ct)), shape=(n,)) if n > 0
+                       else np.zeros(0, np.int8 if label8 else np.int32))
+                if copy:
+                    lab = lab.copy()
+            r = _scan_result(res, lab)
+            if rc != URF_OK:
+                r.status = rc
+            out.append((int(self.tags[j]), r))
+        return out
+
+
+def _next_batch(fn, handle, bufs: "_BatchBuffers | None", max_results: int, timeout_ms: int, label8: bool, copy: bool, where: str):
+    if max_results < 1:
+        raise ValueError("max_results must be >= 1")
+    if bufs is None or bufs.cap < max_results:
+        bufs = _BatchBuffers(max_results)
+    k = fn(handle, max_results, bufs.tags, bufs.rcs, bufs.outs, bufs.views, timeout_ms)
+    if k in (URF_ERR_TIMEOUT, URF_ERR_CLOSED):
+        return bufs, []
+    if k < 0:
+        raise UrfError(k, where)
+    return bufs, bufs.results(k, label8, copy)
+
+
 class MultiGpuQueue:
     """One ingest stream over several GPUs (include/urf.h urf_mq, BASELINE config 4): a context + streaming queue per device,
     every scan goes to the device with the fewest scans in flight, results come back in submission order. Any number of
     producer threads, one consumer. `by_reference` submits hand the array to the library without a copy: keep it alive and
-    unchanged until its result has come back."""
+    unchanged until its result has come back. label8: int8 label slots on every device (see ScanQueue)."""
 
     def __init__(self, devices, max_points: int, slots_per_device: int = 8, max_batch: int = 4, params: UrfParams | None = None,
-                 process_fn=None):
+                 process_fn=None, label8: bool = False):
         self.lib = load_library()
         self._m = C.c_void_p()
         self.max_points = max_points
+        self.label8 = label8
         self._cb = None
+        self._bufs = None
         if process_fn is not None:                      # tests: stand-in devices, no GPU
             self._cb = QUEUE_PROCESS_FN(process_fn)
-            rc = self.lib.urf_mq_create_with(C.byref(self._m), self._cb, None, len(devices), max_points, slots_per_device, max_batch)
+            create = self.lib.urf_mq_create_with_label8 if label8 else self.lib.urf_mq_create_with
+            rc = create(C.byref(self._m), self._cb, None, len(devices), max_points, slots_per_device, max_batch)
         else:
             dv = (C.c_int * len(devices))(*devices)
-            rc = self.lib.urf_mq_create(C.byref(self._m), dv, len(devices), max_points, slots_per_device, max_batch,
-                                        C.byref(params) if params is not None else None)
+            create = self.lib.urf_mq_create_label8 if label8 else self.lib.urf_mq_create
+            rc = create(C.byref(self._m), dv, len(devices), max_points, slots_per_device, max_batch,
+                        C.byref(params) if params is not None else None)
         if rc != URF_OK:
             raise UrfError(rc, "urf_mq_create", self.lib.urf_last_cuda_error(None).decode())
         self._keep = {}
@@ -388,6 +445,16 @@ class MultiGpuQueue:
         self._keep.pop(tag.value, None)
         return tag.value, _scan_result(res, lab[: res.n_in].copy())
 
+    def next_batch(self, max_results: int, timeout_ms: int = -1, copy: bool = False) -> list:
+        """[(tag, ScanResult)] of the run of finished scans at the front of the global order (urf_mq_next_batch), at most
+        max_results; [] on timeout / when the closed queue is drained. Labels are views of the lent slots (int8 with
+        label8), valid until the next next* call, unless `copy`. A scan whose batch failed has status < 0 and label None."""
+        self._bufs, out = _next_batch(self.lib.urf_mq_next_batch, self._m, self._bufs, max_results, timeout_ms, self.label8, copy,
+                                      "urf_mq_next_batch")
+        for t, _ in out:
+            self._keep.pop(t, None)
+        return out
+
     def stats(self) -> dict:
         st = UrfMqStats()
         self.lib.urf_mq_get_stats(self._m, C.byref(st))
@@ -407,15 +474,21 @@ class MultiGpuQueue:
 
 class ScanQueue:
     """Streaming ingest (include/urf.h urf_queue, SURVEY.md §8 f4): producers `submit` scans from any thread, one worker
-    thread batches whatever is pending through the detector, `next` returns results in submission order. With
-    `process_fn` (a Python callable with urf_process_batch's arguments) the queue runs without a GPU — tests only."""
+    thread batches whatever is pending through the detector, `next` returns results in submission order and `next_batch`
+    every result that is ready at once. With `process_fn` (a Python callable with urf_process_batch's arguments) the queue
+    runs without a GPU — tests only. label8: int8 label slots (URF_QUEUE_LABEL8) — a quarter of the label traffic and
+    memory; `next` still returns int32 labels, `next_batch` int8 ones."""
 
     def __init__(self, detector: "Detector | None", max_points: int, slots: int = 8, max_batch: int = 4,
-                 policy: int = URF_QUEUE_BLOCK, process_fn=None):
+                 policy: int = URF_QUEUE_BLOCK, process_fn=None, label8: bool = False):
         self.lib = load_library()
         self._q = C.c_void_p()
         self.max_points = max_points
+        self.label8 = label8
+        if label8:
+            policy |= URF_QUEUE_LABEL8
         self._cb = None
+        self._bufs = None
         if process_fn is not None:
             self._cb = QUEUE_PROCESS_FN(process_fn)
             rc = self.lib.urf_queue_create_with(C.byref(self._q), self._cb, None, max_points, slots, max_batch, policy)
@@ -446,6 +519,18 @@ class ScanQueue:
         if rc != URF_OK:
             raise UrfError(rc, "urf_queue_next")
         return int(tag.value), _scan_result(res, lab[: res.n_in].copy())
+
+    def next_batch(self, max_results: int, timeout_ms: int = -1, copy: bool = False) -> list:
+        """[(tag, ScanResult)] of the run of finished scans that starts with the oldest one (urf_queue_next_batch), at most
+        max_results; [] on timeout / when the closed queue is drained. Labels are views of the lent slots (int8 with
+        label8), valid until the next next* call, unless `copy`. A scan whose batch failed has status < 0 and label None."""
+        self._bufs, out = _next_batch(self.lib.urf_queue_next_batch, self._q, self._bufs, max_results, timeout_ms, self.label8, copy,
+                                      "urf_queue_next_batch")
+        return out
+
+    def release(self):
+        """Gives the slots lent by next_batch back before the next call (urf_queue_release_view)."""
+        self.lib.urf_queue_release_view(self._q)
 
     def stats(self) -> dict:
         st = UrfQueueStats()

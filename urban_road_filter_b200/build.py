@@ -14,7 +14,8 @@ NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-
               "-Xcompiler", "-fPIC"]
 SOURCES = ["urf_api.cu"]
 HOST_SOURCES = ["urf_markers.cpp", "urf_queue.cpp", "urf_mq.cpp"]
-HEADERS = ["urf_kernels.cuh", "urf_logic.cuh", "urf_device.cuh", "urf_math.cuh", "urf_stdsort.cuh", "urf_host.hpp"]
+HEADERS = ["urf_kernels.cuh", "urf_logic.cuh", "urf_device.cuh", "urf_math.cuh", "urf_stdsort.cuh", "urf_host.hpp",
+           "urf_queue_internal.hpp"]
 
 
 def _nvcc() -> str:
@@ -83,7 +84,13 @@ def build_kat() -> None:
     # ThreadSanitizer build of the streaming queue around a stand-in batch function (no CUDA involved)
     tgt = os.path.join(bdir, "queue_stress")
     qsrc = [os.path.join(kat, "queue_stress.cpp"), os.path.join(CSRC, "urf_queue.cpp"), os.path.join(CSRC, "urf_mq.cpp")]
-    if _stale(tgt, qsrc + [os.path.join(ROOT, "include", "urf.h")]):
+    qdeps = [os.path.join(ROOT, "include", "urf.h"), os.path.join(CSRC, "urf_queue_internal.hpp")]
+    if _stale(tgt, qsrc + qdeps):
+        subprocess.run(["g++", "-std=c++17", "-O1", "-g", "-fsanitize=thread", "-pthread", "-o", tgt, *qsrc], check=True)
+    # the same for batched delivery (urf_queue_next_batch / urf_mq_next_batch) and int8 label slots
+    tgt = os.path.join(bdir, "queue_batch_stress")
+    qsrc = [os.path.join(kat, "queue_batch_stress.cpp")] + qsrc[1:]
+    if _stale(tgt, qsrc + qdeps):
         subprocess.run(["g++", "-std=c++17", "-O1", "-g", "-fsanitize=thread", "-pthread", "-o", tgt, *qsrc], check=True)
 
 

@@ -8,9 +8,14 @@
 //   FREE -> FILLING (producer copies the scan, lock released) -> PENDING -> RUNNING (worker) -> DONE -> FREE (consumer)
 //   PENDING -> FREE when URF_QUEUE_DROP_OLDEST needs room (the scan is counted as dropped, never delivered).
 // Results are delivered in submission order: every accepted scan gets a sequence number when it becomes PENDING and the
-// consumer waits for the smallest live one.
+// consumer waits for the smallest live one. urf_queue_next_batch hands out the whole run of DONE slots that follows it.
+//
+// Label slots are int32, or int8 with URF_QUEUE_LABEL8: the worker then asks the batch body for one-byte labels (float4
+// queues go through urf_process_cloud2_batch with 16-byte records, which has the label8 output urf_process_batch lacks).
+#include <algorithm>
 #include <chrono>
 #include <condition_variable>
+#include <cstddef>
 #include <cstdlib>
 #include <cstring>
 #include <mutex>
@@ -18,6 +23,7 @@
 #include <vector>
 
 #include "../../include/urf.h"
+#include "urf_queue_internal.hpp"
 
 namespace {
 enum SlotState { FREE = 0, FILLING, PENDING, RUNNING, DONE, VIEWED };   // VIEWED: delivered, its labels lent to the consumer
@@ -27,7 +33,8 @@ struct Slot {
   int n = 0, rc = URF_OK;
   float* in = nullptr;       // max_points * bytes_per_point bytes (pinned for the real queue)
   const float* ext = nullptr;   // urf_queue_submit_ref: the caller's buffer is used in place (no copy)
-  int32_t* label = nullptr;  // max_points
+  int32_t* label = nullptr;  // max_points; NULL in a real URF_QUEUE_LABEL8 queue
+  int8_t* label8 = nullptr;  // max_points, URF_QUEUE_LABEL8 only
   urf_result res{};
 };
 }  // namespace
@@ -37,6 +44,7 @@ struct urf_queue {
   void* user = nullptr;
   bool pinned = false;
   int max_points = 0, max_batch = 1, policy = URF_QUEUE_BLOCK;
+  bool label8 = false;         // URF_QUEUE_LABEL8: int8 label slots
   // record format of the scans: step == 0: (x, y, z, intensity) float4 points; step > 0: raw PointCloud2 records of `step`
   // bytes (urf_queue_create_cloud2), handed to urf_process_cloud2_batch and unpacked on the device
   int step = 0, ox = 0, oy = 4, oz = 8, oi = -1;
@@ -45,7 +53,8 @@ struct urf_queue {
   std::mutex mu;
   std::condition_variable cv_free, cv_pending, cv_done;
   uint64_t next_seq = 1;       // sequence number of the next accepted scan
-  int viewed = -1;             // slot lent out by urf_queue_next_view, given back on the consumer's next call
+  std::vector<int> lent;       // slots lent out by urf_queue_next_view / _next_batch, given back on the consumer's next call
+  std::vector<std::pair<uint64_t, int>> live;   // consumer scratch (under mu): live slots in submission order
   bool closed = false;
   urf_queue_stats st{};
   std::thread worker;
@@ -68,6 +77,7 @@ void worker_loop(urf_queue* q) {
   std::vector<const float*> ptrs;
   std::vector<int> ns;
   std::vector<urf_result> outs;
+  std::vector<int8_t*> l8;
   for (;;) {
     idx.clear();
     {
@@ -93,15 +103,31 @@ void worker_loop(urf_queue* q) {
       if ((int)idx.size() > q->st.largest_batch) q->st.largest_batch = (int)idx.size();
     }
     const int B = (int)idx.size();
-    ptrs.resize(B); ns.resize(B); outs.assign(B, urf_result{});
+    ptrs.resize(B); ns.resize(B); l8.resize(B); outs.assign(B, urf_result{});
+    const bool stand_in = q->fn != real_process;
     for (int j = 0; j < B; j++) {
       Slot& s = q->slots[idx[j]];
       ptrs[j] = s.ext ? s.ext : s.in; ns[j] = s.n;
-      outs[j].label = s.label;
+      outs[j].label = s.label;                          // NULL in a real int8 queue: no int32 label copy is issued
+      l8[j] = s.label8;
     }
-    const int rc = q->step == 0 ? q->fn(q->user, ptrs.data(), ns.data(), B, outs.data())
-                                : urf_process_cloud2_batch(static_cast<urf_ctx*>(q->user), reinterpret_cast<const void* const*>(ptrs.data()), ns.data(), B,
-                                                           q->step, q->ox, q->oy, q->oz, q->oi, outs.data(), nullptr);
+    int rc;
+    if (stand_in) {
+      rc = q->fn(q->user, ptrs.data(), ns.data(), B, outs.data());
+      if (q->label8 && rc == URF_OK)                    // a stand-in writes int32 labels: the queue narrows them into the slot
+        for (int j = 0; j < B; j++) {
+          const Slot& s = q->slots[idx[j]];
+          for (int i = 0; i < s.n; i++) s.label8[i] = (int8_t)s.label[i];
+        }
+    } else if (q->step == 0 && !q->label8) {
+      rc = q->fn(q->user, ptrs.data(), ns.data(), B, outs.data());
+    } else {
+      // float4 scans with int8 labels are 16-byte records (x, y, z, intensity at 0, 4, 8, 12) to the record body
+      const bool f4 = q->step == 0;
+      rc = urf_process_cloud2_batch(static_cast<urf_ctx*>(q->user), reinterpret_cast<const void* const*>(ptrs.data()), ns.data(), B,
+                                    f4 ? 16 : q->step, f4 ? 0 : q->ox, f4 ? 4 : q->oy, f4 ? 8 : q->oz, f4 ? 12 : q->oi, outs.data(),
+                                    q->label8 ? l8.data() : nullptr);
+    }
     {
       std::lock_guard<std::mutex> lk(q->mu);
       for (int j = 0; j < B; j++) {
@@ -114,23 +140,35 @@ void worker_loop(urf_queue* q) {
   }
 }
 
+void free_slot(const urf_queue* q, Slot& s) {
+  for (void* p : {(void*)s.in, (void*)s.label, (void*)s.label8}) {
+    if (q->pinned) urf_pinned_free(p); else std::free(p);
+  }
+  s.in = nullptr; s.label = nullptr; s.label8 = nullptr;
+}
+
 int create_common(urf_queue** out, urf_queue_process_fn fn, void* user, bool pinned, int max_points, int slots, int max_batch, int policy,
                   int step = 0, int ox = 0, int oy = 4, int oz = 8, int oi = -1) {
+  const bool label8 = (policy & URF_QUEUE_LABEL8) != 0;
+  policy &= ~URF_QUEUE_LABEL8;
   if (!out || !fn || max_points < 1 || slots < 1 || max_batch < 1 || (policy != URF_QUEUE_BLOCK && policy != URF_QUEUE_DROP_OLDEST))
     return URF_ERR_INVALID;
   urf_queue* q = new urf_queue;
   q->fn = fn; q->user = user; q->pinned = pinned; q->max_points = max_points; q->max_batch = max_batch; q->policy = policy;
+  q->label8 = label8;
   q->step = step; q->ox = ox; q->oy = oy; q->oz = oz; q->oi = oi;
   q->bytes_per_point = step > 0 ? (size_t)step : 16;
   q->slots.resize(slots);
+  // int8 slots hold max_points bytes of labels; a stand-in batch function still writes int32 labels, which need a buffer
+  const bool want32 = !label8 || fn != real_process, want8 = label8;
+  auto alloc = [pinned](size_t bytes) { return pinned ? urf_pinned_alloc(bytes) : std::malloc(bytes); };
   for (Slot& s : q->slots) {
-    const size_t in_bytes = q->bytes_per_point * (size_t)max_points, lab_bytes = sizeof(int32_t) * (size_t)max_points;
-    s.in = static_cast<float*>(pinned ? urf_pinned_alloc(in_bytes) : std::malloc(in_bytes));
-    s.label = static_cast<int32_t*>(pinned ? urf_pinned_alloc(lab_bytes) : std::malloc(lab_bytes));
-    if (!s.in || !s.label) {
-      for (Slot& t : q->slots) {
-        if (pinned) { urf_pinned_free(t.in); urf_pinned_free(t.label); } else { std::free(t.in); std::free(t.label); }
-      }
+    const size_t in_bytes = q->bytes_per_point * (size_t)max_points;
+    s.in = static_cast<float*>(alloc(in_bytes));
+    if (want32) s.label = static_cast<int32_t*>(alloc(sizeof(int32_t) * (size_t)max_points));
+    if (want8) s.label8 = static_cast<int8_t*>(alloc((size_t)max_points));
+    if (!s.in || (want32 && !s.label) || (want8 && !s.label8)) {
+      for (Slot& t : q->slots) free_slot(q, t);
       delete q;
       return URF_ERR_NOMEM;
     }
@@ -236,38 +274,92 @@ int next_common(urf_queue* q, uint64_t* tag, urf_result* out, const int32_t** la
 int urf_queue_next(urf_queue* q, uint64_t* tag, urf_result* out, int timeout_ms) { return next_common(q, tag, out, nullptr, timeout_ms); }
 
 int urf_queue_next_view(urf_queue* q, uint64_t* tag, urf_result* out, const int32_t** label_view, int timeout_ms) {
-  if (!label_view) return URF_ERR_INVALID;
+  if (!label_view || (q && q->label8)) return URF_ERR_INVALID;         // int8 slots have no int32 view: urf_queue_next_batch
   return next_common(q, tag, out, label_view, timeout_ms);
 }
 
 namespace {
+// Gives the slots lent by the previous urf_queue_next_view / _next_batch call back to the producers (mu held).
+void release_lent(urf_queue* q) {
+  if (q->lent.empty()) return;
+  for (int i : q->lent) q->slots[i].state = FREE;
+  q->lent.clear();
+  q->cv_free.notify_all();
+}
+
+// The oldest live scan (smallest sequence number among PENDING / RUNNING / DONE slots): 1 and *slot when it is DONE,
+// 2 when the queue is closed and drained, 0 otherwise (mu held).
+int front_state(const urf_queue* q, int* slot) {
+  int best = -1;
+  bool filling = false;
+  for (int i = 0; i < (int)q->slots.size(); i++) {
+    const Slot& s = q->slots[i];
+    if (s.state == FILLING) filling = true;
+    if ((s.state == PENDING || s.state == RUNNING || s.state == DONE) && (best < 0 || s.seq < q->slots[best].seq)) best = i;
+  }
+  if (best >= 0 && q->slots[best].state == DONE) { *slot = best; return 1; }
+  if (best < 0 && !filling && q->closed) return 2;
+  return 0;
+}
+
+// Waits up to timeout_ms until the oldest live scan is done: URF_OK, URF_ERR_TIMEOUT or URF_ERR_CLOSED (mu held).
+int wait_front(urf_queue* q, std::unique_lock<std::mutex>& lk, int timeout_ms, int* slot) {
+  int state = 0;
+  if (!wait_for(q->cv_done, lk, timeout_ms, [&] { return (state = front_state(q, slot)) != 0; })) return URF_ERR_TIMEOUT;
+  return state == 2 ? (int)URF_ERR_CLOSED : (int)URF_OK;
+}
+
+// The run of DONE slots at the front, in submission order, at most max_results of them, into q->live (mu held).
+// A dropped scan's slot was reused and carries a new sequence number, so it is skipped like in urf_queue_next.
+int done_run(urf_queue* q, int max_results) {
+  q->live.clear();
+  for (int i = 0; i < (int)q->slots.size(); i++) {
+    const SlotState st = q->slots[i].state;
+    if (st == PENDING || st == RUNNING || st == DONE) q->live.emplace_back(q->slots[i].seq, i);
+  }
+  std::sort(q->live.begin(), q->live.end());
+  int k = 0;
+  while (k < (int)q->live.size() && k < max_results && q->slots[q->live[k].second].state == DONE) k++;
+  q->live.resize(k);
+  return k;
+}
+
+// Marks the k slots of q->live as lent (invisible to producers and the worker until release_lent) (mu held).
+void lend(urf_queue* q, int k) {
+  for (int j = 0; j < k; j++) { q->slots[q->live[j].second].state = VIEWED; q->lent.push_back(q->live[j].second); }
+  q->st.delivered += (uint64_t)k;
+}
+
+// The fields of a finished scan the consumer gets: counts and flags, and only the n_vert vertices that exist.
+void copy_result(urf_result* dst, const urf_result& src) {
+  std::memcpy(dst, &src, offsetof(urf_result, label));
+  dst->label = nullptr; dst->ring = nullptr; dst->order = nullptr; dst->ring_start = nullptr;
+  const int nv = std::min(std::max(src.n_vert, 0), URF_MAX_VERTS);
+  std::memcpy(dst->vert, src.vert, sizeof(src.vert[0]) * (size_t)nv);
+}
+
+// Hands out the slots lent by lend(): slot[j] goes to index dst ? dst[j] : j. Runs outside the lock (the slots are ours).
+void hand_out(const urf_queue* q, const int* slot, int k, const int* dst, uint64_t* tags, int32_t* rcs, urf_result* outs,
+              const void** label_views) {
+  for (int j = 0; j < k; j++) {
+    const Slot& s = q->slots[slot[j]];
+    const int o = dst ? dst[j] : j;
+    if (tags) tags[o] = s.tag;
+    if (rcs) rcs[o] = s.rc;
+    copy_result(&outs[o], s.res);
+    if (label_views) label_views[o] = s.rc != URF_OK ? nullptr : q->label8 ? (const void*)s.label8 : (const void*)s.label;
+  }
+}
+
 // label_view != NULL: no copy — *label_view points at the labels inside the queue's staging slot, which stays reserved
 // (not reusable by producers) until this consumer's next urf_queue_next* call on the queue.
 int next_common(urf_queue* q, uint64_t* tag, urf_result* out, const int32_t** label_view, int timeout_ms) {
   if (!q || !out) return URF_ERR_INVALID;
   std::unique_lock<std::mutex> lk(q->mu);
-  if (q->viewed >= 0) {                                   // the slot lent out by the previous view call comes back now
-    q->slots[q->viewed].state = FREE;
-    q->viewed = -1;
-    q->cv_free.notify_one();
-  }
+  release_lent(q);                                        // the slots lent out by the previous call come back now
   int slot = -1;
-  bool drained = false;
-  auto ready = [&] {
-    // the oldest live scan: smallest sequence number among PENDING / RUNNING / DONE slots
-    int best = -1;
-    bool filling = false;
-    for (int i = 0; i < (int)q->slots.size(); i++) {
-      const Slot& s = q->slots[i];
-      if (s.state == FILLING) filling = true;
-      if ((s.state == PENDING || s.state == RUNNING || s.state == DONE) && (best < 0 || s.seq < q->slots[best].seq)) best = i;
-    }
-    if (best >= 0 && q->slots[best].state == DONE) { slot = best; return true; }
-    if (best < 0 && !filling && q->closed) { drained = true; return true; }
-    return false;
-  };
-  if (!wait_for(q->cv_done, lk, timeout_ms, ready)) return URF_ERR_TIMEOUT;
-  if (drained) return URF_ERR_CLOSED;
+  const int wrc = wait_front(q, lk, timeout_ms, &slot);
+  if (wrc != URF_OK) return wrc;
   Slot& s = q->slots[slot];
   int32_t* user_label = out->label;
   const int rc = s.rc;
@@ -278,14 +370,16 @@ int next_common(urf_queue* q, uint64_t* tag, urf_result* out, const int32_t** la
   if (label_view) {                                       // lend the slot: DONE slots are invisible to producers and the worker
     *label_view = rc == URF_OK ? s.label : nullptr;
     s.state = VIEWED;
-    q->viewed = slot;
+    q->lent.push_back(slot);
     return rc;
   }
   const int n = s.n;
-  const int32_t* src = s.label;
   s.state = VIEWED;                                       // ours: invisible to producers, the worker and other consumers
   lk.unlock();                                            // the copy runs outside the lock
-  if (user_label && rc == URF_OK && n > 0) std::memcpy(user_label, src, sizeof(int32_t) * (size_t)n);
+  if (user_label && rc == URF_OK && n > 0) {
+    if (q->label8) for (int i = 0; i < n; i++) user_label[i] = s.label8[i];      // int8 slot: widened for the caller
+    else std::memcpy(user_label, s.label, sizeof(int32_t) * (size_t)n);
+  }
   lk.lock();
   s.state = FREE;
   lk.unlock();
@@ -294,10 +388,28 @@ int next_common(urf_queue* q, uint64_t* tag, urf_result* out, const int32_t** la
 }
 }  // namespace
 
+int urf_queue_next_batch(urf_queue* q, int max_results, uint64_t* tags, int32_t* rcs, urf_result* outs, const void** label_views,
+                         int timeout_ms) {
+  if (!q || !outs || max_results < 1) return URF_ERR_INVALID;
+  std::vector<int> idx;
+  {
+    std::unique_lock<std::mutex> lk(q->mu);               // the only lock round of the call
+    release_lent(q);
+    int front = -1;
+    const int wrc = wait_front(q, lk, timeout_ms, &front);
+    if (wrc != URF_OK) return wrc;
+    const int k = done_run(q, max_results);               // >= 1: the front is done
+    for (int j = 0; j < k; j++) idx.push_back(q->live[j].second);
+    lend(q, k);
+  }
+  hand_out(q, idx.data(), (int)idx.size(), nullptr, tags, rcs, outs, label_views);
+  return (int)idx.size();
+}
+
 void urf_queue_release_view(urf_queue* q) {
   if (!q) return;
   std::lock_guard<std::mutex> lk(q->mu);
-  if (q->viewed >= 0) { q->slots[q->viewed].state = FREE; q->viewed = -1; q->cv_free.notify_one(); }
+  release_lent(q);
 }
 
 int urf_queue_get_stats(urf_queue* q, urf_queue_stats* st) {
@@ -324,10 +436,35 @@ void urf_queue_destroy(urf_queue* q) {
   if (!q) return;
   urf_queue_close(q);
   if (q->worker.joinable()) q->worker.join();             // the worker drains what is pending before it returns
-  for (Slot& s : q->slots) {
-    if (q->pinned) { urf_pinned_free(s.in); urf_pinned_free(s.label); } else { std::free(s.in); std::free(s.label); }
-  }
+  for (Slot& s : q->slots) free_slot(q, s);
   delete q;
 }
 
 }  // extern "C"
+
+namespace urf_internal {
+
+int queue_done_run(urf_queue* q, int max_results, int timeout_ms) {
+  std::unique_lock<std::mutex> lk(q->mu);
+  release_lent(q);
+  int front = -1;
+  const int wrc = wait_front(q, lk, timeout_ms, &front);
+  if (wrc == URF_ERR_TIMEOUT && timeout_ms == 0) return 0;
+  if (wrc != URF_OK) return wrc;
+  return done_run(q, max_results);
+}
+
+int queue_lend_run(urf_queue* q, int count, const int* dst, uint64_t* tags, int32_t* rcs, urf_result* outs, const void** label_views) {
+  std::vector<int> idx;
+  {
+    std::lock_guard<std::mutex> lk(q->mu);
+    // a run that was done stays done (only this consumer takes scans out), so this is the run queue_done_run counted
+    const int k = done_run(q, count);
+    for (int j = 0; j < k; j++) idx.push_back(q->live[j].second);
+    lend(q, k);
+  }
+  hand_out(q, idx.data(), (int)idx.size(), dst, tags, rcs, outs, label_views);
+  return (int)idx.size();
+}
+
+}  // namespace urf_internal
