@@ -50,7 +50,7 @@ def kernel_bytes(c: dict, batch: int) -> dict:
     """{kernel: (bytes per step, what is counted)}"""
     N, R, O, D, C = c["n"], c["roi"], c["order"], c["road"], c["channels"]
     T = -(-int(N) // CHUNK)
-    hist = T * RING_KEYS * 4                           # per-chunk ring histograms of a scan
+    hist = T * C * 4                                   # per-chunk ring histograms of a scan: one counter per channel
     per_scan = {
         "k_reset": (RING_KEYS * 28 + DEG_BINS * 20 + SECT_KEYS * 4 + (ELEV_BINS + 1) * 4 + C * DEG_BINS * 8,
                     "per-scan tables, first-index bins, curb bins"),

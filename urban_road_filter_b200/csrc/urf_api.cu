@@ -30,7 +30,10 @@ struct urf_ctx {
   cudaStream_t s_side[kGroups + 1] = {};
   cudaEvent_t ev_sfork[kGroups + 1] = {}, ev_sjoin[kGroups + 1] = {};
   int sort_ctas = 0;                   // resident CTAs of k_star_sort on the whole device (its grid: the warps walk the sectors)
-  int groups = 2;                                 // H100 (400 W), C2 x 128, two runs: 1 stream 1.99 / 2.00 ms, 2 streams 1.95 / 2.06, 4 streams 2.11 / 2.02, 8 streams 2.07 / 2.14
+  // H100 (400 W), C2 x 128: 1 stream 1.628 ms (one run), 2 streams 1.630 (median of six); 3 and 4 streams slower (DESIGN.md §6).
+  // The groups do not hide each other's one-CTA-per-scan stages: descending stream priorities (1.683 ms) and a start
+  // staggered by one k_points (1.631) were tried and dropped
+  int groups = 2;
   // CUDA graph of the kernel sequence for small host-buffer batches (launch latency dominates there); re-captured when
   // the shape, the parameters or an option change
   bool use_graph = true;
@@ -111,7 +114,8 @@ __global__ void k_ring32(DevBuffers buf, int* dst, int S) {
 }
 
 // View of `buf` for the sub-batch that starts at scan b0: every per-scan array is advanced by b0 scans (S points of
-// stride, T histogram rows per scan), so each scan keeps its own slice of the input, the outputs and the workspace.
+// stride, T histogram rows of `channels` counters per scan), so each scan keeps its own slice of the input, the outputs
+// and the workspace.
 DevBuffers offset_view(const DevBuffers& a, int b0, int S, int T, int channels) {
   DevBuffers v = a;
   const size_t o = (size_t)b0 * S;
@@ -122,7 +126,7 @@ DevBuffers offset_view(const DevBuffers& a, int b0, int S, int T, int channels) 
   v.az += o; v.d2 += o; v.baz += o; v.roadlist += o; v.roadcnt += (size_t)b0 * ((S + 31) >> 5); v.sortbuf += 2 * o;
   v.Tf += (size_t)b0 * channels * kTStride; v.Tb += (size_t)b0 * channels * kTStride;
   v.lut += (size_t)b0 * (kElevBins + 1); v.firstidx += (size_t)b0 * (kElevBins + 1);
-  v.hist += (size_t)b0 * T * kRingKeys;
+  v.hist += (size_t)b0 * T * channels;
   v.cmin += (size_t)b0 * channels * kDegBins; v.cmax += (size_t)b0 * channels * kDegBins;
   v.ne += (size_t)b0 * channels * (kDegBins + 1);
   v.tab += b0;
@@ -159,7 +163,7 @@ int launch_pipeline(urf_ctx* ctx, const DevBuffers& buf, int B, int S, bool want
   K("k_points", k_points<<<gpts, 256, 0, st>>>(buf, dp, S));
   K("k_register", k_register<<<B, 256, 0, st>>>(buf, dp, S));
   K("k_assign", k_assign<<<gchunk, kWarpsPerBlock * 32, 0, st>>>(buf, dp, S, T));
-  K("k_scan_offsets", k_scan_offsets<<<B, 1024, 0, st>>>(buf, dp, S, T));   // + exact re-registration of refuted scans
+  K("k_scan_offsets", k_scan_offsets<<<B, kScanOffThreads, 0, st>>>(buf, dp, S, T));   // + exact re-registration of refuted scans
   K("k_scatter", k_scatter<<<dim3((T + kScatterWarps - 1) / kScatterWarps, B), kScatterWarps * 32, kScatterSmem, st>>>(buf, dp, S, T));
   // the ring detector next to the star-shaped search: both only read what k_scatter left and add curb hits (idempotent
   // marks, atomic min / max aggregates); k_tab1 is the first reader of the aggregates. Per-kernel timing keeps every

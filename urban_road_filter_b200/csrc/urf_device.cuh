@@ -110,7 +110,7 @@ struct DevBuffers {
   unsigned short* lut;   // [B][kElevBins + 1] ring-search start per fine elevation bin
   int* order;            // [P]   emission order (input indices), only when requested
   unsigned long long* sortbuf;   // [2P] scratch for segments too large for shared memory
-  unsigned* hist;        // [B][T][kRingKeys] per-chunk ring histograms, turned into scatter offsets in place
+  unsigned* hist;        // [B][T][channels] per-chunk ring histograms, turned into scatter offsets in place
   unsigned* firstidx;    // [B][kElevBins + 1] first input index per fine elevation bin
   unsigned* cmin;        // [B][channels][kDegBins] float bits: min curb azimuth per (ring, degree bin), +inf = empty
   unsigned* cmax;        // [B][channels][kDegBins] float bits: max curb azimuth per (ring, degree bin)

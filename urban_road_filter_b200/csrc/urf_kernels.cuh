@@ -313,8 +313,10 @@ __device__ __forceinline__ bool assign_chunk(const DevBuffers& buf, const DevPar
     }
   }
   __syncwarp();
-  unsigned* row = buf.hist + ((size_t)b * T + chunk) * kRingKeys;
-  for (int t = lane; t < kRingKeys; t += 32) row[t] = cnt[t];
+  // rows are `channels` counters wide: ring ids are below n_rings <= channels
+  const int C = prm.channels;
+  unsigned* row = buf.hist + ((size_t)b * T + chunk) * C;
+  for (int t = lane; t < C; t += 32) row[t] = cnt[t];
   return violation;
 }
 
@@ -340,15 +342,23 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32) k_assign(DevBuffers buf, 
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// k_scan_offsets: one CTA (1024 threads) per scan turns hist[chunk][ring] into exclusive scatter offsets (ring-major
-// bases + prefix over chunks), publishes ring_start, and turns the sector counts into sect_start + scatter cursors.
+// k_scan_offsets: one CTA per scan turns hist[chunk][ring] (rows of `channels` counters) into exclusive scatter offsets
+// (ring-major bases + prefix over chunks), publishes ring_start, and turns the sector counts into sect_start + scatter
+// cursors. Each warp owns a range of rows; a lane keeps kScanOffBatch rows of its column in flight. The ring bases and
+// the sector starts are CTA-wide scans with one ring and one sector per thread. 512 threads at no more than 64 registers
+// take at most half of an SM, so CTAs of the other stream groups run beside it.
 // In front of that it repairs a scan whose speculated registration k_assign refuted (F_SPEC_VIOLATION, rare): the exact
 // registration, then ring ids and chunk histograms of the whole scan again, one chunk per warp at a time.
-__global__ void __launch_bounds__(1024) k_scan_offsets(DevBuffers buf, DevParams prm, int S, int T) {
-  __shared__ unsigned s_part[32][kRingKeys];     // per-warp partial sums, then per-warp exclusive prefixes
+constexpr int kScanOffThreads = 512, kScanOffWarps = kScanOffThreads / 32;
+constexpr int kScanOffBatch = 16;
+static_assert(kRingKeys < kScanOffThreads && kSectKeys <= kScanOffThreads, "one ring_start entry and one sector per thread");
+__global__ void __launch_bounds__(kScanOffThreads, 2) k_scan_offsets(DevBuffers buf, DevParams prm, int S, int T) {
+  __shared__ unsigned s_part[kScanOffWarps][kRingKeys];     // per-warp partial sums, then per-warp exclusive prefixes
   __shared__ unsigned s_base[kRingKeys];
+  __shared__ unsigned s_wsum[2][kScanOffWarps];             // per-warp totals of the ring and sector scans
   const int b = blockIdx.x;
   const int n = buf.n[b];
+  const int C = prm.channels;
   const int rows = (n + kChunk - 1) / kChunk;
   const int warp = threadIdx.x >> 5, lane = lane_id();
   {
@@ -368,7 +378,7 @@ __global__ void __launch_bounds__(1024) k_scan_offsets(DevBuffers buf, DevParams
       publish_rings_cta(buf.tab[b], out, buf.lut + (size_t)b * (kElevBins + 1), prm.interval, s_reg, s_idx, s_m, s_keys, s_sorted);
       __syncthreads();                                                // s_sorted = the sorted angles, lut written
       const int R = s_m;
-      for (int c0 = 0; c0 < rows; c0 += 32) {
+      for (int c0 = 0; c0 < rows; c0 += kScanOffWarps) {
         for (int t = lane; t < kRingKeys; t += 32) s_part[warp][t] = 0;
         __syncwarp();
         if (c0 + warp < rows) assign_chunk(buf, prm, b, S, T, c0 + warp, n, true, false, s_sorted, nullptr, nullptr, R, lut, s_part[warp], lane);
@@ -378,39 +388,58 @@ __global__ void __launch_bounds__(1024) k_scan_offsets(DevBuffers buf, DevParams
       __syncthreads();                                                // the histogram rows are read back below
     }
   }
-  const int rpw = (rows + 31) / 32;
+  ScanTab& tab = buf.tab[b];
+  const unsigned scnt = threadIdx.x < kSectKeys ? (unsigned)tab.sect_cnt[threadIdx.x] : 0u;   // in flight during the row sums
+  const int rpw = (rows + kScanOffWarps - 1) / kScanOffWarps;
   const int r0 = min(rows, warp * rpw), r1 = min(rows, (warp + 1) * rpw);
-  unsigned* hist = buf.hist + (size_t)b * T * kRingKeys;
-  for (int key = lane; key < kRingKeys; key += 32) {
+  unsigned* hist = buf.hist + (size_t)b * T * C;
+  for (int key = lane; key < C; key += 32) {
     unsigned s = 0;
-    for (int r = r0; r < r1; r++) s += hist[(size_t)r * kRingKeys + key];
+    for (int r = r0; r < r1; r += kScanOffBatch) {
+      unsigned v[kScanOffBatch];
+#pragma unroll
+      for (int u = 0; u < kScanOffBatch; u++) v[u] = r + u < r1 ? hist[(size_t)(r + u) * C + key] : 0u;
+#pragma unroll
+      for (int u = 0; u < kScanOffBatch; u++) s += v[u];
+    }
     s_part[warp][key] = s;
   }
   __syncthreads();
-  if (threadIdx.x < kRingKeys) {
-    unsigned run = 0;
-    for (int w = 0; w < 32; w++) { unsigned v = s_part[w][threadIdx.x]; s_part[w][threadIdx.x] = run; run += v; }
-    s_base[threadIdx.x] = run;                  // total of this ring
+  unsigned rtot = 0;                              // total of ring threadIdx.x
+  if (threadIdx.x < C)
+    for (int w = 0; w < kScanOffWarps; w++) { const unsigned v = s_part[w][threadIdx.x]; s_part[w][threadIdx.x] = rtot; rtot += v; }
+  // CTA-wide exclusive scans of the ring totals (-> ring bases) and of the sector counts (-> sector starts)
+  unsigned xr = rtot, xs = scnt;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const unsigned ur = __shfl_up_sync(0xffffffffu, xr, d), us = __shfl_up_sync(0xffffffffu, xs, d);
+    if (lane >= d) { xr += ur; xs += us; }
   }
+  if (lane == 31) { s_wsum[0][warp] = xr; s_wsum[1][warp] = xs; }
   __syncthreads();
-  if (threadIdx.x == 0) {
-    unsigned run = 0;
-    ScanOut& o = buf.out[b];
-    for (int k = 0; k < kRingKeys; k++) { unsigned v = s_base[k]; s_base[k] = run; o.ring_start[k] = (int)run; run += v; }
-    o.ring_start[kRingKeys] = (int)run;
-    o.n_order = (int)run;
-  } else if (threadIdx.x == 32) {
-    ScanTab& t = buf.tab[b];
-    int run = 0;
-    for (int k = 0; k < kSectKeys; k++) { const int v = t.sect_cnt[k]; t.sect_start[k] = run; t.sect_cur[k] = run; run += v; }
-    t.sect_start[kSectKeys] = run;
+  unsigned all_r = 0, all_s = 0;
+#pragma unroll
+  for (int w = 0; w < kScanOffWarps; w++) {
+    const unsigned ur = s_wsum[0][w], us = s_wsum[1][w];
+    if (w < warp) { xr += ur; xs += us; }
+    all_r += ur; all_s += us;
   }
+  xr -= rtot; xs -= scnt;                         // exclusive
+  ScanOut& o = buf.out[b];
+  if (threadIdx.x < C) s_base[threadIdx.x] = xr;
+  if (threadIdx.x <= kRingKeys) o.ring_start[threadIdx.x] = (int)(threadIdx.x < C ? xr : all_r);
+  if (threadIdx.x < kSectKeys) { tab.sect_start[threadIdx.x] = (int)xs; tab.sect_cur[threadIdx.x] = (int)xs; }
+  if (threadIdx.x == 0) { o.n_order = (int)all_r; tab.sect_start[kSectKeys] = (int)all_s; }
   __syncthreads();
-  for (int key = lane; key < kRingKeys; key += 32) {
+  for (int key = lane; key < C; key += 32) {
     unsigned run = s_base[key] + s_part[warp][key];
-    for (int r = r0; r < r1; r++) {
-      unsigned* p = &hist[(size_t)r * kRingKeys + key];
-      unsigned v = *p; *p = run; run += v;
+    for (int r = r0; r < r1; r += kScanOffBatch) {
+      unsigned v[kScanOffBatch];
+#pragma unroll
+      for (int u = 0; u < kScanOffBatch; u++) v[u] = r + u < r1 ? hist[(size_t)(r + u) * C + key] : 0u;
+#pragma unroll
+      for (int u = 0; u < kScanOffBatch; u++)
+        if (r + u < r1) { hist[(size_t)(r + u) * C + key] = run; run += v[u]; }
     }
   }
 }
@@ -465,7 +494,7 @@ __global__ void __launch_bounds__(kScatterWarps * 32, 4) k_scatter(DevBuffers bu
   unsigned short* perm = s_perm[warp];
   ScanTab& tab = buf.tab[b];
   const bool live = chunk * kChunk < n;                           // a warp past the end only takes part in the barriers
-  const unsigned* row = buf.hist + ((size_t)b * T + chunk) * kRingKeys;
+  const unsigned* row = buf.hist + ((size_t)b * T + chunk) * prm.channels;
   const unsigned gb = scan_base(b, S), g0 = gb + (unsigned)chunk * kChunk;
   if (live && lane == 0) {                                        // clipped at the end of the scan
     mbar_init(&s_bar[warp], 1);
