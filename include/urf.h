@@ -127,7 +127,8 @@ typedef struct urf_ctx urf_ctx;
 void urf_default_params(urf_params* p);
 
 /* Create a context on CUDA device `device` able to process scans of up to max_points input points, up to max_batch
- * scans per urf_process_batch call. Replaces Detector::Detector + beam_init (lidar_segmentation.cpp:51-65). */
+ * scans per urf_process_batch call. Replaces Detector::Detector + beam_init (lidar_segmentation.cpp:51-65).
+ * max_points above 2^24 is URF_ERR_INVALID; max_batch above 65535 (the kernels' grid y limit) is URF_ERR_CAPACITY. */
 int urf_create(urf_ctx** out, int device, int max_points, int max_batch);
 void urf_destroy(urf_ctx* ctx);
 

@@ -83,8 +83,23 @@ class PortResult:
 
 
 class OracleDebug(C.Structure):
+    """struct urf_oracle_debug (oracle/urf_oracle.cpp): per-point arrays are indexed by input point, the rest per ring /
+    window start; NULL fields are not produced."""
     _fields_ = [("alpha_v", C.c_void_p), ("az", C.c_void_p), ("d2", C.c_void_p), ("star_mark", C.c_void_p),
-                ("det_label", C.c_void_p), ("ring_angle", C.c_void_p), ("max_dist", C.c_void_p)]
+                ("det_label", C.c_void_p), ("ring_angle", C.c_void_p), ("max_dist", C.c_void_p),
+                ("sector", C.c_void_p), ("q", C.c_void_p), ("A", C.c_void_p), ("reach", C.c_void_p)]
+
+    PER_POINT = ("alpha_v", "az", "d2", "star_mark", "det_label", "sector")
+
+    @staticmethod
+    def arrays(n: int) -> dict:
+        """Host arrays for every field, holding the fill value entries keep when their stage does not reach them."""
+        m = max(n, 1)
+        return dict(alpha_v=np.full(m, np.nan, np.float32), az=np.full(m, np.nan, np.float32), d2=np.full(m, np.nan, np.float32),
+                    star_mark=np.zeros(m, np.int8), det_label=np.full(m, -1, np.int8),
+                    ring_angle=np.full(URF_MAX_CHANNELS, np.nan, np.float32), max_dist=np.full(URF_MAX_CHANNELS, np.nan, np.float32),
+                    sector=np.full(m, -1, np.int16), q=np.full(4, np.nan, np.float32),
+                    A=np.full(URF_MAX_CHANNELS, np.nan, np.float64), reach=np.full((2, 361), -1, np.int32))
 
 
 class PortOracle:
@@ -110,11 +125,7 @@ class PortOracle:
         res = UrfResult()
         dbg = None
         if debug:
-            m = max(n, 1)
-            dbg_arrays = dict(alpha_v=np.full(m, np.nan, np.float32), az=np.full(m, np.nan, np.float32),
-                              d2=np.full(m, np.nan, np.float32), star_mark=np.zeros(m, np.int8),
-                              det_label=np.full(m, -1, np.int8), ring_angle=np.full(URF_MAX_CHANNELS, np.nan, np.float32),
-                              max_dist=np.full(URF_MAX_CHANNELS, np.nan, np.float32))
+            dbg_arrays = OracleDebug.arrays(n)
             dbg = OracleDebug(**{k: v.ctypes.data for k, v in dbg_arrays.items()})
         label = np.full(max(n, 1), -1, np.int32)
         ring = np.full(max(n, 1), -1, np.int32)
@@ -132,7 +143,7 @@ class PortOracle:
         r = PortResult()
         if debug:
             for k, v in dbg_arrays.items():
-                setattr(r, k, v[:n] if v.shape[0] == max(n, 1) and k not in ("ring_angle", "max_dist") else v)
+                setattr(r, k, v[:n] if k in OracleDebug.PER_POINT else v)
         r.status = res.status
         r.n_roi, r.n_rings, r.n_order = res.n_roi, res.n_rings, res.n_order
         r.n_road, r.n_curb, r.n_vert, r.flags = res.n_road, res.n_curb, res.n_vert, res.flags

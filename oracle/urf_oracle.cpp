@@ -30,6 +30,13 @@ struct urf_oracle_debug {
   int8_t* det_label;  // label after star/x-zero/z-zero, before blindSpots (ring-assigned points only)
   float* ring_angle;  // [URF_MAX_CHANNELS] sorted registered angles (:205)
   float* max_dist;    // [URF_MAX_CHANNELS] maxDistance per ring (:271-274)
+  // blindSpots / star-shaped search inputs (each may be NULL)
+  int16_t* sector;    // star sector of the point (star_shaped_search.cpp:164-173, after the wrap); -1 outside the ROI or
+                      // removed by the beam filter (:73-107); untouched when the star search is off
+  float* q;           // [4] q1..q4 (blind_spots.cpp:13-57)
+  double* A;          // [URF_MAX_CHANNELS] arcDistance / ((maxDistance[k] * M_PI) / 180) (:142), written for k >= 1
+  int* reach;         // [2][361] rings window start i accepted in the forward (:68-174) / backward (:177-283) loop:
+                      // 0 when ring 0 holds a curb point, n_rings when no ring does; -1 where the loop skips i or i is blind
 };
 
 namespace {
@@ -94,8 +101,9 @@ bool ptcmpr(const Polar& a, const Polar& b) { return a.r < b.r; }   // star_shap
 
 // star_shaped_search.cpp:155-181 + beamfunc :68-153. mark2D[i] := 2 for the <=360 detected points (ROI order).
 // Returns the number of sectors that hold an exact radius tie among their (filtered) points.
+// sector_out (or NULL): per ROI point its sector, -1 when the beam filter drops it.
 int star_shaped(const P& prm, const std::vector<float>& X, const std::vector<float>& Y, const std::vector<float>& Z,
-                std::vector<short>& mark2D) {
+                std::vector<short>& mark2D, std::vector<short>* sector_out = nullptr) {
   static Beam beams[360];
   static float Kfi = 0;
   static bool init = false;
@@ -111,6 +119,7 @@ int star_shaped(const P& prm, const std::vector<float>& X, const std::vector<flo
     if (f >= 360) f = 0;   // reference dereferences a null beamp[360] here (UB, SURVEY.md §7.4 H5); we wrap to sector 0
     if (f < 0) f = 0;
     sect[f].push_back(Polar{i, r});                           // :173
+    if (sector_out) (*sector_out)[i] = (short)f;
   }
   int tie_sectors = 0;
   for (int tid = 0; tid < 360; tid++) {
@@ -119,13 +128,16 @@ int star_shaped(const P& prm, const std::vector<float>& X, const std::vector<flo
       std::vector<Polar> kept;
       const Beam& b = beams[tid];
       for (const Polar& q : v) {
+        bool keep;
         if (b.yx) {
           float c = b.d * Y[q.id];                            // :79
-          if ((c - b.o) < X[q.id] && X[q.id] < (c + b.o)) kept.push_back(q);   // :80
+          keep = (c - b.o) < X[q.id] && X[q.id] < (c + b.o);  // :80
         } else {
           float c = b.d * X[q.id];                            // :95
-          if ((c - b.o) < Y[q.id] && Y[q.id] < (c + b.o)) kept.push_back(q);   // :96
+          keep = (c - b.o) < Y[q.id] && Y[q.id] < (c + b.o);  // :96
         }
+        if (keep) kept.push_back(q);
+        else if (sector_out) (*sector_out)[q.id] = -1;
       }
       v.swap(kept);
     }
@@ -258,7 +270,7 @@ void z_zero(const P& prm, std::vector<Ring>& rings) {
 
 // blind_spots.cpp:7-283. Bounded-loop form of the reference's `for (j = 0; alpha[j] <= hi && j < n; j++)` scans: the
 // reference reads alpha one element past the ring before testing j (zero-initialised storage, no effect on results).
-void blind_spots(const P& prm, std::vector<Ring>& rings, const std::vector<float>& maxDistance) {
+void blind_spots(const P& prm, std::vector<Ring>& rings, const std::vector<float>& maxDistance, const urf_oracle_debug* dbg) {
   const int index = (int)rings.size();
   float q1 = 0, q2 = 180, q3 = 180, q4 = 360;                     // :13
   if (prm.blind && index > 1) {                                    // :17-57 (ring index 1; empty when index < 2)
@@ -274,6 +286,10 @@ void blind_spots(const P& prm, std::vector<Ring>& rings, const std::vector<float
     }
   }
   float arcDistance = ((maxDistance[0] * M_PI) / 180) * prm.beamZone;   // :65
+  int* reach = dbg ? dbg->reach : nullptr;
+  if (dbg && dbg->q) { dbg->q[0] = q1; dbg->q[1] = q2; dbg->q[2] = q3; dbg->q[3] = q4; }
+  if (dbg && dbg->A) for (int k = 1; k < index; k++) dbg->A[k] = arcDistance / ((maxDistance[k] * M_PI) / 180);   // :142
+  if (reach) for (int t = 0; t < 2 * 361; t++) reach[t] = -1;
   auto is_blind = [&](int i) {                                     // :72-99 / :181-208
     if (!prm.blind) return false;
     if (prm.xDirection == 0)
@@ -289,9 +305,11 @@ void blind_spots(const P& prm, std::vector<Ring>& rings, const std::vector<float
     Ring& g0 = rings[0];
     for (int j = 0; j < g0.n() && g0.alpha[j] <= i + prm.beamZone; j++)            // :107
       if (g0.alpha[j] >= i && g0.label[j] == 2) { notRoad = 1; break; }
+    if (reach) reach[i] = 0;
     if (notRoad) continue;
     for (int j = 0; j < g0.n() && g0.alpha[j] <= i + prm.beamZone; j++)            // :124
       if (g0.alpha[j] >= i) g0.label[j] = 1;
+    if (reach) reach[i] = index;
     for (int k = 1; k < index; k++) {                                              // :133
       float currentDegree;
       if (i == 360 - prm.beamZone) currentDegree = 360;                            // :136-139
@@ -299,7 +317,7 @@ void blind_spots(const P& prm, std::vector<Ring>& rings, const std::vector<float
       Ring& g = rings[k];
       for (int l = 0; l < g.n() && g.alpha[l] <= currentDegree; l++)               // :146
         if (g.alpha[l] >= i && g.label[l] == 2) { notRoad = 1; break; }
-      if (notRoad) break;                                                          // :160
+      if (notRoad) { if (reach) reach[i] = k; break; }                             // :160
       for (int l = 0; l < g.n() && g.alpha[l] <= currentDegree; l++)               // :164
         if (g.alpha[l] >= i) g.label[l] = 1;
     }
@@ -311,9 +329,11 @@ void blind_spots(const P& prm, std::vector<Ring>& rings, const std::vector<float
     Ring& g0 = rings[0];
     for (int j = g0.n() - 1; j >= 0 && g0.alpha[j] >= i - prm.beamZone; --j)       // :216
       if (g0.alpha[j] <= i && g0.label[j] == 2) { notRoad = 1; break; }
+    if (reach) reach[361 + i] = 0;
     if (notRoad) continue;
     for (int j = g0.n() - 1; j >= 0 && g0.alpha[j] >= i - prm.beamZone; --j)       // :233
       if (g0.alpha[j] <= i) g0.label[j] = 1;
+    if (reach) reach[361 + i] = index;
     for (int k = 1; k < index; k++) {                                              // :242
       float currentDegree;
       if (i == 0 + prm.beamZone) currentDegree = 0;                                // :245-248
@@ -321,7 +341,7 @@ void blind_spots(const P& prm, std::vector<Ring>& rings, const std::vector<float
       Ring& g = rings[k];
       for (int l = g.n() - 1; l >= 0 && g.alpha[l] >= currentDegree; --l)          // :255
         if (g.alpha[l] <= i && g.label[l] == 2) { notRoad = 1; break; }
-      if (notRoad) break;
+      if (notRoad) { if (reach) reach[361 + i] = k; break; }
       for (int l = g.n() - 1; l >= 0 && g.alpha[l] >= currentDegree; --l)          // :273
         if (g.alpha[l] <= i) g.label[l] = 1;
     }
@@ -373,8 +393,10 @@ int run(const float* xyzi, int n_in, const urf_params* up, urf_result* out, cons
   // ---- star shaped search on ROI order, :199-200 ---------------------------------------------------------------------
   std::vector<short> mark2D(piece, 0);
   if (prm.star) {
-    int ties = star_shaped(prm, X, Y, Z, mark2D);
+    std::vector<short> sector(dbg && dbg->sector ? piece : 0);
+    int ties = star_shaped(prm, X, Y, Z, mark2D, dbg && dbg->sector ? &sector : nullptr);
     if (ties) out->flags |= 2;
+    if (dbg && dbg->sector) for (int i = 0; i < piece; i++) dbg->sector[rid[i]] = sector[i];
   }
 
   std::sort(angle.begin(), angle.begin() + index);                                 // :205
@@ -447,7 +469,7 @@ int run(const float* xyzi, int n_in, const urf_params* up, urf_result* out, cons
     apply_perm(g.alpha, perm); apply_perm(g.label, perm); apply_perm(g.id, perm);
   }
 
-  blind_spots(prm, rings, maxDistance);                                            // :293
+  blind_spots(prm, rings, maxDistance, dbg);                                       // :293
 
   // ---- marker candidate vertices, :298-351 ---------------------------------------------------------------------------
   int cM = 0;

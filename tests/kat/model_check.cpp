@@ -17,6 +17,7 @@ using namespace urf;
 
 struct urf_oracle_debug {   // same layout as oracle/urf_oracle.cpp
   float* alpha_v; float* az; float* d2; int8_t* star_mark; int8_t* det_label; float* ring_angle; float* max_dist;
+  int16_t* sector; float* q; double* A; int* reach;
 };
 
 namespace {
@@ -274,6 +275,12 @@ extern "C" int urf_model_run(const float* xyzi, int n, const urf_params* up, urf
           const unsigned short a = spm->st[dir][l - 1][i], c = j < kDegBins ? spm->st[dir][l - 1][j] : (unsigned short)0;
           spm->st[dir][l][i] = a > c ? a : c;
         }
+  }
+  if (dbg) {                  // the tables as k_points / k_tab1 / k_reach leave them on the device
+    if (dbg->sector && prm.star) for (int i = 0; i < n; i++) if (alpha[i] >= 0.0f) dbg->sector[i] = sect[i];
+    if (dbg->q) for (int w = 0; w < 4; w++) dbg->q[w] = tab.q[w];
+    if (dbg->A) for (int k = 1; k < R; k++) dbg->A[k] = tab.A[k];
+    if (dbg->reach) std::memcpy(dbg->reach, tab.reach, sizeof(tab.reach));
   }
 
   // ---- k_label (input order), k_dmax, k_best, k_verts

@@ -66,6 +66,18 @@ def test_no_gpu_means_error_not_fallback():
     assert e.value.code == -2
 
 
+def test_create_rejects_batches_beyond_the_grid_limit():
+    """Every kernel takes its scan from blockIdx.y (at most 65535): urf_create refuses a larger max_batch with
+    URF_ERR_CAPACITY before it touches a device, however small the scans."""
+    lib = api.load_library()
+    for max_batch in (65536, 65537, 1 << 20):
+        ctx = C.c_void_p()
+        assert lib.urf_create(C.byref(ctx), 0, 1, max_batch) == -5, max_batch
+        assert not ctx.value
+    if not torch.cuda.is_available():                  # 65535 passes the size checks and only then fails for want of a device
+        assert lib.urf_create(C.byref(C.c_void_p()), 0, 1, 65535) == -2
+
+
 def test_marker_tail_is_host_code():
     v = np.array([[1, 0, -1.8, 0], [2, 0, -1.8, 0], [3, 1, -1.8, 1], [4, 1, -1.7, 1], [5, 2, -1.8, 0], [6, 2, -1.8, 0]], np.float32)
     strips, ghost = api.build_markers(make_params(simple_poly_allow=0, poly_z_avg_allow=0), v, 5)

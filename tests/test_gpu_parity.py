@@ -12,7 +12,7 @@ from urban_road_filter_b200 import FULL_ROI, make_params
 from urban_road_filter_b200 import api
 from urban_road_filter_b200.synth import SHAPES, make_scan, random_cloud
 
-from util import Golden, assert_matches_golden, cloud2_records, golden_names, stage_diffs
+from util import GpuDebug, Golden, assert_matches_golden, cloud2_records, golden_names, stage_diffs
 
 pytestmark = pytest.mark.gpu
 
@@ -28,23 +28,6 @@ def det():
 @pytest.fixture(scope="module")
 def port():
     return PortOracle()
-
-
-class GpuDebug:
-    """Stage intermediates of scan 0 of the last call, re-indexed by input index like the oracle's debug run."""
-
-    def __init__(self, det, res, n):
-        N = res.n_order
-        self.__dict__.update(res.__dict__ if hasattr(res, "__dict__") else {s: getattr(res, s) for s in res.__slots__})
-        a = det.debug_fetch(0, 0, np.float32, n)
-        self.alpha_v = np.where(a < 0, np.nan, a).astype(np.float32)
-        ring = det.debug_fetch(0, 2, np.int16, n)
-        in_ring = ring >= 0
-        self.az = np.where(in_ring, det.debug_fetch(0, 4, np.float32, n), np.float32(np.nan)).astype(np.float32)
-        self.d2 = np.where(in_ring, det.debug_fetch(0, 5, np.float32, n), np.float32(np.nan)).astype(np.float32)
-        self.star_mark = None      # the device keeps one mark for all three detectors
-        self.det_label = np.where(in_ring, det.debug_fetch(0, 1, np.uint8, n).astype(np.int8), np.int8(-1)).astype(np.int8)
-        self.ring_angle = None
 
 
 def check(det, port, pts, prm, exact=False):

@@ -12,7 +12,8 @@ from urban_road_filter_b200 import FULL_ROI, make_params
 from urban_road_filter_b200.api import build_markers
 from urban_road_filter_b200.synth import SHAPES, make_scan, random_cloud
 
-from util import CpuModel, Golden, assert_matches_golden, golden_names, stage_diffs
+from util import (HUGE_ROI, SECTOR_RADII, CpuModel, Golden, assert_matches_golden, golden_names, random_param_case,
+                  sector_boundary_cloud, stage_diffs)
 
 
 @pytest.fixture(scope="module")
@@ -63,6 +64,29 @@ def test_model_random_clouds_and_exact_registration(both, seed):
     assert e.flags & 1
     assert np.array_equal(m.label, e.label)
     _check(both, random_cloud(20000, seed, rings=40), make_params())
+
+
+@pytest.mark.parametrize("starbeam", [0, 1])
+@pytest.mark.parametrize("r", SECTOR_RADII)
+def test_model_sector_boundaries(both, r, starbeam):
+    """Star sectors of points within a few ulps of every integer-degree boundary, of the fast path's 1e-3 degree margin,
+    on the axes (+-0.0), at the 0/360 wrap, subnormal and (under a +-3e38 ROI) beyond 2^126: the model's sector equals
+    the oracle's for every point, and so does everything downstream."""
+    port, model = both
+    for huge in (False, True):
+        pts = sector_boundary_cloud(r, seed=int(r * 10), huge=huge)
+        prm = make_params(starbeam_filter=starbeam, **(HUGE_ROI if huge else FULL_ROI))
+        o = port.run(pts, prm, debug=True)
+        assert o.status == 0 and (o.sector >= 0).sum() > pts.shape[0] // 3
+        _check(both, pts, prm)
+
+
+@pytest.mark.parametrize("seed", range(12))
+def test_model_random_parameter_cases(both, seed):
+    """Seeded draws over the parameter ranges (util.random_param_case; seeds 0-5 are also pinned against the unmodified
+    reference in test_oracle.py): every stage, including q1..q4, the ring widths and the window reach tables."""
+    pts, prm = random_param_case(seed)
+    _check(both, pts, prm)
 
 
 def test_model_speculation_failure_is_repaired(both):

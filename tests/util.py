@@ -49,6 +49,58 @@ def random_param_case(seed: int):
     return pts, prm
 
 
+HUGE_ROI = dict(min_x=-3e38, max_x=3e38, min_y=-3e38, max_y=3e38, min_z=-200.0, max_z=200.0)
+SECTOR_RADII = (0.3, 2.5, 19.0, 190.0)
+
+
+def _ulps(v, d):
+    """float32 v moved by d ulps (d may be negative), elementwise; crosses zero through the signed subnormals."""
+    v = np.asarray(v, np.float32)
+    i = v.view(np.int32).astype(np.int64)
+    o = np.where(i < 0, -(i & 0x7fffffff), i) + d                 # ordered integer: ... -1ulp, -0/+0, +1ulp ...
+    return np.where(o < 0, (-o) | (1 << 31), o).astype(np.uint32).view(np.float32)
+
+
+def sector_boundary_cloud(r: float, seed: int = 0, huge: bool = False) -> np.ndarray:
+    """Points on a flat ring (z = -1.7) at planar radius r that put the star sector (star_shaped_search.cpp:164-173) on
+    a knife edge: +-1..8 ulps of y (or x, whichever moves the angle more) around every integer-degree direction, around
+    k +- 1e-3 degrees (the margin of the fast sector path, urf_logic.cuh star_sector_fast) +-3 ulps, points on both axes
+    with +-0.0, at the 0/360 wrap (x > 0, y = -tiny) and with subnormal coordinates; with `huge`, points with |x| or
+    |y| above 2^126 (need HUGE_ROI). Seeded shuffle: no ring is in azimuth order."""
+    pts = []
+    deg = np.arange(360, dtype=np.float64)
+    for centre, spread in ((deg, range(-8, 9)), (deg + 1e-3, range(-3, 4)), (deg - 1e-3, range(-3, 4))):
+        th = np.deg2rad(centre)
+        x = (r * np.cos(th)).astype(np.float32)
+        y = (r * np.sin(th)).astype(np.float32)
+        along_y = np.abs(np.cos(th)) >= np.abs(np.sin(th))       # the angle is most sensitive to the smaller coordinate
+        for d in spread:
+            pts.append(np.stack([np.where(along_y, x, _ulps(x, d)), np.where(along_y, _ulps(y, d), y)], 1))
+    tiny = np.float32(1e-30)
+    sub = np.float32(1e-40)                                       # subnormal
+    s = np.float32(r)
+    special = [(s, 0.0), (s, -0.0), (-s, 0.0), (-s, -0.0), (0.0, s), (-0.0, s), (0.0, -s), (-0.0, -s),
+               (s, -tiny), (s, -sub), (s, sub), (s, -np.float32(1e-45)), (s, _ulps(np.float32(0.0), -1)),
+               (sub, sub), (-sub, sub), (sub, -sub), (-sub, -sub), (sub, np.float32(3e-41)), (np.float32(3e-41), -sub),
+               (sub, s * np.float32(1e-3)), (-s * np.float32(1e-3), -sub)]
+    pts.append(np.array(special, np.float32))
+    if huge:
+        big = np.float32(2.0 ** 126)
+        hp = []
+        for a, b in ((1.5, 0.01), (1.9, 1.3), (0.7, 1.99), (1.0, 1.0), (1.99, 1e-30), (3e-30, 1.7)):
+            for sx, sy in ((1, 1), (-1, 1), (-1, -1), (1, -1)):
+                hp.append((sx * a * big, sy * b * big))
+                hp.append((sy * b * big, sx * a * big))
+        hp += [(2.0 ** 127, 5.0), (-(2.0 ** 127), -5.0), (5.0, 2.0 ** 127), (-3.0, -(2.0 ** 127)), (1.5e38, 7.0)]
+        pts.append(np.array(hp, np.float32))
+    xy = np.concatenate(pts).astype(np.float32)
+    out = np.zeros((xy.shape[0], 4), np.float32)
+    out[:, :2] = xy
+    out[:, 2] = -1.7
+    out[:, 3] = 1.0
+    return out[np.random.default_rng(seed).permutation(out.shape[0])]
+
+
 _SCAN_CACHE: dict = {}
 
 
@@ -178,9 +230,7 @@ class CpuModel:
                  ring_start=np.zeros(URF_MAX_CHANNELS + 1, np.int32))
         for k, v in a.items():
             setattr(res, k, v.ctypes.data_as(C.POINTER(C.c_int32)))
-        d = dict(alpha_v=np.full(m, np.nan, np.float32), az=np.full(m, np.nan, np.float32), d2=np.full(m, np.nan, np.float32),
-                 star_mark=np.zeros(m, np.int8), det_label=np.full(m, -1, np.int8),
-                 ring_angle=np.full(URF_MAX_CHANNELS, np.nan, np.float32), max_dist=np.full(URF_MAX_CHANNELS, np.nan, np.float32))
+        d = OracleDebug.arrays(n)
         dbg = OracleDebug(**{k: v.ctypes.data for k, v in d.items()})
         rc = self.lib.urf_model_run(pts.ctypes.data, n, C.byref(prm), C.byref(res), C.byref(dbg), force_exact)
         assert rc == 0, rc
@@ -189,13 +239,60 @@ class CpuModel:
         r.__dict__.update(d)
         for f in ("status", "n_roi", "n_rings", "n_order", "n_road", "n_curb", "n_vert", "flags"):
             setattr(r, f, int(getattr(res, f)))
+        for k in OracleDebug.PER_POINT:
+            setattr(r, k, d[k][:n])
         r.label, r.ring, r.order = r.label[:n], r.ring[:n], r.order[: res.n_order]
         r.vert = np.ctypeslib.as_array(res.vert).reshape(URF_MAX_VERTS, 4)[: res.n_vert].copy()
         return r
 
 
+_K = URF_MAX_CHANNELS
+
+
+class ScanTab(C.Structure):
+    """ctypes mirror of urf::ScanTab (urban_road_filter_b200/csrc/urf_device.cuh): the per-scan tables, debug item 8."""
+    _fields_ = [("angle", C.c_float * _K), ("regidx", C.c_int * _K), ("regorder", C.c_int * _K), ("maxs", C.c_uint64 * _K),
+                ("maxdist", C.c_uint32 * _K), ("A", C.c_double * _K), ("sect_start", C.c_int * 361), ("sect_cnt", C.c_int * 360),
+                ("sect_cur", C.c_int * 360), ("nbig", C.c_int), ("nslow", C.c_int), ("biglist", C.c_uint16 * 360),
+                ("slowlist", C.c_uint16 * 360), ("q", C.c_float * 4), ("reach", (C.c_int * 361) * 2),
+                ("cutbest", C.c_uint64 * 361), ("dmax", C.c_uint32 * 361), ("best", C.c_uint64 * 361),
+                ("sorted_len", C.c_int * 360), ("nrefine", C.c_int), ("pad_", C.c_int), ("refine", C.c_uint16 * 360),
+                ("resume", (C.c_float * 4) * 360)]
+
+
+class GpuDebug:
+    """Stage intermediates of scan b of the detector's last call, re-indexed by input index like the oracle's debug run.
+    The device keeps one mark for all three detectors, so there is no star_mark of its own."""
+
+    def __init__(self, det, res, n, b=0):
+        self.__dict__.update(res.__dict__ if hasattr(res, "__dict__") else {s: getattr(res, s) for s in res.__slots__})
+        a = det.debug_fetch(b, 0, np.float32, n)
+        self.alpha_v = np.where(a < 0, np.nan, a).astype(np.float32)
+        in_ring = det.debug_fetch(b, 2, np.int16, n) >= 0
+        self.az = np.where(in_ring, det.debug_fetch(b, 4, np.float32, n), np.float32(np.nan)).astype(np.float32)
+        self.d2 = np.where(in_ring, det.debug_fetch(b, 5, np.float32, n), np.float32(np.nan)).astype(np.float32)
+        self.star_mark = None
+        self.det_label = np.where(in_ring, det.debug_fetch(b, 1, np.uint8, n).astype(np.int8), np.int8(-1)).astype(np.int8)
+        self.sector = det.debug_fetch(b, 3, np.int16, n)[:n]
+        size = det.lib.urf_debug_sizeof_tab()
+        assert size == C.sizeof(ScanTab), f"ScanTab mirror is {C.sizeof(ScanTab)} bytes, the library's {size}"
+        tab = ScanTab.from_buffer_copy(det.debug_fetch(b, 8, np.uint8, size).tobytes())
+        self.tab = tab
+        self.ring_angle = np.array(tab.angle, np.float32)
+        self.max_dist = np.array(tab.maxdist, np.uint32).view(np.float32)
+        self.q = np.array(tab.q, np.float32)
+        self.A = np.array(tab.A, np.float64)
+        self.reach = np.array(tab.reach, np.int32).reshape(2, 361)
+
+
 def stage_diffs(o, m, n: int, check_order: bool = True) -> list[str]:
-    """Names of the stages in which result m (model / GPU) differs from the oracle's debug run o."""
+    """Names of the stages in which result m (model / GPU) differs from the oracle's debug run o. Stages m does not
+    provide (attribute missing or None) are skipped.
+
+    reach: the oracle writes -1 for window starts its loops skip (outside the loop range, or blind). Those entries are
+    never read when labels are decided, and the device leaves them as it likes: k_tab1 sets every entry to n_rings,
+    k_reach then overwrites the starts inside the loop range, blind or not. Only the entries the oracle defines (>= 0)
+    are compared. A is compared for rings 1 .. n_rings - 1 (blind_spots.cpp:142 never uses A[0])."""
     bad = []
     if o.status != m.status:
         return ["status"]
@@ -204,16 +301,24 @@ def stage_diffs(o, m, n: int, check_order: bool = True) -> list[str]:
     for f in ("alpha_v", "az", "d2"):
         if getattr(m, f, None) is not None and not feq(getattr(o, f)[:n], getattr(m, f)[:n]):
             bad.append(f)
-    for f in ("star_mark", "det_label"):
+    for f in ("star_mark", "det_label", "sector"):
         if getattr(m, f, None) is not None and not np.array_equal(getattr(o, f)[:n], getattr(m, f)[:n]):
             bad.append(f)
-    if o.n_rings != m.n_rings:
+    if getattr(m, "q", None) is not None and not feq(o.q, m.q):
+        bad.append("q")
+    R = o.n_rings
+    if R != m.n_rings:
         bad.append("n_rings")
-    elif getattr(m, "ring_angle", None) is not None:
-        if not feq(o.ring_angle[: o.n_rings], m.ring_angle[: o.n_rings]):
-            bad.append("ring_angle")
-        if not feq(o.max_dist[: o.n_rings], m.max_dist[: o.n_rings]):
-            bad.append("max_dist")
+    else:
+        for f in ("ring_angle", "max_dist"):
+            if getattr(m, f, None) is not None and not feq(getattr(o, f)[:R], getattr(m, f)[:R]):
+                bad.append(f)
+        if getattr(m, "A", None) is not None and not np.array_equal(np.asarray(o.A[1:R]).view(np.uint64), np.asarray(m.A[1:R]).view(np.uint64)):
+            bad.append("A")
+        if getattr(m, "reach", None) is not None:
+            defined = o.reach >= 0
+            if not np.array_equal(o.reach[defined], m.reach[defined]):
+                bad.append("reach")
     if m.ring is not None and not np.array_equal(o.ring, m.ring):
         bad.append("ring")
     if not np.array_equal(o.label, m.label):
@@ -228,7 +333,7 @@ def stage_diffs(o, m, n: int, check_order: bool = True) -> list[str]:
             bad.append("azimuth_tie_flag")
         if not ties and not np.array_equal(o.order, m.order):
             bad.append("order")
-        if not np.array_equal(o.ring_start[: o.n_rings + 1], m.ring_start[: o.n_rings + 1]):
+        if getattr(m, "ring_start", None) is not None and not np.array_equal(o.ring_start[: o.n_rings + 1], m.ring_start[: o.n_rings + 1]):
             bad.append("ring_start")
     if not ties and (o.n_vert != m.n_vert or not feq(o.vert, m.vert)):
         bad.append("vert")

@@ -13,6 +13,8 @@
 
 using namespace urf;
 
+constexpr int kMaxBatch = 65535;   // scans per context: the largest grid y dimension
+
 struct urf_ctx {
   int device = 0;
   int max_points = 0;      // per scan, rounded up to kChunk
@@ -293,6 +295,7 @@ void urf_default_params(urf_params* p) {
 int urf_create(urf_ctx** out, int device, int max_points, int max_batch) {
   if (!out || max_points < 1 || max_batch < 1 || max_points > (1 << 24)) return URF_ERR_INVALID;
   if ((long long)(max_points + kChunk) * max_batch >= (1ll << 31)) return URF_ERR_CAPACITY;   // kernels use 32-bit offsets
+  if (max_batch > kMaxBatch) return URF_ERR_CAPACITY;          // every kernel takes its scan from blockIdx.y
   *out = nullptr;
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0 || device < 0 || device >= ndev) return URF_ERR_NO_DEVICE;
