@@ -44,5 +44,7 @@ sh = SHAPES["C5"]
 det = api.Detector(max_points=1_048_576, max_batch=1, params=make_params(channels=sh.channels, interval=sh.interval, **FULL_ROI))
 r5 = det.filtered(make_scan("C5", 0))
 assert r5.status == 0 and r5.n_vert > 0
+flat5 = make_scan("C5", 1).copy(); flat5[:, 2] = -1.8                           # sectors of ~2,900 points refined: k_star_refine's CTA loop
+assert det.filtered(flat5).status == 0
 det.close()
 print("ok")

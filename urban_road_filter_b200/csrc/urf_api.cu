@@ -394,8 +394,7 @@ int urf_create(urf_ctx** out, int device, int max_points, int max_batch) {
   urf_default_params(&ctx->params);
   const char* fe = std::getenv("URF_FORCE_EXACT_REGISTRATION");
   narrow_params(&ctx->params, &ctx->dp, ctx->dp.Kfi, fe && fe[0] == '1', 0);
-  const char* sp = std::getenv("URF_STAR_PREFIX");          // near-first star sort, on unless URF_STAR_PREFIX=0 (A/B measurements)
-  ctx->dp.star_prefix = !(sp && sp[0] == '0');
+  ctx->dp.star_prefix = 1;                                  // near-first star sort (option 4 turns it off)
   ctx->dp.star_pivot = 17;
 #undef TRY
 #undef CKF
