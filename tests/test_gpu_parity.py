@@ -12,6 +12,7 @@ from urban_road_filter_b200 import FULL_ROI, make_params
 from urban_road_filter_b200 import api
 from urban_road_filter_b200.synth import SHAPES, make_scan, random_cloud
 
+import tie_policy
 from util import GpuDebug, Golden, assert_matches_golden, cloud2_records, golden_names, stage_diffs
 
 pytestmark = pytest.mark.gpu
@@ -338,8 +339,9 @@ def test_gpu_radius_ties_take_the_reference_order(det, port):
         assert r.flags & 2 and m.flags & 2 and o.flags & 2
         assert np.array_equal(m.label, o.label), "CPU model of the tie path vs the oracle"
         assert np.array_equal(r.label, o.label) and np.array_equal(r.ring, o.ring)
-        if not (r.flags & 4):
-            assert np.array_equal(r.order, o.order) and np.array_equal(r.vert, o.vert)
+        p = tie_policy.policy(pts, port.run(pts, prm, debug=True))    # duplicates tie in azimuth too: the policy's order
+        assert bool(r.flags & 4) == p.tie
+        assert np.array_equal(r.order, p.order) and r.vert.tobytes() == p.vert.tobytes()
     # quantised ranges (what a real sensor delivers): a flat ring returns the same range in neighbouring columns
     pts = make_scan("C2", 12).copy()
     rng = np.linalg.norm(pts[:, :3], axis=1, keepdims=True)
@@ -350,6 +352,8 @@ def test_gpu_radius_ties_take_the_reference_order(det, port):
     r = det.filtered(pts)
     o = port.run(pts, prm)
     assert np.array_equal(r.label, o.label) and (r.flags & 2) == (o.flags & 2)
+    assert not (o.flags & 4) and not (r.flags & 4)                   # no azimuth tie: the port's order and vertices are the truth
+    assert np.array_equal(r.order, o.order) and r.vert.tobytes() == o.vert.tobytes()
 
 
 def test_gpu_device_resident_multi_stream_groups(port):
