@@ -217,8 +217,10 @@ extern "C" int urf_model_run(const float* xyzi, int n, const urf_params* up, urf
       const int idx = URF_F2I(ring[t].w);
       tab.maxs[k] = std::max(tab.maxs[k], planar_sum_bits(ring[t].x, ring[t].y));
       maxd_ref = std::max(maxd_ref, fbits(d2[idx]));
-      const bool hit = (prm.x_zero && xzero_mark(prm, ring, m, t, newY.data())) ||
-                       (prm.z_zero && (prm.curbPoints == 5 ? zzero_mark_t<5>(prm, ring, m, t) : zzero_mark_t<0>(prm, ring, m, t)));
+      // curb_points 5 runs the <5> instantiations, as k_ring_detect4 does; every other value the <0> ones of k_ring_detect
+      const bool hit = prm.curbPoints == 5
+          ? (prm.x_zero && xzero_mark_t<5>(prm, ring, m, t, newY.data())) || (prm.z_zero && zzero_mark_t<5>(prm, ring, m, t))
+          : (prm.x_zero && xzero_mark_t<0>(prm, ring, m, t, newY.data())) || (prm.z_zero && zzero_mark_t<0>(prm, ring, m, t));
       if (hit) curb_hit(idx, k);
     }
     tab.maxdist[k] = fbits(maxdist_from_bits(tab.maxs[k]));        // k_tab1

@@ -176,6 +176,7 @@ int launch_pipeline(urf_ctx* ctx, const DevBuffers& buf, int B, int S, bool want
     CK(cudaEventRecord(ctx->ev_sfork[group], st));
     CK(cudaStreamWaitEvent(st_ring, ctx->ev_sfork[group], 0));
   }
+  // k_ring_detect never sees curb_points = 5, so it runs the detectors' runtime (<0>) instantiations only
   if (dp.curbPoints == 5)              // four positions per thread (default curb_points only)
     K("k_ring_detect4", k_ring_detect4<<<dim3((S + kTile4 - 1) / kTile4, B), 256, 0, st_ring>>>(buf, dp, S));
   else K("k_ring_detect", k_ring_detect<<<gpts, 256, 0, st_ring>>>(buf, dp, S));

@@ -1282,6 +1282,44 @@ __global__ void __launch_bounds__(kScanWarps * 32) k_star_scan(DevBuffers buf, D
 // the angle tests over (x-zero items from thread 0 upwards, z-zero items from thread 255 downwards). Points found to be
 // curb points are marked in input order and entered into the curb bins (curb_hit); nothing else is written per point.
 constexpr int kHalo = 32;
+
+// Threads 0 .. 2 kHalo - 1 of a ring-detector CTA: the kHalo bucket records on either side of the tile [p0, p0 + T) into
+// the tile slots [0, kHalo) and [kHalo + T, T + 2 kHalo) of the coordinate arrays, zeros outside the ordered points [0, N).
+template <int T>
+__device__ __forceinline__ void load_halo(const float4* bucket, int p0, int N, float* s_x, float* s_y, float* s_z) {
+  const int tid = threadIdx.x;
+  if (tid < 2 * kHalo) {
+    const int ph = tid < kHalo ? p0 - kHalo + tid : p0 + T + tid - kHalo;
+    const int sh = tid < kHalo ? tid : T + tid;
+    float4 h = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (ph >= 0 && ph < N) h = bucket[ph];
+    s_x[sh] = h.x; s_y[sh] = h.y; s_z[sh] = h.z;
+  }
+}
+// Warp-aggregated 64-bit atomicMax (MIN = false) or atomicMin (MIN = true) of v into a[key] from the lanes that hold a
+// value; the other lanes pass v = 0 (max) or ~0 (min). One atomic, from lane 0, when every holder has the same key, else
+// one per holder; either only where it would move a[key] past cur, the value the lane last read there (0 for a max that
+// read nothing). The warp reduces the high words first, then the low words of the lanes that hold the extreme high word.
+template <bool MIN>
+__device__ __forceinline__ void warp_atomic64(unsigned long long* a, bool holds, int key, unsigned long long v,
+                                              unsigned long long cur) {
+  const unsigned long long idle = MIN ? ~0ull : 0ull;
+  const unsigned hm = __ballot_sync(0xffffffffu, holds);
+  if (!hm) return;
+  const int key0 = __shfl_sync(0xffffffffu, key, __ffs(hm) - 1);
+  if (__all_sync(0xffffffffu, !holds || key == key0)) {
+    const unsigned hi = (unsigned)(v >> 32), mh = MIN ? __reduce_min_sync(0xffffffffu, hi) : __reduce_max_sync(0xffffffffu, hi);
+    const unsigned lo = hi == mh ? (unsigned)v : (unsigned)idle;
+    const unsigned ml = MIN ? __reduce_min_sync(0xffffffffu, lo) : __reduce_max_sync(0xffffffffu, lo);
+    const unsigned long long cur0 = __shfl_sync(0xffffffffu, cur, __ffs(hm) - 1);
+    if (lane_id() == 0) {                                           // results unused: REDs
+      const unsigned long long r = ((unsigned long long)mh << 32) | ml;
+      if (MIN ? cur0 > r : cur0 < r) { if (MIN) atomicMin(&a[key0], r); else atomicMax(&a[key0], r); }
+    }
+  } else if (holds && (MIN ? cur > v : cur < v)) {
+    if (MIN) atomicMin(&a[key], v); else atomicMax(&a[key], v);
+  }
+}
 __global__ void __launch_bounds__(256, 8) k_ring_detect(DevBuffers buf, DevParams prm, int S) {
   const int b = blockIdx.y;
   const ScanOut& out = buf.out[b];
@@ -1308,11 +1346,7 @@ __global__ void __launch_bounds__(256, 8) k_ring_detect(DevBuffers buf, DevParam
   const float4 me = act ? me0 : make_float4(0.f, 0.f, 0.f, 0.f);
   if (tiled) {                                            // one bucket record per thread + a halo record for the first 64 threads
     s_x[kHalo + tid] = me.x; s_y[kHalo + tid] = me.y; s_z[kHalo + tid] = me.z;
-    if (tid < 2 * kHalo) {
-      const int ph = tid < kHalo ? p0 - kHalo + tid : p0 + 256 + tid - kHalo;
-      const int sh = tid < kHalo ? tid : 256 + tid;
-      if (ph >= 0 && ph < N) { const float4 h = bucket[ph]; s_x[sh] = h.x; s_y[sh] = h.y; s_z[sh] = h.z; }
-    }
+    load_halo<256>(bucket, p0, N, s_x, s_y, s_z);
     s_hit[tid] = 0;
   }
   __syncthreads();
@@ -1327,12 +1361,12 @@ __global__ void __launch_bounds__(256, 8) k_ring_detect(DevBuffers buf, DevParam
       s_base[tid] = base;
       const int off = base - (p0 - kHalo);                // ring-local index q lives at tile slot off + q
       const RingSoA ring{s_x + off, s_y + off, s_z + off};
-      need_x = prm.x_zero && xzero_pre(prm, ring, n, m);
-      need_z = prm.z_zero && (prm.curbPoints == 5 ? zzero_pre_t<5>(prm, ring, n, m) : zzero_pre_t<0>(prm, ring, n, m));
+      need_x = prm.x_zero && xzero_pre_t<0>(prm, ring, n, m);
+      need_z = prm.z_zero && zzero_pre_t<0>(prm, ring, n, m);
     } else {                                              // huge curb_points: straight from global memory
       const float4* ring = bucket + base;
-      hit = (prm.x_zero && xzero_mark(prm, ring, n, m, buf.newY)) ||                  // x_zero_method.cpp:66
-            (prm.z_zero && zzero_mark(prm, ring, n, m));                              // z_zero_method.cpp:71
+      hit = (prm.x_zero && xzero_mark_t<0>(prm, ring, n, m, buf.newY)) ||             // x_zero_method.cpp:66
+            (prm.z_zero && zzero_mark_t<0>(prm, ring, n, m));                         // z_zero_method.cpp:71
     }
   }
   if (tiled) {
@@ -1356,29 +1390,22 @@ __global__ void __launch_bounds__(256, 8) k_ring_detect(DevBuffers buf, DevParam
     for (int it = 255 - tid; it < nz; it += 256) {                      // z-zero angle tests, z_zero_method.cpp:23-66
       const int t = s_item[511 - it], base = s_base[t], off = base - (p0 - kHalo);
       const RingSoA ring{s_x + off, s_y + off, s_z + off};
-      if (prm.curbPoints == 5 ? zzero_post_t<5>(prm, ring, p0 + t - base) : zzero_post_t<0>(prm, ring, p0 + t - base)) s_hit[t] = 1;
+      if (zzero_post_t<0>(prm, ring, p0 + t - base)) s_hit[t] = 1;
     }
     __syncthreads();
     hit = act && s_hit[tid];                                            // x_zero_method.cpp:66, z_zero_method.cpp:71
   }
   if (hit) curb_hit(buf, prm, b, gb, __float_as_int(me.w), k);
-  // maxDistance[k], lidar_segmentation.cpp:271-274 (warp-aggregated when the whole warp sits in one ring)
-  const unsigned long long sb = act ? planar_sum_bits(me.x, me.y) : 0ull;
-  const int k0 = __shfl_sync(0xffffffffu, k, 0);
-  if (__all_sync(0xffffffffu, k == k0)) {
-    if (k0 >= 0) {
-      const unsigned hi = (unsigned)(sb >> 32), mh = __reduce_max_sync(0xffffffffu, hi);
-      const unsigned ml = __reduce_max_sync(0xffffffffu, hi == mh ? (unsigned)sb : 0u);
-      if (lane_id() == 0) atomicMax(&buf.tab[b].maxs[k0], ((unsigned long long)mh << 32) | ml);   // result unused: a RED
-    }
-  } else if (act) atomicMax(&buf.tab[b].maxs[k], sb);
+  // maxDistance[k], lidar_segmentation.cpp:271-274
+  warp_atomic64<false>(buf.tab[b].maxs, k >= 0, k, planar_sum_bits(me.x, me.y), 0ull);
 }
 
 // k_ring_detect4: the same work for the default curb_points = 5 with FOUR consecutive bucket positions per thread (tile of
 // 1024 positions + halo per CTA). The two height gates of a position only read z: of its own ring, 5 positions to either
 // side (z-zero) and at -2 / +3 (x-zero). Four consecutive positions share a window of 14 heights, which the thread fetches
 // with five 16-byte shared-memory loads instead of 4 x 14 scalar ones; ring lookup, work-list compaction and the maximum of
-// the planar sums are amortised over the four positions as well. Same logic functions, same results as k_ring_detect.
+// the planar sums are amortised over the four positions as well. The gates restate xzero_pre_t<5> / zzero_pre_t<5> on the
+// register window (called through a view on it, they made the kernel 2 % slower on an H100 80GB HBM3 at 700 W).
 constexpr int kTile4 = 1024;
 __global__ void __launch_bounds__(256, 6) k_ring_detect4(DevBuffers buf, DevParams prm, int S) {
   constexpr int CP = 5;
@@ -1410,13 +1437,7 @@ __global__ void __launch_bounds__(256, 6) k_ring_detect4(DevBuffers buf, DevPara
     s_x[kHalo + t] = in ? rec[j].x : 0.f; s_y[kHalo + t] = in ? rec[j].y : 0.f; s_z[kHalo + t] = in ? rec[j].z : 0.f;
     s_hit[t] = 0;
   }
-  if (tid < 2 * kHalo) {
-    const int ph = tid < kHalo ? p0 - kHalo + tid : p0 + kTile4 + tid - kHalo;
-    const int sh = tid < kHalo ? tid : kTile4 + tid;
-    float4 h = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (ph >= 0 && ph < N) h = bucket[ph];
-    s_x[sh] = h.x; s_y[sh] = h.y; s_z[sh] = h.z;
-  }
+  load_halo<kTile4>(bucket, p0, N, s_x, s_y, s_z);
   __syncthreads();
   // the thread's four consecutive positions t0 .. t0 + 3 of the tile; heights of tile slots t0 - 8 .. t0 + 11
   const int t0 = 4 * tid;
@@ -1451,7 +1472,7 @@ __global__ void __launch_bounds__(256, 6) k_ring_detect4(DevBuffers buf, DevPara
       if ((__fsub_rn(max1, az0) >= prm.curbHeight || __fsub_rn(max2, az0) >= prm.curbHeight) && (double)fabsf(__fsub_rn(max1, max2)) >= 0.05)
         nz_mask |= 1u << j;
     }
-    // x-zero gate, xzero_pre with this point as p2 = j + cp / 2 (x_zero_method.cpp:62-64)
+    // x-zero gate, xzero_pre_t<5> with this point as p2 = j + cp / 2 (x_zero_method.cpp:62-64)
     const int jx = m - CP / 2;
     if (prm.x_zero && jx >= CP && jx <= (n - 1) - CP) {
       const float za = zw[8 + j - CP / 2], zc = zw[8 + j - CP / 2 + CP];
@@ -1714,20 +1735,7 @@ __global__ void __launch_bounds__(kLabelThreads) k_label(DevBuffers buf, DevPara
     // into a group, a ring-major one a few neighbouring bins: when all keys of the group belong to one bin only their
     // minimum goes out (one atomic per group instead of one per point). A key loaded before an earlier group of this warp
     // lowered it is only larger: the atomic then goes out needlessly, never wrongly.
-    const bool has_key = key != ~0ull;
-    const unsigned hk = __ballot_sync(0xffffffffu, has_key);
-    if (hk) {
-      const int bin0 = __shfl_sync(0xffffffffu, bin[u], __ffs(hk) - 1);
-      if (__all_sync(0xffffffffu, !has_key || bin[u] == bin0)) {
-        const unsigned hi = (unsigned)(key >> 32), mh = __reduce_min_sync(0xffffffffu, hi);
-        const unsigned ml = __reduce_min_sync(0xffffffffu, hi == mh ? (unsigned)key : 0xffffffffu);
-        const unsigned long long cb0 = __shfl_sync(0xffffffffu, cb[u], __ffs(hk) - 1);
-        if (lane == 0) {
-          const unsigned long long mk = ((unsigned long long)mh << 32) | ml;
-          if (cb0 > mk) atomicMin(&tab.cutbest[bin0], mk);
-        }
-      } else if (has_key && cb[u] > key) atomicMin(&tab.cutbest[bin[u]], key);
-    }
+    warp_atomic64<true>(tab.cutbest, key != ~0ull, bin[u], key, cb[u]);
     const unsigned br = __ballot_sync(0xffffffffu, lab == 1), bc = __ballot_sync(0xffffffffu, lab == 2);
     nroad += __popc(br);
     ncurb += __popc(bc);
@@ -1798,9 +1806,32 @@ __device__ __forceinline__ void markers_pass(const uint4* __restrict__ list, con
     }
   }
 }
+// The per-bin winners best[] (~0 = none) compacted in bin order into markerPointsArray (:343-350), with redPoints where
+// the bin has a first non-road point cut[] (:320,348), and a zeroed tail. One bin per thread: the CTA has at least
+// kDegBins threads, and s_wsum one entry per warp.
+__device__ __forceinline__ void write_vertices(const DevBuffers& buf, int b, int S, const unsigned long long* best,
+                                               const unsigned long long* cut, int* s_wsum) {
+  ScanOut& out = buf.out[b];
+  const int i = threadIdx.x, nwarps = blockDim.x >> 5;
+  const bool has = i < kDegBins && best[i] != ~0ull;
+  const unsigned bal = __ballot_sync(0xffffffffu, has);
+  const int warp = i >> 5, lane = lane_id();
+  if (lane == 0) s_wsum[warp] = __popc(bal);
+  __syncthreads();
+  const int c = lane < nwarps ? s_wsum[lane] : 0;      // at most 32 warps: lane w reads warp w's count
+  const int off = __reduce_add_sync(0xffffffffu, lane < warp ? c : 0), total = __reduce_add_sync(0xffffffffu, c);
+  if (has) {
+    const int slot = off + __popc(bal & ((1u << lane) - 1u));
+    const int p = (int)(best[i] & 0xffffffull);         // input index of the winner
+    const float4 q = buf.in[(size_t)b * S + p];
+    out.vert[slot][0] = q.x; out.vert[slot][1] = q.y; out.vert[slot][2] = q.z;
+    out.vert[slot][3] = cut[i] != ~0ull ? 1.0f : 0.0f;
+  }
+  if (i == 0) out.n_vert = total;
+  if (i >= total && i < URF_MAX_VERTS) { out.vert[i][0] = 0.f; out.vert[i][1] = 0.f; out.vert[i][2] = 0.f; out.vert[i][3] = 0.f; }   // defined tail
+}
 __global__ void __launch_bounds__(kMark1Threads) k_markers1(DevBuffers buf, int S) {
   const int b = blockIdx.y;                            // grid (1, B)
-  ScanOut& out = buf.out[b];
   const ScanTab& tab = buf.tab[b];
   __shared__ unsigned long long s_cut[kDegBins], s_best[kDegBins];
   __shared__ unsigned s_dmax[kDegBins];
@@ -1816,23 +1847,7 @@ __global__ void __launch_bounds__(kMark1Threads) k_markers1(DevBuffers buf, int 
   __syncthreads();
   markers_pass<2>(list, cnt, nseg, s_cut, s_dmax, s_best);
   __syncthreads();
-  const int i = tid;                                   // kMark1Threads >= kDegBins: one bin per thread
-  const bool has = i < kDegBins && s_best[i] != ~0ull;
-  const unsigned bal = __ballot_sync(0xffffffffu, has);
-  const int warp = i >> 5, lane = lane_id();
-  if (lane == 0) s_wsum[warp] = __popc(bal);
-  __syncthreads();
-  int off = 0, total = 0;
-  for (int w = 0; w < kMark1Threads / 32; w++) { if (w < warp) off += s_wsum[w]; total += s_wsum[w]; }
-  if (has) {
-    const int slot = off + __popc(bal & ((1u << lane) - 1u));
-    const int p = (int)(s_best[i] & 0xffffffull);      // input index of the winner
-    const float4 q = buf.in[(size_t)b * S + p];
-    out.vert[slot][0] = q.x; out.vert[slot][1] = q.y; out.vert[slot][2] = q.z;
-    out.vert[slot][3] = s_cut[i] != ~0ull ? 1.0f : 0.0f;                // redPoints, :320,348
-  }
-  if (i == 0) out.n_vert = total;
-  if (i >= total && i < URF_MAX_VERTS) { out.vert[i][0] = 0.f; out.vert[i][1] = 0.f; out.vert[i][2] = 0.f; out.vert[i][3] = 0.f; }   // defined tail
+  write_vertices(buf, b, S, s_best, s_cut, s_wsum);
 }
 
 // The same search for LARGE scans (hundreds of thousands of road points want more than one CTA): a grid of CTAs per scan,
@@ -1862,29 +1877,12 @@ __global__ void __launch_bounds__(kMarkGridThreads) k_markers_grid(DevBuffers bu
     else { const unsigned long long v = s_best[t]; if (v != ~0ull) atomicMin(&tab.best[t], v); }
   }
 }
-// k_verts: compact the per-bin winners (tab.best) in bin order into markerPointsArray (lidar_segmentation.cpp:343-350)
+// k_verts: the vertex compaction of k_markers1 on the merged winners (tab.best)
 __global__ void __launch_bounds__(384) k_verts(DevBuffers buf, int S) {
   const int b = blockIdx.x;
-  ScanOut& out = buf.out[b];
   const ScanTab& tab = buf.tab[b];
   __shared__ int s_wsum[12];
-  const int i = threadIdx.x;
-  const bool has = i < kDegBins && tab.best[i] != ~0ull;
-  const unsigned bal = __ballot_sync(0xffffffffu, has);
-  const int warp = i >> 5, lane = lane_id();
-  if (lane == 0) s_wsum[warp] = __popc(bal);
-  __syncthreads();
-  int off = 0, total = 0;
-  for (int w = 0; w < 12; w++) { if (w < warp) off += s_wsum[w]; total += s_wsum[w]; }
-  if (has) {
-    const int slot = off + __popc(bal & ((1u << lane) - 1u));
-    const int p = (int)(tab.best[i] & 0xffffffull);    // input index of the winner
-    const float4 q = buf.in[(size_t)b * S + p];
-    out.vert[slot][0] = q.x; out.vert[slot][1] = q.y; out.vert[slot][2] = q.z;
-    out.vert[slot][3] = tab.cutbest[i] != ~0ull ? 1.0f : 0.0f;          // redPoints, :320,348
-  }
-  if (i == 0) out.n_vert = total;
-  if (i >= total && i < URF_MAX_VERTS) { out.vert[i][0] = 0.f; out.vert[i][1] = 0.f; out.vert[i][2] = 0.f; out.vert[i][3] = 0.f; }   // defined tail
+  write_vertices(buf, b, S, tab.best, tab.cutbest, s_wsum);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------

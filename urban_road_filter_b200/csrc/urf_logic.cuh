@@ -202,7 +202,7 @@ URF_HD bool registration_violation(const float* angle, const int* regidx, const 
 }
 
 // A ring's points in ring order, as the two detectors read them: array-of-float4 (global memory, host model) or three
-// separate coordinate arrays (the shared-memory tile of k_ring_detect). q = local index inside the ring.
+// separate coordinate arrays (the shared-memory tiles of the ring detectors). q = local index inside the ring.
 struct RingAoS {
   const float4* p;
   URF_HDM float x(int q) const { return p[q].x; }
@@ -218,10 +218,11 @@ struct RingSoA {
 
 // x-zero test with local index m as the middle point p2 = j + cp/2 (x_zero_method.cpp:30-67), split in two: the index
 // range + height gate (cheap, float only; false for most points) and the triangle-angle test behind it. The kernel runs
-// the second half only for the points that pass the first (compacted per CTA); xzero_mark is both, for the host model.
-template <class RV>
-URF_HD bool xzero_pre(const DevParams& prm, const RV& ring, int n, int m) {
-  const int cp = prm.curbPoints;
+// the second half only for the points that pass the first (compacted per CTA); xzero_mark_t is both, for the host model.
+// CP > 0: curb_points known at compile time; CP == 0: taken from the parameters. Same arithmetic either way.
+template <int CP, class RV>
+URF_HD bool xzero_pre_t(const DevParams& prm, const RV& ring, int n, int m) {
+  const int cp = CP > 0 ? CP : prm.curbPoints;
   const int j = m - cp / 2;
   if (!(j >= cp && j <= (n - 1) - cp)) return false;
   const float az = ring.z(j), cz = ring.z(j + cp), z = ring.z(m);
@@ -245,13 +246,14 @@ URF_HD bool xzero_post(const DevParams& prm, const RV& ring, int m, const float*
   const float al = URF_D2F(deg_d(urfm::acosf_glibc(bk)));                                                     // :58
   return al <= prm.angleFilter1;                                                                              // :61
 }
-URF_HD bool xzero_mark(const DevParams& prm, const float4* ring, int n, int m, const float* newY) {
+template <int CP>
+URF_HD bool xzero_mark_t(const DevParams& prm, const float4* ring, int n, int m, const float* newY) {
   const RingAoS rv{ring};
-  return xzero_pre(prm, rv, n, m) && xzero_post(prm, rv, m, newY);
+  return xzero_pre_t<CP>(prm, rv, n, m) && xzero_post(prm, rv, m, newY);
 }
 
-// z-zero test centred on local index m (z_zero_method.cpp:21-72), split the same way. CP > 0: curb_points known at
-// compile time (loops unroll); CP == 0: taken from the parameters. Same arithmetic either way.
+// z-zero test centred on local index m (z_zero_method.cpp:21-72), split the same way, with the same CP convention (loops
+// unroll when CP > 0).
 template <int CP, class RV>
 URF_HD bool zzero_pre_t(const DevParams& prm, const RV& ring, int n, int m) {
   const int cp = CP > 0 ? CP : prm.curbPoints;
@@ -289,7 +291,6 @@ URF_HD bool zzero_mark_t(const DevParams& prm, const float4* ring, int n, int m)
   const RingAoS rv{ring};
   return zzero_pre_t<CP>(prm, rv, n, m) && zzero_post_t<CP>(prm, rv, m);
 }
-URF_HD bool zzero_mark(const DevParams& prm, const float4* ring, int n, int m) { return zzero_mark_t<0>(prm, ring, n, m); }
 
 // Edge search along one radius-sorted sector (star_shaped_search.cpp:112-150) as a step function: state after point
 // i-1, fed point i (planar radius r, height z); returns true when point i gets marked (the scan then stops).
