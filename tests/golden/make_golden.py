@@ -6,7 +6,8 @@ tests need neither the reference's sources nor its build.
     python tests/golden/make_golden.py --only c5
     python tests/golden/make_golden.py --ref-checks    # tests/golden/ref/: the reference's outputs for the random-parameter
                                                        # draws of tests/test_oracle.py, the strips of tests/test_markers.py
-                                                       # and the tie clouds of tests/test_ties.py
+                                                       # the tie clouds of tests/test_ties.py and the azimuth
+                                                       # edge clouds of tests/test_azimuth_edges.py
 
 Each fixture holds: params (cfg overrides), the input cloud (or, for big clouds, the generator recipe + sha256 of the
 bytes it must produce), and what the reference published: per-point labels (recovered from the roi/road/curb clouds),
@@ -32,6 +33,7 @@ from urban_road_filter_b200 import FULL_ROI, make_params  # noqa: E402
 from urban_road_filter_b200.synth import SHAPES, make_scan, random_cloud  # noqa: E402
 from oracle.pyoracle import PortOracle  # noqa: E402
 from util import MARKER_EPS, REF_DIR, cloud_digest, digest, random_param_case  # noqa: E402
+import azimuth_edges  # noqa: E402
 import tie_policy  # noqa: E402
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -99,6 +101,27 @@ def ref_checks():
             strips[f"s{seed}_e{k}_meta"], strips[f"s{seed}_e{k}_pts"] = strips_to_arrays(r.strips)
     np.savez_compressed(os.path.join(REF_DIR, "marker_strips.npz"), **strips)
     ref_ties(ref)
+    ref_azimuth_edges(ref)
+
+
+def ref_azimuth_edges(ref):
+    """azimuth_edges.npz: per cloud of tests/azimuth_edges.py the points appended to its base scan (so the tests run
+    exactly these points whatever libm the machine has; the base scan is checked by the cloud's sha256), what the
+    reference published (labels, road / curb / road_probably input indices, as
+    sha256) and its marker strips with simplification off."""
+    port = PortOracle()
+    meta, arrays = {}, {}
+    for name, build in azimuth_edges.CASES.items():
+        pts, prm = build(port)
+        r = ref.run(pts, prm)
+        meta[name] = dict(cloud_sha256=cloud_digest(pts), published=r.published, label=digest(r.label),
+                          road_ids=digest(r.road_ids), curb_ids=digest(r.curb_ids), prob_ids=digest(r.prob_ids))
+        prm.simple_poly_allow, prm.poly_z_avg_allow = 0, 0
+        r = ref.run(pts, prm, ghostcount=0)
+        meta[name]["markers_published"] = r.markers_published
+        arrays[name + "_tail"] = pts[azimuth_edges.base_scan(name).shape[0]:]
+        arrays[name + "_meta"], arrays[name + "_pts"] = strips_to_arrays(r.strips)
+    np.savez_compressed(os.path.join(REF_DIR, "azimuth_edges.npz"), meta=json.dumps(meta, sort_keys=True), **arrays)
 
 
 def ref_ties(ref):

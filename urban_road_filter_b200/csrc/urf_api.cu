@@ -797,7 +797,9 @@ int urf_test_math(int device, int which, const float* a, const float* b, float* 
 //   what: 0 alpha_v[f32,n]  1 mark[u8,n] (all detectors)  2 ringid[i16,n]  3 sect[i16,n]  4 az[f32,n]  5 d2[f32,n]
 //         (4, 5: defined for ROI points only)  8 ScanTab (raw)  9 star sort work lists [i32,2]: sectors handed to the
 //         eight-warp sort (nbig) and to the exact fallback (nslow)  10 sectors completed by k_star_refine [i32,1]
-//         (nrefine: their edge search ran off the near-first prefix)
+//         (nrefine: their edge search ran off the near-first prefix)  11 Tf, 12 Tb: the blindSpots threshold tables as
+//         k_tab2 left them [f32, kDegBins * channels], degree-major (entry (j, k) at j * channels + k; rows k >= n_rings
+//         are not written)
 int urf_debug_fetch(urf_ctx* ctx, int b, int what, void* dst, size_t bytes) {
   if (!ctx || !dst || b < 0 || b >= ctx->last_B) return URF_ERR_INVALID;
   CK(cudaSetDevice(ctx->device));
@@ -814,6 +816,12 @@ int urf_debug_fetch(urf_ctx* ctx, int b, int what, void* dst, size_t bytes) {
     case 8: src = ctx->buf.tab + b; if (bytes > sizeof(ScanTab)) bytes = sizeof(ScanTab); break;
     case 9: src = &ctx->buf.tab[b].nbig; if (bytes > 2 * sizeof(int)) bytes = 2 * sizeof(int); break;
     case 10: src = &ctx->buf.tab[b].nrefine; if (bytes > sizeof(int)) bytes = sizeof(int); break;
+    case 11: case 12: {
+      const size_t ch = (size_t)ctx->dp.channels;
+      src = (what == 11 ? ctx->buf.Tf : ctx->buf.Tb) + (size_t)b * ch * kTStride;
+      if (bytes > sizeof(float) * ch * kDegBins) bytes = sizeof(float) * ch * kDegBins;
+      break;
+    }
     default: return URF_ERR_INVALID;
   }
   CK(cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost));
