@@ -103,7 +103,9 @@ typedef struct urf_result {
                                     unsorted; ties there are neither seen nor relevant); bit2: ring-azimuth ties present
                                     (bit1 / bit2: tie policy differs from the reference's unstable sorts); bit3: a ROI point
                                     with x == y == 0 exists (azimuth NaN: it belongs to no window or bin here, while in the
-                                    reference it truncates the window scans of its ring) */
+                                    reference it truncates the window scans of its ring). With the reference tie order
+                                    (urf_set_tie_order below) bit2 is reported whether or not `order` is requested, and
+                                    the order it marks is the reference's own */
   int32_t  reserved;
   int32_t* label;                /* [n_in] or NULL */
   int32_t* ring;                 /* [n_in] or NULL */
@@ -135,6 +137,24 @@ void urf_destroy(urf_ctx* ctx);
 /* Replaces paramsCallback (src/main.cpp:4-34). Takes effect for the next urf_process* call. */
 int urf_set_params(urf_ctx* ctx, const urf_params* p);
 int urf_get_params(const urf_ctx* ctx, urf_params* p);
+
+/*
+ * Tie order of the emission order (urf_result.order, the packed clouds) and of the marker vertices where a ring holds
+ * equal azimuths (dual-return modes, duplicated points, rings merged by a large `interval`):
+ *   URF_TIES_INPUT_ORDER (default): equal azimuths in input order, NaN azimuths last. Labels never depend on the tie order.
+ *   URF_TIES_REFERENCE: the order the reference's unstable Lomuto quicksort leaves (lidar_segmentation.cpp:70-93,
+ *     289-291) on every ring that holds a float-equal pair or a NaN azimuth — its road, curb and road_probably clouds and
+ *     its marker vertices (:313-335) bit for bit. Costs the ring sort on every call (even without `order`) and, per
+ *     ring with ties, about one CTA-wide partition per point in the worst case (DESIGN.md §6).
+ *     Not covered: a NaN azimuth (x == y == 0) still truncates the reference's blindSpots window scans, so with
+ *     blind_spots on, labels of such scans can differ (flags bit3).
+ * The setting applies to the next urf_process* / urf_enqueue* call. The first switch to URF_TIES_REFERENCE allocates 4
+ * bytes of device memory per point of capacity (URF_ERR_NOMEM if that fails); urf_process* never allocates for it.
+ * A urf_queue uses its ctx's setting; urf_mq_set_tie_order sets it on every device, only while nothing is in flight.
+ */
+enum { URF_TIES_INPUT_ORDER = 0, URF_TIES_REFERENCE = 1 };
+int urf_set_tie_order(urf_ctx* ctx, int mode);
+int urf_get_tie_order(const urf_ctx* ctx, int* mode);
 
 /* Replaces one Detector::filtered() call. xyzi = n points of 4 floats (x, y, z, intensity) in HOST memory: the first
  * 16 bytes of each pcl::PointXYZI record once the PointCloud2 has been deserialised. Synchronous. */
@@ -309,7 +329,7 @@ int urf_queue_create_with(urf_queue** out, urf_queue_process_fn fn, void* user, 
  * a context and a urf_queue (above) per device, hands every scan to the device with the fewest scans in flight, and
  * delivers the results in the order the submissions completed. Scans are independent, so no data moves between devices.
  * Any number of producer threads; ONE consumer thread. urf_mq_submit_ref is the no-copy variant (see urf_queue_submit_ref).
- * urf_mq_set_params applies to all devices and is only accepted while nothing is in flight (like the reference's
+ * urf_mq_set_params (and urf_mq_set_tie_order) applies to all devices and is only accepted while nothing is in flight (like the reference's
  * paramsCallback between two scan callbacks).
  */
 typedef struct urf_mq urf_mq;
@@ -322,6 +342,7 @@ typedef struct urf_mq_stats {
 int urf_mq_create(urf_mq** out, const int* devices, int n_devices, int max_points, int slots_per_device, int max_batch,
                   const urf_params* params /* or NULL: cfg defaults */);
 int urf_mq_set_params(urf_mq* mq, const urf_params* p);
+int urf_mq_set_tie_order(urf_mq* mq, int mode);   /* urf_set_tie_order on every device; the same in-flight rule */
 int urf_mq_submit(urf_mq* mq, const float* xyzi, int n, uint64_t tag, int timeout_ms);
 int urf_mq_submit_ref(urf_mq* mq, const float* xyzi, int n, uint64_t tag, int timeout_ms);
 int urf_mq_next(urf_mq* mq, uint64_t* tag, urf_result* out, int timeout_ms);

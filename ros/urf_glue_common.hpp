@@ -17,6 +17,16 @@ namespace urf_glue {
 inline urf_params g_params;          // what paramsCallback last received (the reference keeps them in params:: globals)
 inline bool g_params_dirty = true;
 
+// node parameter ~reference_tie_order (default false): equal azimuths inside a ring in the order the reference's Lomuto
+// quicksort leaves them (its clouds and marker vertices bit for bit) instead of input order; see urf_set_tie_order
+inline void set_tie_order(urf_ctx* ctx, bool reference) {
+  const int rc = urf_set_tie_order(ctx, reference ? URF_TIES_REFERENCE : URF_TIES_INPUT_ORDER);
+  if (rc != URF_OK) {
+    ROS_FATAL("urf_set_tie_order: %s (%s)", urf_strerror(rc), urf_last_cuda_error(ctx));
+    throw std::runtime_error(std::string("urf_set_tie_order: ") + urf_strerror(rc));
+  }
+}
+
 // paramsCallback, src/main.cpp:4-34: same fields, same order; narrowing to float happens inside urf_set_params
 inline void paramsCallback(urban_road_filter::LidarFiltersConfig& config, uint32_t /*level*/) {
   urf_params& p = g_params;

@@ -25,12 +25,13 @@ namespace urf_glue {
 class Detector {
  public:
   // device: CUDA device index; max_points: largest scan the sensor can produce; channels: ring count (reference constant 64)
-  Detector(ros::NodeHandle* nh, int device = 0, int max_points = 1 << 20, int channels = 64) : channels_(channels) {
+  Detector(ros::NodeHandle* nh, int device = 0, int max_points = 1 << 20, int channels = 64, bool reference_tie_order = false) : channels_(channels) {
     const int rc = urf_create(&ctx_, device, max_points, 1);
     if (rc != URF_OK) {                                   // no GPU, no node: the reference never runs silently without output
       ROS_FATAL("urf_create(device %d, %d points): %s (%s)", device, max_points, urf_strerror(rc), urf_last_cuda_error(nullptr));
       throw std::runtime_error(std::string("urf_create: ") + urf_strerror(rc));
     }
+    set_tie_order(ctx_, reference_tie_order);
     sub_ = nh->subscribe(std::string(g_params.topic_name), 1, &Detector::filtered, this);        // lidar_segmentation.cpp:53
     pub_road_ = nh->advertise<pcl::PCLPointCloud2>("road", 1);                                     // :55-59
     pub_high_ = nh->advertise<pcl::PCLPointCloud2>("curb", 1);
@@ -117,7 +118,9 @@ int main(int argc, char** argv) {                        // src/main.cpp:37-56
   pnh.param("device", device, 0);
   pnh.param("max_points", max_points, 1 << 20);
   pnh.param("channels", channels, 64);                   // the reference's global `int channels = 64` (lidar_segmentation.cpp:4)
-  urf_glue::Detector detector(&nh, device, max_points, channels);
+  bool reference_tie_order = false;
+  pnh.param("reference_tie_order", reference_tie_order, false);
+  urf_glue::Detector detector(&nh, device, max_points, channels, reference_tie_order);
   ros::spin();
   return 0;
 }

@@ -20,12 +20,13 @@ namespace urf_glue {
 
 class DetectorCloud2 {
  public:
-  DetectorCloud2(ros::NodeHandle* nh, int device = 0, int max_points = 1 << 20, int channels = 64) : max_points_(max_points), channels_(channels) {
+  DetectorCloud2(ros::NodeHandle* nh, int device = 0, int max_points = 1 << 20, int channels = 64, bool reference_tie_order = false) : max_points_(max_points), channels_(channels) {
     const int rc = urf_create(&ctx_, device, max_points, 1);
     if (rc != URF_OK) {
       ROS_FATAL("urf_create(device %d, %d points): %s (%s)", device, max_points, urf_strerror(rc), urf_last_cuda_error(nullptr));
       throw std::runtime_error(std::string("urf_create: ") + urf_strerror(rc));
     }
+    set_tie_order(ctx_, reference_tie_order);
     for (urf_point_xyzi** c : {&clouds_.road, &clouds_.curb, &clouds_.roi, &clouds_.road_probably}) {
       *c = static_cast<urf_point_xyzi*>(urf_pinned_alloc(sizeof(urf_point_xyzi) * (size_t)max_points));   // D2H at full PCIe rate
       if (!*c) throw std::runtime_error("urf_pinned_alloc failed");
@@ -124,7 +125,9 @@ int main(int argc, char** argv) {                        // src/main.cpp:37-56
   pnh.param("device", device, 0);
   pnh.param("max_points", max_points, 1 << 20);
   pnh.param("channels", channels, 64);                   // the reference's global `int channels = 64` (lidar_segmentation.cpp:4)
-  urf_glue::DetectorCloud2 detector(&nh, device, max_points, channels);
+  bool reference_tie_order = false;
+  pnh.param("reference_tie_order", reference_tie_order, false);
+  urf_glue::DetectorCloud2 detector(&nh, device, max_points, channels, reference_tie_order);
   ros::spin();
   return 0;
 }

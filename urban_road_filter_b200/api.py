@@ -22,7 +22,10 @@ EXPORTS = ["urf_queue_next_batch", "urf_mq_next_batch", "urf_mq_create_label8", 
            "urf_version", "urf_strerror", "urf_last_cuda_error", "urf_default_params", "urf_create", "urf_destroy",
            "urf_set_params", "urf_get_params", "urf_process", "urf_process_batch", "urf_process_batch_device",
            "urf_process_batch_xyz", "urf_process_cloud2_batch", "urf_enqueue_batch_device", "urf_enqueue_batch_device_ex", "urf_finish_batch_device", "urf_stream", "urf_last_device_ms",
-           "urf_last_launch_count", "urf_build_markers"]
+           "urf_last_launch_count", "urf_build_markers", "urf_set_tie_order", "urf_get_tie_order", "urf_mq_set_tie_order"]
+
+# urf_set_tie_order modes (include/urf.h): equal azimuths inside a ring in input order, or in the reference's Lomuto order
+TIE_ORDERS = {"input": 0, "reference": 1}
 
 _lib = None
 
@@ -54,6 +57,9 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
     lib.urf_set_params.argtypes = [vp, C.POINTER(UrfParams)]
     lib.urf_get_params.argtypes = [vp, C.POINTER(UrfParams)]
     lib.urf_set_option.argtypes = [vp, ip, ip]
+    lib.urf_set_tie_order.argtypes = [vp, ip]
+    lib.urf_get_tie_order.argtypes = [vp, C.POINTER(ip)]
+    lib.urf_mq_set_tie_order.argtypes = [vp, ip]
     lib.urf_process.argtypes = [vp, vp, ip, C.POINTER(UrfResult)]
     lib.urf_process_batch.argtypes = [vp, C.POINTER(vp), C.POINTER(ip), ip, C.POINTER(UrfResult)]
     lib.urf_process_cloud2.argtypes = [vp, vp, ip, ip, ip, ip, ip, C.POINTER(UrfResult)]
@@ -174,7 +180,8 @@ def build_markers(prm: UrfParams, vert: np.ndarray, ghostcount: int = 0):
 class Detector:
     """Host-side mirror of the reference's `Detector` (include/urban_road_filter/data_structures.hpp:110-141) on one GPU."""
 
-    def __init__(self, max_points: int, max_batch: int = 1, device: int = 0, params: UrfParams | None = None):
+    def __init__(self, max_points: int, max_batch: int = 1, device: int = 0, params: UrfParams | None = None,
+                 tie_order: str = "input"):
         self.lib = load_library()
         self._ctx = C.c_void_p()
         rc = self.lib.urf_create(C.byref(self._ctx), device, max_points, max_batch)
@@ -183,6 +190,8 @@ class Detector:
         self.max_points, self.max_batch, self.device = max_points, max_batch, device
         self.params = params if params is not None else make_params()
         self.set_params(self.params)
+        if tie_order != "input":
+            self.set_tie_order(tie_order)
         self.ghostcount = 0      # lidar_segmentation.cpp:23
 
     def close(self):
@@ -207,6 +216,18 @@ class Detector:
 
     def set_option(self, option: int, value: int):
         self._check(self.lib.urf_set_option(self._ctx, option, value), "urf_set_option")
+
+    def set_tie_order(self, mode: str):
+        """"input" (default: equal azimuths of a ring in input order) or "reference" (the order the reference's Lomuto
+        quicksort leaves: its clouds and marker vertices bit for bit). Applies from the next call (urf_set_tie_order)."""
+        if mode not in TIE_ORDERS:
+            raise ValueError(f"tie order {mode!r}: expected one of {sorted(TIE_ORDERS)}")
+        self._check(self.lib.urf_set_tie_order(self._ctx, TIE_ORDERS[mode]), "urf_set_tie_order")
+
+    def tie_order(self) -> str:
+        m = C.c_int()
+        self._check(self.lib.urf_get_tie_order(self._ctx, C.byref(m)), "urf_get_tie_order")
+        return {v: k for k, v in TIE_ORDERS.items()}[m.value]
 
     def filtered_batch(self, clouds, want_ring: bool = True, want_order: bool = True) -> list[ScanResult]:
         """`batch` independent Detector::filtered() calls (lidar_segmentation.cpp:95) on host (N,4) float32 arrays."""
@@ -419,6 +440,14 @@ class MultiGpuQueue:
         rc = self.lib.urf_mq_set_params(self._m, C.byref(prm))
         if rc != URF_OK:
             raise UrfError(rc, "urf_mq_set_params")
+
+    def set_tie_order(self, mode: str):
+        """Detector.set_tie_order on every device; like set_params, only while nothing is in flight."""
+        if mode not in TIE_ORDERS:
+            raise ValueError(f"tie order {mode!r}: expected one of {sorted(TIE_ORDERS)}")
+        rc = self.lib.urf_mq_set_tie_order(self._m, TIE_ORDERS[mode])
+        if rc != URF_OK:
+            raise UrfError(rc, "urf_mq_set_tie_order")
 
     def submit(self, cloud: np.ndarray, tag: int = 0, timeout_ms: int = -1, by_reference: bool = False) -> int:
         pts = np.ascontiguousarray(cloud, np.float32)

@@ -10,6 +10,7 @@
 
 #include "urf_kernels.cuh"
 #include "urf_host.hpp"
+#include "urf_queue_internal.hpp"
 
 using namespace urf;
 
@@ -55,6 +56,8 @@ struct urf_ctx {
   float4* pack = nullptr;              // packed output clouds (urf_process_cloud2_packed): 3 * max_points 32-byte records, allocated on first use
   int* packcnt = nullptr;              // [3][tiles] per-tile counts / offsets
   int* packtot = nullptr;              // [4] cloud sizes
+  int tie_order = URF_TIES_INPUT_ORDER;   // urf_set_tie_order; the reference order's buffers (buf.epos, buf.lomuto) are
+                                          // allocated by the first switch to it
   int* h_packtot = nullptr;            // pinned copy
   urf_params params{};
   DevParams dp{};
@@ -122,6 +125,7 @@ DevBuffers offset_view(const DevBuffers& a, int b0, int S, int T, int channels) 
   DevBuffers v = a;
   const size_t o = (size_t)b0 * S;
   v.in += o; v.label += o; v.order += o; v.n += b0; v.out += b0;
+  if (v.epos) { v.epos += o; v.lomuto += (size_t)b0 * (kRingKeys + 1); }
   if (v.label8) v.label8 += o;
   v.alpha_v += o; v.mark += o; v.ringid += o; v.sect += o; v.bpt += o;
   v.sr += o; v.sz += o; v.sidx += o; v.ssrz += o; v.ssl += o;
@@ -143,7 +147,10 @@ thread_local std::string g_create_err;
 // stream, kGroups: the context's own stream) and stores the number of kernels launched in *launched.
 int launch_pipeline(urf_ctx* ctx, const DevBuffers& buf, int B, int S, bool want_order, int group, int* launched) {
   DevParams dp = ctx->dp;
-  dp.want_order = want_order ? 1 : 0;
+  // reference tie order: the emission order decides the marker search's scan order, so the ring sort always runs, in
+  // front of k_label (into the context's own order buffer when the caller asked for none)
+  const bool ref = ctx->tie_order == URF_TIES_REFERENCE;
+  dp.want_order = want_order || ref ? 1 : 0;
   cudaStream_t st = group < urf_ctx::kGroups ? ctx->s_grp[group] : ctx->stream;
   const int T = (S + kChunk - 1) / kChunk;
   if (T > ctx->Tmax) return URF_ERR_CAPACITY;
@@ -199,14 +206,21 @@ int launch_pipeline(urf_ctx* ctx, const DevBuffers& buf, int B, int S, bool want
   K("k_tab1", k_tab1<<<dim3((dp.channels + 7) / 8, B), 256, 0, st>>>(buf, dp));
   K("k_reach", k_reach<<<dim3((2 * kDegBins + 7) / 8, B), 256, 0, st>>>(buf, dp));
   K("k_tab2", k_tab2<<<dim3((dp.channels + kTab2Rings - 1) / kTab2Rings, B), kTab2Rings * 64, 0, st>>>(buf, dp));
-  K("k_label", k_label<<<dim3((S + kLabelThreads * kLabelGroups - 1) / (kLabelThreads * kLabelGroups), B), kLabelThreads, 0, st>>>(buf, dp, S));
+  const dim3 glabel((S + kLabelThreads * kLabelGroups - 1) / (kLabelThreads * kLabelGroups), B), gsort(dp.channels, B);
+  if (ref) {
+    K("k_sort_rings", k_sort_rings<true><<<gsort, kSortThreads, kRingSmemKeys * sizeof(unsigned long long), st>>>(buf, S));
+    K("k_lomuto_rings", k_lomuto_rings<<<gsort, kLomutoThreads, kLomutoSmem, st>>>(buf, S));
+    K("k_label", k_label<true><<<glabel, kLabelThreads, 0, st>>>(buf, dp, S));
+  } else K("k_label", k_label<false><<<glabel, kLabelThreads, 0, st>>>(buf, dp, S));
   if (S > kMarkSingleMax) {            // large scans: a grid of CTAs per scan, three launches
     const dim3 gm(std::max(1, std::min(64, S / 16384)), B);
     K("k_markers_grid1", k_markers_grid<1><<<gm, kMarkGridThreads, 0, st>>>(buf, S));
     K("k_markers_grid2", k_markers_grid<2><<<gm, kMarkGridThreads, 0, st>>>(buf, S));
-    K("k_verts", k_verts<<<B, 384, 0, st>>>(buf, S));
-  } else K("k_markers1", k_markers1<<<dim3(1, B), kMark1Threads, 0, st>>>(buf, S));   // one CTA per scan
-  if (want_order) K("k_sort_rings", k_sort_rings<<<dim3(dp.channels, B), kSortThreads, kRingSmemKeys * sizeof(unsigned long long), st>>>(buf, S));
+    if (ref) K("k_verts", k_verts<true><<<B, 384, 0, st>>>(buf, S));
+    else K("k_verts", k_verts<false><<<B, 384, 0, st>>>(buf, S));
+  } else if (ref) K("k_markers1", k_markers1<true><<<dim3(1, B), kMark1Threads, 0, st>>>(buf, S));
+  else K("k_markers1", k_markers1<false><<<dim3(1, B), kMark1Threads, 0, st>>>(buf, S));   // one CTA per scan
+  if (want_order && !ref) K("k_sort_rings", k_sort_rings<false><<<gsort, kSortThreads, kRingSmemKeys * sizeof(unsigned long long), st>>>(buf, S));
 #undef K
   if (ctx->profile) {
     CK(cudaEventRecord(ctx->kev[(size_t)ctx->kslot * (kMaxKernels + 1) + kMaxKernels], st));
@@ -391,7 +405,9 @@ int urf_create(urf_ctx** out, int device, int max_points, int max_batch) {
   CKF(cudaFuncSetAttribute(k_star_refine, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kStarCtaSmem));
   CKF(cudaFuncSetAttribute(k_scatter, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kScatterSmem));
   CKF(cudaFuncSetAttribute(k_scatter, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));   // four CTAs per SM
-  CKF(cudaFuncSetAttribute(k_sort_rings, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kRingSmemKeys * sizeof(unsigned long long))));
+  CKF(cudaFuncSetAttribute(k_sort_rings<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kRingSmemKeys * sizeof(unsigned long long))));
+  CKF(cudaFuncSetAttribute(k_sort_rings<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kRingSmemKeys * sizeof(unsigned long long))));
+  CKF(cudaFuncSetAttribute(k_lomuto_rings, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kLomutoSmem));
   urf_default_params(&ctx->params);
   const char* fe = std::getenv("URF_FORCE_EXACT_REGISTRATION");
   narrow_params(&ctx->params, &ctx->dp, ctx->dp.Kfi, fe && fe[0] == '1', 0);
@@ -496,6 +512,34 @@ int urf_set_option(urf_ctx* ctx, int option, int value) {
     return URF_OK;
   }
   return URF_ERR_INVALID;
+}
+
+int urf_set_tie_order(urf_ctx* ctx, int mode) {
+  if (!ctx || (mode != URF_TIES_INPUT_ORDER && mode != URF_TIES_REFERENCE)) return URF_ERR_INVALID;
+  CK(cudaSetDevice(ctx->device));
+  if (mode == URF_TIES_REFERENCE && !ctx->buf.lomuto) {   // 4 bytes per point of capacity plus one ring list per scan
+    int* epos = nullptr;
+    int* lomuto = nullptr;
+    int rc = dalloc(ctx, &epos, ctx->P);
+    if (rc == URF_OK) rc = dalloc(ctx, &lomuto, (size_t)ctx->max_batch * (kRingKeys + 1));
+    if (rc != URF_OK) return rc;
+    ctx->buf.epos = epos;
+    ctx->buf.lomuto = lomuto;
+  }
+  ctx->tie_order = mode;
+  ctx->version++;                                          // the captured graph holds the other launch sequence
+  return URF_OK;
+}
+
+int urf_get_tie_order(const urf_ctx* ctx, int* mode) {
+  if (!ctx || !mode) return URF_ERR_INVALID;
+  *mode = ctx->tie_order;
+  return URF_OK;
+}
+
+int urf_mq_set_tie_order(urf_mq* mq, int mode) {
+  if (!mq || (mode != URF_TIES_INPUT_ORDER && mode != URF_TIES_REFERENCE)) return URF_ERR_INVALID;
+  return urf_internal::mq_apply_idle(mq, [](urf_ctx* c, const void* m) { return urf_set_tie_order(c, *static_cast<const int*>(m)); }, &mode);
 }
 
 void* urf_stream(urf_ctx* ctx) { return ctx ? (void*)ctx->stream : nullptr; }

@@ -109,6 +109,8 @@ struct DevBuffers {
   float* Tb;             // [B][channels][kTStride] backward threshold table
   unsigned short* lut;   // [B][kElevBins + 1] ring-search start per fine elevation bin
   int* order;            // [P]   emission order (input indices), only when requested
+  int* epos;             // [P] or NULL: emission position per input point (reference tie order: the marker search's scan order)
+  int* lomuto;           // [B][kRingKeys + 1] or NULL: count, then the rings whose tie order k_lomuto_rings computes
   unsigned long long* sortbuf;   // [2P] scratch for segments too large for shared memory
   unsigned* hist;        // [B][T][channels] per-chunk ring histograms, turned into scatter offsets in place
   unsigned* firstidx;    // [B][kElevBins + 1] first input index per fine elevation bin
