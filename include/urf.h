@@ -211,6 +211,35 @@ int urf_process_batch_xyz(urf_ctx* ctx, const float* const* xyz, const int* n, i
 int urf_process_cloud2_batch(urf_ctx* ctx, const void* const* data, const int* n_points, int batch, int point_step, int off_x,
                              int off_y, int off_z, int off_intensity, urf_result* outs, int8_t* const* label8);
 
+/*
+ * Asynchronous host-buffer batches: urf_enqueue_batch (float4 scans, as urf_process_batch) and urf_enqueue_cloud2_batch
+ * (PointCloud2 records, as urf_process_cloud2_batch) queue the copies and kernels of a batch and return at once;
+ * urf_finish_batch waits for the OLDEST batch in flight and fills its outs[] (and label8[] buffers). While batch N runs,
+ * the caller can hand over batch N+1: its input copies overlap batch N's kernels, its kernels follow them on the same
+ * stream, and batch N's result copies overlap batch N+1's kernels.
+ *   - A context holds at most TWO host batches in flight: a third enqueue returns URF_ERR_CAPACITY; urf_finish_batch with
+ *     nothing in flight returns URF_ERR_INVALID.
+ *   - Every output (labels, int8 labels, ring, order, ring_start, counts, flags, vertices) is bit for bit what
+ *     urf_process_batch / urf_process_cloud2_batch give for the same scans, in both tie orders. label8 as in
+ *     urf_process_batch_xyz; label8 == NULL: no int8 labels.
+ *   - The input buffers, the outs array and every buffer it or label8 points at must stay valid and unchanged until the
+ *     batch's urf_finish_batch returns. Copies from pinned memory (urf_pinned_alloc) run asynchronously. A copy to or from
+ *     pageable memory makes the call wait for it: with pageable outs the enqueue returns only once the batch's results
+ *     are on the host, and nothing overlaps.
+ *   - While host batches are in flight, urf_process*, urf_enqueue_batch_device*, urf_finish_batch_device, urf_set_params,
+ *     urf_set_tie_order and urf_set_option return URF_ERR_INVALID. urf_destroy waits for them (their outs are not filled).
+ *   - urf_last_device_ms and urf_last_launch_count describe the last finished batch.
+ * The first asynchronous call allocates a second set of the buffers a batch's copies touch, and a ring-id buffer for the
+ * first set (which until then keeps ring ids in sort scratch that the next batch's kernels overwrite): 32 bytes of device
+ * memory per point of capacity (input, labels, order, two ring-id buffers), plus 1 byte per point once int8 labels are
+ * asked for and point_step bytes per point once records are given, and two small pinned arrays per scan of max_batch.
+ * No batch waits for another batch's copies.
+ */
+int urf_enqueue_batch(urf_ctx* ctx, const float* const* xyzi, const int* n, int batch, urf_result* outs, int8_t* const* label8);
+int urf_enqueue_cloud2_batch(urf_ctx* ctx, const void* const* data, const int* n_points, int batch, int point_step, int off_x,
+                             int off_y, int off_z, int off_intensity, urf_result* outs, int8_t* const* label8);
+int urf_finish_batch(urf_ctx* ctx);
+
 /* Device-resident variant used to time the kernels without PCIe: d_xyzi is a DEVICE pointer to the scans stored back to
  * back (scan b starts at point offset b*stride_points, has n[b] points), d_label a DEVICE pointer with the same layout
  * (int32 per point) that receives the labels. Small per-scan metadata (counts, vertices) is still returned in outs[b]
@@ -251,9 +280,10 @@ void urf_pinned_free(void* p);
  * Detector::filtered() runs, newer scans replace each other and all but the last are dropped. urf_queue keeps that
  * contract available (URF_QUEUE_DROP_OLDEST) but makes it rare: producers (one per LiDAR topic / driver thread) copy
  * their scan into one of `slots` pinned staging buffers and return at once; one worker thread owns the ctx and runs
- * every scan that is pending — up to `max_batch` of them per urf_process_batch call, whose chunked three-stream pipeline
- * overlaps the H2D copy of one chunk with the kernels of the previous one — and consumers take the results in
- * submission order. The ctx must have been created with max_batch >= the queue's max_batch and must not be used by
+ * every scan that is pending — up to `max_batch` of them per batch, whose chunked three-stream pipeline overlaps the H2D
+ * copy of one chunk with the kernels of the previous one, with two batches in flight (urf_enqueue_batch /
+ * urf_finish_batch: the next batch is enqueued before the worker waits for the oldest) — and consumers take the results
+ * in submission order. A scan counts as started (DROP_OLDEST no longer drops it) once its batch has been enqueued. The ctx must have been created with max_batch >= the queue's max_batch and must not be used by
  * anyone else until urf_queue_destroy returns.
  */
 typedef struct urf_queue urf_queue;
@@ -265,7 +295,9 @@ enum { URF_QUEUE_BLOCK = 0, URF_QUEUE_DROP_OLDEST = 1, URF_QUEUE_LABEL8 = 2 };
 enum { URF_ERR_TIMEOUT = -6, URF_ERR_CLOSED = -7 };
 typedef struct urf_queue_stats {
   uint64_t submitted, processed, dropped, delivered, batches;
-  int32_t  largest_batch, pending, reserved;
+  int32_t  largest_batch, pending;
+  int32_t  most_in_flight;       /* most batches the worker had enqueued at once (2 on a real context once a run was
+                                    enqueued behind another; a synchronous stand-in: 1) */
 } urf_queue_stats;
 
 int urf_queue_create(urf_queue** out, urf_ctx* ctx, int max_points, int slots, int max_batch, int policy);
@@ -322,6 +354,13 @@ int urf_queue_submit_cloud2(urf_queue* q, const void* data, int n_points, uint64
 typedef int (*urf_queue_process_fn)(void* user, const float* const* xyzi, const int* n, int batch, urf_result* outs);
 int urf_queue_create_with(urf_queue** out, urf_queue_process_fn fn, void* user, int max_points, int slots, int max_batch,
                           int policy);
+/* Test hook: the worker schedule of a real queue (two batches in flight) around stand-ins for urf_enqueue_batch and
+ * urf_finish_batch: `enqueue` (urf_process_batch's signature) takes a batch and may keep the pointers it is given until the
+ * batch is finished; `finish(user)` completes the OLDEST batch enqueued, fills its outs, and returns its status. The
+ * worker never has more than two batches enqueued. Staging and int8 narrowing as urf_queue_create_with. */
+typedef int (*urf_queue_finish_fn)(void* user);
+int urf_queue_create_with_async(urf_queue** out, urf_queue_process_fn enqueue, urf_queue_finish_fn finish, void* user, int max_points,
+                                int slots, int max_batch, int policy);
 
 /*
  * Multi-GPU ingest (BASELINE config 4: one continuous scan stream sharded across the GPUs of a box). The reference is one

@@ -4,12 +4,13 @@ src/lidar_segmentation.cpp:95). There is no CPU fallback: loading fails loudly w
 every compute call raises without a GPU."""
 from __future__ import annotations
 
+import collections
 import ctypes as C
 import os
 
 import numpy as np
 
-from .ctypes_abi import (UrfMqStats, QUEUE_PROCESS_FN, URF_ERR_CLOSED, URF_ERR_TIMEOUT, URF_MAX_CHANNELS, URF_MAX_VERTS, URF_OK, URF_QUEUE_BLOCK,
+from .ctypes_abi import (UrfMqStats, QUEUE_FINISH_FN, QUEUE_PROCESS_FN, URF_ERR_CLOSED, URF_ERR_TIMEOUT, URF_MAX_CHANNELS, URF_MAX_VERTS, URF_OK, URF_QUEUE_BLOCK,
                          URF_QUEUE_DROP_OLDEST, URF_QUEUE_LABEL8, URF_TOO_FEW_POINTS, UrfClouds, UrfParams, UrfQueueStats, UrfResult,
                          UrfStrip, make_params)
 
@@ -22,7 +23,8 @@ EXPORTS = ["urf_queue_next_batch", "urf_mq_next_batch", "urf_mq_create_label8", 
            "urf_version", "urf_strerror", "urf_last_cuda_error", "urf_default_params", "urf_create", "urf_destroy",
            "urf_set_params", "urf_get_params", "urf_process", "urf_process_batch", "urf_process_batch_device",
            "urf_process_batch_xyz", "urf_process_cloud2_batch", "urf_enqueue_batch_device", "urf_enqueue_batch_device_ex", "urf_finish_batch_device", "urf_stream", "urf_last_device_ms",
-           "urf_last_launch_count", "urf_build_markers", "urf_set_tie_order", "urf_get_tie_order", "urf_mq_set_tie_order"]
+           "urf_last_launch_count", "urf_build_markers", "urf_set_tie_order", "urf_get_tie_order", "urf_mq_set_tie_order",
+           "urf_enqueue_batch", "urf_enqueue_cloud2_batch", "urf_finish_batch", "urf_queue_create_with_async"]
 
 # urf_set_tie_order modes (include/urf.h): equal azimuths inside a ring in input order, or in the reference's Lomuto order
 TIE_ORDERS = {"input": 0, "reference": 1}
@@ -66,6 +68,9 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
     lib.urf_process_cloud2_packed.argtypes = [vp, vp, ip, ip, ip, ip, ip, ip, C.POINTER(UrfResult), C.POINTER(UrfClouds)]
     lib.urf_process_batch_xyz.argtypes = [vp, C.POINTER(vp), C.POINTER(ip), ip, C.POINTER(UrfResult), C.POINTER(vp)]
     lib.urf_process_cloud2_batch.argtypes = [vp, C.POINTER(vp), C.POINTER(ip), ip, ip, ip, ip, ip, ip, C.POINTER(UrfResult), C.POINTER(vp)]
+    lib.urf_enqueue_batch.argtypes = [vp, C.POINTER(vp), C.POINTER(ip), ip, C.POINTER(UrfResult), C.POINTER(vp)]
+    lib.urf_enqueue_cloud2_batch.argtypes = [vp, C.POINTER(vp), C.POINTER(ip), ip, ip, ip, ip, ip, ip, C.POINTER(UrfResult), C.POINTER(vp)]
+    lib.urf_finish_batch.argtypes = [vp]
     lib.urf_process_batch_device.argtypes = [vp, vp, ip, C.POINTER(ip), ip, vp, C.POINTER(UrfResult)]
     lib.urf_enqueue_batch_device.argtypes = [vp, vp, ip, C.POINTER(ip), ip, vp]
     lib.urf_enqueue_batch_device_ex.argtypes = [vp, vp, ip, C.POINTER(ip), ip, vp, vp]
@@ -83,6 +88,7 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
     lib.urf_pinned_free.argtypes = [vp]
     lib.urf_queue_create.argtypes = [C.POINTER(vp), vp, ip, ip, ip, ip]
     lib.urf_queue_create_with.argtypes = [C.POINTER(vp), QUEUE_PROCESS_FN, vp, ip, ip, ip, ip]
+    lib.urf_queue_create_with_async.argtypes = [C.POINTER(vp), QUEUE_PROCESS_FN, QUEUE_FINISH_FN, vp, ip, ip, ip, ip]
     lib.urf_queue_submit.argtypes = [vp, vp, ip, C.c_uint64, ip]
     lib.urf_queue_next.argtypes = [vp, C.POINTER(C.c_uint64), C.POINTER(UrfResult), ip]
     lib.urf_queue_get_stats.argtypes = [vp, C.POINTER(UrfQueueStats)]
@@ -177,6 +183,98 @@ def build_markers(prm: UrfParams, vert: np.ndarray, ghostcount: int = 0):
     return out, gc.value
 
 
+class BatchHandle:
+    """The inputs, arguments and result buffers of one host-buffer batch call. They stay referenced here until the call has
+    finished; `results` (list of ScanResult) is set by collect(), which Detector.finish_batch calls for an enqueued batch.
+    step == 0: float4 scans; step > 0: PointCloud2 records of `step` bytes with x / y / z / intensity at `offs`.
+    pinned: the inputs are copied into, and the results land in, page-locked memory (urf_pinned_alloc), so an enqueued
+    batch's copies run asynchronously; a copy from or to pageable memory makes the enqueue wait for it. Allocating
+    page-locked memory can wait for the device: build handles before enqueueing if batches are to overlap. A handle can be
+    enqueued again once it is finished (collect copies the results out); its page-locked memory is freed by free() or when
+    the handle is dropped."""
+
+    def __init__(self, inputs, ns, want_ring: bool, want_order: bool, label8: bool, step: int = 0, offs=(0, 4, 8, -1),
+                 pinned: bool = False):
+        B = len(inputs)
+        self.lib = load_library()
+        self.step, self.offs, self.pinned = step, tuple(offs), pinned
+        self._pins = []
+        self.inputs = [self._array(a) for a in inputs] if pinned else inputs
+        self.ptrs = (C.c_void_p * B)(*[a.ctypes.data for a in self.inputs])
+        self.ns = (C.c_int * B)(*ns)
+        self.res = (UrfResult * B)()
+        self.l8 = (C.c_void_p * B)() if label8 else None
+        self.bufs = []
+        self.results = None
+        for b, n in enumerate(ns):
+            m = max(n, 1)
+            lab = self._array(np.full(m, -1, np.int8 if label8 else np.int32))
+            ring = self._array(np.full(m, -1, np.int32)) if want_ring else None
+            order = self._array(np.zeros(m, np.int32)) if want_order else None
+            rs = self._array(np.zeros(URF_MAX_CHANNELS + 1, np.int32))
+            if label8:
+                self.l8[b] = lab.ctypes.data
+            else:
+                self.res[b].label = lab.ctypes.data_as(C.POINTER(C.c_int32))
+            if want_ring:
+                self.res[b].ring = ring.ctypes.data_as(C.POINTER(C.c_int32))
+            if want_order:
+                self.res[b].order = order.ctypes.data_as(C.POINTER(C.c_int32))
+            self.res[b].ring_start = rs.ctypes.data_as(C.POINTER(C.c_int32))
+            self.bufs.append((lab, ring, order, rs))
+
+    def _array(self, a: np.ndarray) -> np.ndarray:
+        """`a` itself, or with `pinned` a page-locked copy of it."""
+        if not self.pinned:
+            return a
+        p = self.lib.urf_pinned_alloc(max(a.nbytes, 1))
+        if not p:
+            raise MemoryError("urf_pinned_alloc failed")
+        self._pins.append(p)
+        dst = np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_uint8)), shape=(max(a.nbytes, 1),))[: a.nbytes].view(a.dtype).reshape(a.shape)
+        dst[...] = a
+        return dst
+
+    @classmethod
+    def of_clouds(cls, clouds, want_ring: bool, want_order: bool, label8: bool, pinned: bool = False) -> "BatchHandle":
+        arrs = [np.ascontiguousarray(c, np.float32).reshape(-1, 4) for c in clouds]
+        return cls(arrs, [a.shape[0] for a in arrs], want_ring, want_order, label8, pinned=pinned)
+
+    @classmethod
+    def of_records(cls, records, point_step: int, off_x: int, off_y: int, off_z: int, off_intensity: int, want_ring: bool,
+                   want_order: bool, label8: bool, pinned: bool = False) -> "BatchHandle":
+        raws = [np.ascontiguousarray(r).view(np.uint8).reshape(-1) for r in records]
+        return cls(raws, [r.size // point_step for r in raws], want_ring, want_order, label8, point_step,
+                   (off_x, off_y, off_z, off_intensity), pinned)
+
+    def collect(self) -> list[ScanResult]:
+        """ScanResults of the finished call: labels as int32 (int8 ones widened), ring cut to n_in; copies of page-locked
+        buffers, so they outlive free()."""
+        out = []
+        for b, n in enumerate(self.ns):
+            lab, ring, order, rs = self.bufs[b]
+            lab = lab[:n].astype(np.int32) if self.l8 is not None else lab[:n]
+            ring = None if ring is None else ring[:n]
+            if self.pinned:
+                lab = lab.copy()
+                ring = None if ring is None else ring.copy()
+            out.append(_scan_result(self.res[b], lab, ring, order, rs))
+        self.results = out
+        return out
+
+    def free(self):
+        """Gives the page-locked buffers back; the handle must not be in flight."""
+        for p in self._pins:
+            self.lib.urf_pinned_free(p)
+        self._pins = []
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
+
+
 class Detector:
     """Host-side mirror of the reference's `Detector` (include/urban_road_filter/data_structures.hpp:110-141) on one GPU."""
 
@@ -184,6 +282,7 @@ class Detector:
                  tie_order: str = "input"):
         self.lib = load_library()
         self._ctx = C.c_void_p()
+        self._inflight = collections.deque()         # BatchHandles of enqueue_batch*, oldest first
         rc = self.lib.urf_create(C.byref(self._ctx), device, max_points, max_batch)
         if rc != URF_OK:
             raise UrfError(rc, "urf_create", self.lib.urf_strerror(rc).decode())
@@ -196,8 +295,9 @@ class Detector:
 
     def close(self):
         if getattr(self, "_ctx", None) and self._ctx.value:
-            self.lib.urf_destroy(self._ctx)
+            self.lib.urf_destroy(self._ctx)           # waits for batches in flight, whose buffers _inflight still holds
             self._ctx = C.c_void_p()
+            self._inflight.clear()
 
     def __del__(self):
         try:
@@ -231,69 +331,56 @@ class Detector:
 
     def filtered_batch(self, clouds, want_ring: bool = True, want_order: bool = True) -> list[ScanResult]:
         """`batch` independent Detector::filtered() calls (lidar_segmentation.cpp:95) on host (N,4) float32 arrays."""
-        B = len(clouds)
-        arrs = [np.ascontiguousarray(c, np.float32).reshape(-1, 4) for c in clouds]
-        ptrs = (C.c_void_p * B)(*[a.ctypes.data for a in arrs])
-        ns = (C.c_int * B)(*[a.shape[0] for a in arrs])
-        res = (UrfResult * B)()
-        keep = []
-        for b, a in enumerate(arrs):
-            m = max(a.shape[0], 1)
-            lab = np.full(m, -1, np.int32)
-            ring = np.full(m, -1, np.int32) if want_ring else None
-            order = np.zeros(m, np.int32) if want_order else None
-            rs = np.zeros(URF_MAX_CHANNELS + 1, np.int32)
-            res[b].label = lab.ctypes.data_as(C.POINTER(C.c_int32))
-            if want_ring:
-                res[b].ring = ring.ctypes.data_as(C.POINTER(C.c_int32))
-            if want_order:
-                res[b].order = order.ctypes.data_as(C.POINTER(C.c_int32))
-            res[b].ring_start = rs.ctypes.data_as(C.POINTER(C.c_int32))
-            keep.append((lab, ring, order, rs))
-        self._check(self.lib.urf_process_batch(self._ctx, ptrs, ns, B, res), "urf_process_batch")
-        out = []
-        for b, a in enumerate(arrs):
-            lab, ring, order, rs = keep[b]
-            n = a.shape[0]
-            out.append(_scan_result(res[b], lab[:n], ring[:n] if want_ring else None, order, rs))
-        return out
+        hb = BatchHandle.of_clouds(clouds, want_ring, want_order, label8=False)
+        self._check(self.lib.urf_process_batch(self._ctx, hb.ptrs, hb.ns, len(hb.ns), hb.res), "urf_process_batch")
+        return hb.collect()
 
     def filtered_batch_records(self, records, point_step: int, off_x: int, off_y: int, off_z: int, off_intensity: int = -1,
-                               want_order: bool = False, label8: bool = True) -> list[ScanResult]:
+                               want_order: bool = False, label8: bool = True, want_ring: bool = False) -> list[ScanResult]:
         """`batch` scans given as raw PointCloud2 record arrays (uint8, n * point_step bytes each) of one sensor format,
         unpacked on the device (urf_process_cloud2_batch). point_step == 12 with offsets 0, 4, 8 is the packed-xyz lean
         input of urf_process_batch_xyz, which this method then calls. label8: labels come back as int8."""
-        B = len(records)
-        raws = [np.ascontiguousarray(r).view(np.uint8).reshape(-1) for r in records]
-        ns = [r.size // point_step for r in raws]
-        ptrs = (C.c_void_p * B)(*[r.ctypes.data for r in raws])
-        cn = (C.c_int * B)(*ns)
-        res = (UrfResult * B)()
-        keep = []
-        l8 = (C.c_void_p * B)()
-        for b, n in enumerate(ns):
-            m = max(n, 1)
-            lab = np.full(m, -1, np.int8 if label8 else np.int32)
-            order = np.zeros(m, np.int32) if want_order else None
-            rs = np.zeros(URF_MAX_CHANNELS + 1, np.int32)
-            if label8:
-                l8[b] = lab.ctypes.data
-            else:
-                res[b].label = lab.ctypes.data_as(C.POINTER(C.c_int32))
-            if want_order:
-                res[b].order = order.ctypes.data_as(C.POINTER(C.c_int32))
-            res[b].ring_start = rs.ctypes.data_as(C.POINTER(C.c_int32))
-            keep.append((lab, order, rs))
+        hb = BatchHandle.of_records(records, point_step, off_x, off_y, off_z, off_intensity, want_ring, want_order, label8)
+        B = len(hb.ns)
         if point_step == 12 and (off_x, off_y, off_z) == (0, 4, 8) and off_intensity < 0:
-            self._check(self.lib.urf_process_batch_xyz(self._ctx, ptrs, cn, B, res, l8 if label8 else None), "urf_process_batch_xyz")
+            self._check(self.lib.urf_process_batch_xyz(self._ctx, hb.ptrs, hb.ns, B, hb.res, hb.l8), "urf_process_batch_xyz")
         else:
-            self._check(self.lib.urf_process_cloud2_batch(self._ctx, ptrs, cn, B, point_step, off_x, off_y, off_z, off_intensity, res,
-                                                          l8 if label8 else None), "urf_process_cloud2_batch")
-        out = []
-        for b, n in enumerate(ns):
-            lab, order, rs = keep[b]
-            out.append(_scan_result(res[b], lab[:n].astype(np.int32), None, order, rs))
-        return out
+            self._check(self.lib.urf_process_cloud2_batch(self._ctx, hb.ptrs, hb.ns, B, point_step, off_x, off_y, off_z, off_intensity, hb.res,
+                                                          hb.l8), "urf_process_cloud2_batch")
+        return hb.collect()
+
+    def enqueue(self, hb: "BatchHandle") -> "BatchHandle":
+        """Enqueues a prepared batch (BatchHandle.of_clouds / of_records; urf_enqueue_batch / urf_enqueue_cloud2_batch) and
+        returns at once when its buffers are pinned. finish_batch fills its `results`. At most two batches are in flight;
+        the detector keeps the handle alive until then. While batches are in flight every other compute call and
+        set_params / set_tie_order / set_option raise (URF_ERR_INVALID)."""
+        B = len(hb.ns)
+        if hb.step == 0:
+            rc, where = self.lib.urf_enqueue_batch(self._ctx, hb.ptrs, hb.ns, B, hb.res, hb.l8), "urf_enqueue_batch"
+        else:
+            rc, where = self.lib.urf_enqueue_cloud2_batch(self._ctx, hb.ptrs, hb.ns, B, hb.step, *hb.offs, hb.res, hb.l8), "urf_enqueue_cloud2_batch"
+        self._check(rc, where)
+        self._inflight.append(hb)
+        return hb
+
+    def enqueue_batch(self, clouds, want_ring: bool = True, want_order: bool = True, label8: bool = False) -> "BatchHandle":
+        """filtered_batch without waiting: enqueue() of a pinned handle built here. Allocating its page-locked buffers can
+        wait for a batch already in flight; callers that want batches to overlap build the handles first."""
+        return self.enqueue(BatchHandle.of_clouds(clouds, want_ring, want_order, label8, pinned=True))
+
+    def enqueue_batch_records(self, records, point_step: int, off_x: int, off_y: int, off_z: int, off_intensity: int = -1,
+                              want_order: bool = False, label8: bool = True, want_ring: bool = False) -> "BatchHandle":
+        """filtered_batch_records without waiting (urf_enqueue_cloud2_batch); see enqueue_batch."""
+        return self.enqueue(BatchHandle.of_records(records, point_step, off_x, off_y, off_z, off_intensity, want_ring, want_order, label8,
+                                                   pinned=True))
+
+    def finish_batch(self) -> "BatchHandle":
+        """Waits for the oldest batch in flight (urf_finish_batch), fills its handle's `results` and returns the handle."""
+        rc = self.lib.urf_finish_batch(self._ctx)
+        hb = self._inflight.popleft() if self._inflight else None      # the library frees the slot whatever the outcome
+        self._check(rc, "urf_finish_batch")
+        hb.collect()
+        return hb
 
     def filtered_cloud2(self, data: bytes | np.ndarray, n_points: int, point_step: int, off_x: int, off_y: int, off_z: int) -> ScanResult:
         """One scan from the raw `data` bytes of a sensor_msgs/PointCloud2 (unpacked on the device)."""
@@ -505,11 +592,12 @@ class ScanQueue:
     """Streaming ingest (include/urf.h urf_queue, SURVEY.md §8 f4): producers `submit` scans from any thread, one worker
     thread batches whatever is pending through the detector, `next` returns results in submission order and `next_batch`
     every result that is ready at once. With `process_fn` (a Python callable with urf_process_batch's arguments) the queue
-    runs without a GPU — tests only. label8: int8 label slots (URF_QUEUE_LABEL8) — a quarter of the label traffic and
-    memory; `next` still returns int32 labels, `next_batch` int8 ones."""
+    runs without a GPU — tests only; with `enqueue_fn` and `finish_fn` instead (urf_enqueue_batch's arguments / none) it
+    runs the real queue's two-batches-in-flight schedule around them. label8: int8 label slots (URF_QUEUE_LABEL8) — a
+    quarter of the label traffic and memory; `next` still returns int32 labels, `next_batch` int8 ones."""
 
     def __init__(self, detector: "Detector | None", max_points: int, slots: int = 8, max_batch: int = 4,
-                 policy: int = URF_QUEUE_BLOCK, process_fn=None, label8: bool = False):
+                 policy: int = URF_QUEUE_BLOCK, process_fn=None, label8: bool = False, enqueue_fn=None, finish_fn=None):
         self.lib = load_library()
         self._q = C.c_void_p()
         self.max_points = max_points
@@ -518,7 +606,11 @@ class ScanQueue:
             policy |= URF_QUEUE_LABEL8
         self._cb = None
         self._bufs = None
-        if process_fn is not None:
+        self._keep = {}                   # arrays of by-reference submits, until their results come back
+        if enqueue_fn is not None:
+            self._cb = (QUEUE_PROCESS_FN(enqueue_fn), QUEUE_FINISH_FN(lambda user: finish_fn()))
+            rc = self.lib.urf_queue_create_with_async(C.byref(self._q), *self._cb, None, max_points, slots, max_batch, policy)
+        elif process_fn is not None:
             self._cb = QUEUE_PROCESS_FN(process_fn)
             rc = self.lib.urf_queue_create_with(C.byref(self._q), self._cb, None, max_points, slots, max_batch, policy)
         else:
@@ -528,10 +620,14 @@ class ScanQueue:
         if rc != URF_OK:
             raise UrfError(rc, "urf_queue_create")
 
-    def submit(self, cloud: np.ndarray, tag: int = 0, timeout_ms: int = -1) -> int:
-        """Returns URF_OK, URF_ERR_TIMEOUT or URF_ERR_CLOSED; raises on anything else."""
+    def submit(self, cloud: np.ndarray, tag: int = 0, timeout_ms: int = -1, by_reference: bool = False) -> int:
+        """Returns URF_OK, URF_ERR_TIMEOUT or URF_ERR_CLOSED; raises on anything else. by_reference: no copy
+        (urf_queue_submit_ref): keep the array alive and unchanged until its result has come back."""
         pts = np.ascontiguousarray(cloud, np.float32)
-        rc = self.lib.urf_queue_submit(self._q, pts.ctypes.data, pts.shape[0], tag, timeout_ms)
+        if by_reference:
+            self._keep[tag] = pts
+        submit = self.lib.urf_queue_submit_ref if by_reference else self.lib.urf_queue_submit
+        rc = submit(self._q, pts.ctypes.data, pts.shape[0], tag, timeout_ms)
         if rc not in (URF_OK, URF_ERR_TIMEOUT, URF_ERR_CLOSED):
             raise UrfError(rc, "urf_queue_submit")
         return rc
@@ -547,6 +643,7 @@ class ScanQueue:
             return None
         if rc != URF_OK:
             raise UrfError(rc, "urf_queue_next")
+        self._keep.pop(tag.value, None)
         return int(tag.value), _scan_result(res, lab[: res.n_in].copy())
 
     def next_batch(self, max_results: int, timeout_ms: int = -1, copy: bool = False) -> list:
@@ -555,6 +652,8 @@ class ScanQueue:
         label8), valid until the next next* call, unless `copy`. A scan whose batch failed has status < 0 and label None."""
         self._bufs, out = _next_batch(self.lib.urf_queue_next_batch, self._q, self._bufs, max_results, timeout_ms, self.label8, copy,
                                       "urf_queue_next_batch")
+        for t, _ in out:
+            self._keep.pop(t, None)
         return out
 
     def release(self):
@@ -564,7 +663,7 @@ class ScanQueue:
     def stats(self) -> dict:
         st = UrfQueueStats()
         self.lib.urf_queue_get_stats(self._q, C.byref(st))
-        return {k: int(getattr(st, k)) for k, _ in UrfQueueStats._fields_ if k != "reserved"}
+        return {k: int(getattr(st, k)) for k, _ in UrfQueueStats._fields_}
 
     def close(self):
         if self._q:

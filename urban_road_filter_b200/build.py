@@ -88,15 +88,18 @@ def build_kat() -> None:
                         os.path.join(kat, "lomuto_check.cpp")], check=True)
     # ThreadSanitizer build of the streaming queue around a stand-in batch function (no CUDA involved)
     tgt = os.path.join(bdir, "queue_stress")
-    qsrc = [os.path.join(kat, "queue_stress.cpp"), os.path.join(CSRC, "urf_queue.cpp"), os.path.join(CSRC, "urf_mq.cpp")]
+    qsrc = [os.path.join(kat, "queue_stress.cpp"), os.path.join(CSRC, "urf_queue.cpp"), os.path.join(CSRC, "urf_mq.cpp"),
+            os.path.join(kat, "queue_async_stubs.cpp")]
     qdeps = [os.path.join(ROOT, "include", "urf.h"), os.path.join(CSRC, "urf_queue_internal.hpp")]
     if _stale(tgt, qsrc + qdeps):
         subprocess.run(["g++", "-std=c++17", "-O1", "-g", "-fsanitize=thread", "-pthread", "-o", tgt, *qsrc], check=True)
-    # the same for batched delivery (urf_queue_next_batch / urf_mq_next_batch) and int8 label slots
-    tgt = os.path.join(bdir, "queue_batch_stress")
-    qsrc = [os.path.join(kat, "queue_batch_stress.cpp")] + qsrc[1:]
-    if _stale(tgt, qsrc + qdeps):
-        subprocess.run(["g++", "-std=c++17", "-O1", "-g", "-fsanitize=thread", "-pthread", "-o", tgt, *qsrc], check=True)
+    # the same for batched delivery (urf_queue_next_batch / urf_mq_next_batch) and int8 label slots, and for the worker's
+    # two-batches-in-flight schedule around an asynchronous stand-in
+    for name in ("queue_batch_stress", "queue_async_stress"):
+        tgt = os.path.join(bdir, name)
+        src = [os.path.join(kat, name + ".cpp")] + qsrc[1:]
+        if _stale(tgt, src + qdeps):
+            subprocess.run(["g++", "-std=c++17", "-O1", "-g", "-fsanitize=thread", "-pthread", "-o", tgt, *src], check=True)
 
 
 def build_tools() -> str:

@@ -44,15 +44,36 @@ struct urf_ctx {
   int g_B = -1, g_S = -1, g_order = -1, g_launches = 0;
   unsigned long long g_version = 0, version = 1;
   std::vector<cudaEvent_t> ev_in, ev_comp;        // per chunk: input landed / results ready
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+  cudaEvent_t ev0 = nullptr, ev1 = nullptr;       // the device-resident pair
   DevBuffers buf{};
-  float4* own_in = nullptr;
-  // record staging of the PointCloud2 / packed-xyz entry points: max_points * URF_MAX_POINT_STEP bytes from urf_create, so
-  // single scans never allocate; re-allocated at P * step bytes by the first batch that needs more
-  unsigned char* rawb = nullptr;
-  size_t rawb_bytes = 0;
-  signed char* label8 = nullptr;       // int8 labels (P bytes), allocated when a caller first asks for them
-  int* own_label = nullptr;
+  // A host-buffer batch between its enqueue and its finish (urf_enqueue_batch / urf_finish_batch; the synchronous entry
+  // points are one enqueue and one finish, always in slot 0). A slot holds what the batch's copies touch while the other
+  // batch's kernels run; the per-point workspace is shared, and the kernels of both batches queue on `stream`.
+  // Slot 0 is the context's own set (from urf_create); slot 1 is allocated by the first asynchronous call.
+  struct HostSlot {
+    float4* in = nullptr;
+    // record staging of the PointCloud2 / packed-xyz entry points: slot 0 has max_points * URF_MAX_POINT_STEP bytes from
+    // urf_create, so single scans never allocate; re-allocated at P * step bytes by the first batch that needs more
+    unsigned char* rawb = nullptr;
+    size_t rawb_bytes = 0;
+    int* n = nullptr;
+    int* label = nullptr;
+    signed char* label8 = nullptr;     // int8 labels (P bytes), allocated when a caller first asks for them
+    int* order = nullptr;
+    int* ring = nullptr;               // ring ids for the caller; slot 0 before the first asynchronous call: the sort
+                                       // scratch (buf.sortbuf), see ring_chunk
+    ScanOut* out = nullptr;
+    int* h_n = nullptr;                // pinned
+    ScanOut* h_out = nullptr;          // pinned
+    cudaEvent_t ev0 = nullptr, ev1 = nullptr;   // bracket the batch's kernels
+    cudaEvent_t ev_done = nullptr;              // after the batch's last copy to the host
+    // the batch in flight
+    int batch = 0, S = 0, launches = 0;
+    urf_result* outs = nullptr;
+    urf_clouds* clouds = nullptr;
+  };
+  HostSlot hs[2];
+  int hs_head = 0, hs_count = 0;       // oldest host batch in flight, number in flight (0..2)
   float4* pack = nullptr;              // packed output clouds (urf_process_cloud2_packed): 3 * max_points 32-byte records, allocated on first use
   int* packcnt = nullptr;              // [3][tiles] per-tile counts / offsets
   int* packtot = nullptr;              // [4] cloud sizes
@@ -61,18 +82,16 @@ struct urf_ctx {
   int* h_packtot = nullptr;            // pinned copy
   urf_params params{};
   DevParams dp{};
-  int* h_n = nullptr;          // pinned
   // asynchronous enqueues stage their point counts in a ring of pinned rows, each guarded by the event of its H2D copy,
   // so back-to-back enqueues with different counts never overwrite a row whose copy has not run yet
   static constexpr int kNRing = 8;
   int* h_nring = nullptr;      // pinned, [kNRing][max_batch]
   cudaEvent_t ev_nring[kNRing] = {};
   int nring_pos = 0;
-  ScanOut* h_out = nullptr;    // pinned
   int last_B = 0, last_S = 0;
   int launches = 0;
-  float last_ms = 0.f;
-  bool timing_valid = false;
+  float last_ms = 0.f;                 // device ms of the last finished host batch (timing_host)
+  bool timing_valid = false, timing_host = false;
   std::string err;
   std::vector<void*> allocs;
   // optional per-kernel CUDA-event timing (urf_set_option(ctx, 1, 1)); events live on the ctx stream
@@ -343,14 +362,15 @@ int urf_create(urf_ctx** out, int device, int max_points, int max_batch) {
   CKF(cudaEventCreate(&ctx->ev1));
   const size_t P = ctx->P;
   DevBuffers& b = ctx->buf;
-  TRY(dalloc(ctx, &ctx->own_in, P));
-  ctx->rawb_bytes = (size_t)ctx->max_points * URF_MAX_POINT_STEP;
-  TRY(dalloc(ctx, &ctx->rawb, ctx->rawb_bytes));
+  urf_ctx::HostSlot& h0 = ctx->hs[0];
+  TRY(dalloc(ctx, &h0.in, P));
+  h0.rawb_bytes = (size_t)ctx->max_points * URF_MAX_POINT_STEP;
+  TRY(dalloc(ctx, &h0.rawb, h0.rawb_bytes));
   TRY(dalloc(ctx, &b.alpha_v, P));
   TRY(dalloc(ctx, &b.mark, P));
   TRY(dalloc(ctx, &b.ringid, P));
   TRY(dalloc(ctx, &b.sect, P));
-  TRY(dalloc(ctx, &ctx->own_label, P));
+  TRY(dalloc(ctx, &h0.label, P));
   TRY(dalloc(ctx, &b.bpt, P));
   TRY(dalloc(ctx, &b.sr, P));
   TRY(dalloc(ctx, &b.sz, P));
@@ -376,12 +396,17 @@ int urf_create(urf_ctx** out, int device, int max_points, int max_batch) {
   TRY(dalloc(ctx, &b.n, (size_t)max_batch));
   TRY(dalloc(ctx, &b.out, (size_t)max_batch));
   TRY(dalloc(ctx, &b.tab, (size_t)max_batch));
-  b.in = ctx->own_in;
-  b.label = ctx->own_label;
-  CKF(cudaMallocHost((void**)&ctx->h_n, sizeof(int) * max_batch));
+  b.in = h0.in;
+  b.label = h0.label;
+  h0.n = b.n; h0.order = b.order; h0.out = b.out;
+  h0.ring = reinterpret_cast<int*>(b.sortbuf);
+  CKF(cudaMallocHost((void**)&h0.h_n, sizeof(int) * max_batch));
   CKF(cudaMallocHost((void**)&ctx->h_nring, sizeof(int) * max_batch * urf_ctx::kNRing));
   for (int r = 0; r < urf_ctx::kNRing; r++) CKF(cudaEventCreateWithFlags(&ctx->ev_nring[r], cudaEventDisableTiming));
-  CKF(cudaMallocHost((void**)&ctx->h_out, sizeof(ScanOut) * max_batch));
+  CKF(cudaMallocHost((void**)&h0.h_out, sizeof(ScanOut) * max_batch));
+  CKF(cudaEventCreate(&h0.ev0));
+  CKF(cudaEventCreate(&h0.ev1));
+  CKF(cudaEventCreateWithFlags(&h0.ev_done, cudaEventDisableTiming));
   {
     std::vector<float> ny;
     host_newY(ny, ctx->max_points);
@@ -422,12 +447,16 @@ int urf_create(urf_ctx** out, int device, int max_points, int max_batch) {
 void urf_destroy(urf_ctx* ctx) {
   if (!ctx) return;
   cudaSetDevice(ctx->device);
-  if (ctx->stream) cudaStreamSynchronize(ctx->stream);
+  // host batches still in flight copy into the caller's buffers on s_in / s_out: wait for them too
+  for (cudaStream_t s : {ctx->s_in, ctx->stream, ctx->s_out}) if (s) cudaStreamSynchronize(s);
   for (void* p : ctx->allocs) cudaFree(p);
-  if (ctx->h_n) cudaFreeHost(ctx->h_n);
   if (ctx->h_nring) cudaFreeHost(ctx->h_nring);
   for (cudaEvent_t e : ctx->ev_nring) if (e) cudaEventDestroy(e);
-  if (ctx->h_out) cudaFreeHost(ctx->h_out);
+  for (urf_ctx::HostSlot& h : ctx->hs) {
+    if (h.h_n) cudaFreeHost(h.h_n);
+    if (h.h_out) cudaFreeHost(h.h_out);
+    for (cudaEvent_t e : {h.ev0, h.ev1, h.ev_done}) if (e) cudaEventDestroy(e);
+  }
   if (ctx->h_packtot) cudaFreeHost(ctx->h_packtot);
   if (ctx->gexec) cudaGraphExecDestroy(ctx->gexec);
   for (cudaEvent_t e : ctx->kev) cudaEventDestroy(e);
@@ -456,7 +485,7 @@ void* urf_pinned_alloc(size_t bytes) {
 void urf_pinned_free(void* p) { if (p) cudaFreeHost(p); }
 
 int urf_set_params(urf_ctx* ctx, const urf_params* p) {
-  if (!ctx || !p) return URF_ERR_INVALID;
+  if (!ctx || !p || ctx->hs_count) return URF_ERR_INVALID;
   int rc = validate_params(p);
   if (rc != URF_OK) return rc;
   ctx->params = *p;
@@ -478,7 +507,7 @@ int urf_get_params(const urf_ctx* ctx, urf_params* p) {
 // (sub-batch size, batch graph, shared workspace slots, ring detector and marker search variants, ring detector on the
 // pipeline's own stream, star sort network width) that measured no better than the defaults, which are all that is left.
 int urf_set_option(urf_ctx* ctx, int option, int value) {
-  if (!ctx) return URF_ERR_INVALID;
+  if (!ctx || ctx->hs_count) return URF_ERR_INVALID;
   CK(cudaSetDevice(ctx->device));
   ctx->version++;
   if (option == 0) { ctx->dp.force_exact = value != 0; ctx->version++; return URF_OK; }
@@ -515,7 +544,7 @@ int urf_set_option(urf_ctx* ctx, int option, int value) {
 }
 
 int urf_set_tie_order(urf_ctx* ctx, int mode) {
-  if (!ctx || (mode != URF_TIES_INPUT_ORDER && mode != URF_TIES_REFERENCE)) return URF_ERR_INVALID;
+  if (!ctx || ctx->hs_count || (mode != URF_TIES_INPUT_ORDER && mode != URF_TIES_REFERENCE)) return URF_ERR_INVALID;
   CK(cudaSetDevice(ctx->device));
   if (mode == URF_TIES_REFERENCE && !ctx->buf.lomuto) {   // 4 bytes per point of capacity plus one ring list per scan
     int* epos = nullptr;
@@ -547,6 +576,7 @@ void* urf_stream(urf_ctx* ctx) { return ctx ? (void*)ctx->stream : nullptr; }
 float urf_last_device_ms(const urf_ctx* c) {
   urf_ctx* ctx = const_cast<urf_ctx*>(c);
   if (!ctx || !ctx->timing_valid) return -1.f;
+  if (ctx->timing_host) return ctx->last_ms;
   float ms = -1.f;
   if (cudaEventSynchronize(ctx->ev1) != cudaSuccess) return -1.f;
   if (cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1) != cudaSuccess) return -1.f;
@@ -572,7 +602,7 @@ int urf_profile_get(urf_ctx* ctx, int slot, int idx, const char** name, float* m
 
 int urf_enqueue_batch_device_ex(urf_ctx* ctx, const float* d_xyzi, int stride_points, const int* n, int batch, int32_t* d_label,
                                 int32_t* d_order) {
-  if (!ctx || !d_xyzi || !n || !d_label || batch < 1 || stride_points < 1) return URF_ERR_INVALID;
+  if (!ctx || ctx->hs_count || !d_xyzi || !n || !d_label || batch < 1 || stride_points < 1) return URF_ERR_INVALID;
   if (batch > ctx->max_batch || (size_t)stride_points * batch > ctx->P || stride_points > ctx->max_points) return URF_ERR_CAPACITY;
   CK(cudaSetDevice(ctx->device));
   for (int b = 0; b < batch; b++) if (n[b] < 0 || n[b] > stride_points) return URF_ERR_INVALID;
@@ -614,6 +644,7 @@ int urf_enqueue_batch_device_ex(urf_ctx* ctx, const float* d_xyzi, int stride_po
   CK(cudaEventRecord(ctx->ev1, ctx->stream));
   ctx->launches = launches;
   ctx->timing_valid = true;
+  ctx->timing_host = false;
   ctx->last_B = batch; ctx->last_S = stride_points;
   return URF_OK;
 }
@@ -623,12 +654,13 @@ int urf_enqueue_batch_device(urf_ctx* ctx, const float* d_xyzi, int stride_point
 }
 
 int urf_finish_batch_device(urf_ctx* ctx, urf_result* outs) {
-  if (!ctx) return URF_ERR_INVALID;
+  if (!ctx || ctx->hs_count) return URF_ERR_INVALID;
   CK(cudaSetDevice(ctx->device));
   const int B = ctx->last_B;
-  if (outs) CK(cudaMemcpyAsync(ctx->h_out, ctx->buf.out, sizeof(ScanOut) * B, cudaMemcpyDeviceToHost, ctx->stream));
+  ScanOut* h_out = ctx->hs[0].h_out;
+  if (outs) CK(cudaMemcpyAsync(h_out, ctx->buf.out, sizeof(ScanOut) * B, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  if (outs) for (int b = 0; b < B; b++) fill_result(ctx->h_out[b], &outs[b], false);
+  if (outs) for (int b = 0; b < B; b++) fill_result(h_out[b], &outs[b], false);
   return URF_OK;
 }
 
@@ -645,16 +677,19 @@ namespace {
 // intensity at the given byte offsets (oi < 0: none) — the raw bytes cross PCIe and are unpacked on the device.
 // label8 (or NULL): per scan an int8 HOST buffer for the labels (one byte per point instead of four).
 // clouds (or NULL, batch == 1 only): the four published clouds of the scan, packed on the device.
-int process_batch_impl(urf_ctx* ctx, const void* const* data, const int* n, int batch, int step, int ox, int oy, int oz, int oi,
-                       urf_result* outs, int8_t* const* label8, urf_clouds* clouds) {
+// Enqueues the batch into the next free host slot and returns; finish_batch waits for it and fills outs.
+int enqueue_batch(urf_ctx* ctx, const void* const* data, const int* n, int batch, int step, int ox, int oy, int oz, int oi,
+                  urf_result* outs, int8_t* const* label8, urf_clouds* clouds) {
   if (!ctx || !data || !n || !outs || batch < 1) return URF_ERR_INVALID;
-  if (batch > ctx->max_batch) return URF_ERR_CAPACITY;
+  if (batch > ctx->max_batch || ctx->hs_count == 2) return URF_ERR_CAPACITY;
   if (step != 0) {
     if (step < 12 || step > URF_MAX_POINT_STEP) return URF_ERR_INVALID;
     for (int o : {ox, oy, oz}) if (o < 0 || o + 4 > step) return URF_ERR_INVALID;
     if (oi >= 0 && oi + 4 > step) return URF_ERR_INVALID;
   }
   CK(cudaSetDevice(ctx->device));
+  const int slot = (ctx->hs_head + ctx->hs_count) % 2;
+  urf_ctx::HostSlot& h = ctx->hs[slot];                       // free: its last batch was finished, its copies are done
   int nmax = 1;
   bool want_order = clouds != nullptr, want_ring = false, want_l8 = false;
   for (int b = 0; b < batch; b++) {
@@ -664,20 +699,20 @@ int process_batch_impl(urf_ctx* ctx, const void* const* data, const int* n, int 
     want_order |= outs[b].order != nullptr;
     want_ring |= outs[b].ring != nullptr;
     want_l8 |= label8 && label8[b];
-    ctx->h_n[b] = n[b];
+    h.h_n[b] = n[b];
   }
   const int S = ((nmax + 255) / 256) * 256;
   const int T = (S + kChunk - 1) / kChunk;
-  if ((size_t)batch * S * step > ctx->rawb_bytes) {            // records of a batch beyond the staging buffer: P * step bytes
+  if ((size_t)batch * S * step > h.rawb_bytes) {              // records of a batch beyond the staging buffer: P * step bytes
     CK(cudaStreamSynchronize(ctx->stream));
-    if (ctx->rawb) { cudaFree(ctx->rawb); ctx->allocs.erase(std::find(ctx->allocs.begin(), ctx->allocs.end(), (void*)ctx->rawb)); ctx->rawb = nullptr; }
-    ctx->rawb_bytes = 0;
-    const int rc = dalloc(ctx, &ctx->rawb, ctx->P * (size_t)step);
+    if (h.rawb) { cudaFree(h.rawb); ctx->allocs.erase(std::find(ctx->allocs.begin(), ctx->allocs.end(), (void*)h.rawb)); h.rawb = nullptr; }
+    h.rawb_bytes = 0;
+    const int rc = dalloc(ctx, &h.rawb, ctx->P * (size_t)step);
     if (rc != URF_OK) return rc;
-    ctx->rawb_bytes = ctx->P * (size_t)step;
+    h.rawb_bytes = ctx->P * (size_t)step;
   }
-  if (want_l8 && !ctx->label8) {
-    const int rc = dalloc(ctx, &ctx->label8, ctx->P);
+  if (want_l8 && !h.label8) {
+    const int rc = dalloc(ctx, &h.label8, ctx->P);
     if (rc != URF_OK) return rc;
   }
   if (clouds && !ctx->pack) {                                  // first packed call: 96 bytes per point of capacity
@@ -689,8 +724,9 @@ int process_batch_impl(urf_ctx* ctx, const void* const* data, const int* n, int 
     CK(cudaMallocHost((void**)&ctx->h_packtot, sizeof(int) * 4));
   }
   cudaStream_t st = ctx->stream;
-  DevBuffers bufv = ctx->buf;
-  bufv.label8 = want_l8 ? ctx->label8 : nullptr;
+  DevBuffers bufv = ctx->buf;                                 // slot 0: the same pointers as ctx->buf
+  bufv.in = h.in; bufv.n = h.n; bufv.label = h.label; bufv.order = h.order; bufv.out = h.out;
+  bufv.label8 = want_l8 ? h.label8 : nullptr;
   // Software pipeline over chunks of scans: H2D of chunk c+1 (s_in), kernels of chunk c (stream) and D2H of chunk c-1
   // (s_out) overlap; scans are independent, every chunk owns its slice of every buffer.
   // Chunks of batch / 16 scans. (Tried and dropped: smaller chunks at both ends of the call — a shorter pipeline fill and
@@ -708,8 +744,13 @@ int process_batch_impl(urf_ctx* ctx, const void* const* data, const int* n, int 
     CK(cudaEventCreateWithFlags(&c, cudaEventDisableTiming));
     ctx->ev_in.push_back(a); ctx->ev_comp.push_back(c);
   }
-  int* ring32 = reinterpret_cast<int*>(ctx->buf.sortbuf);     // free once the sorts of a chunk are done (chunk-private slice)
-  const bool graphed = nchunks == 1 && batch <= 8 && !want_l8 && ctx->use_graph && !ctx->profile;
+  // ring ids of chunk c: until the first asynchronous call, slot 0 writes them into the chunk's private slice of the sort
+  // scratch (16 bytes per point), free once the chunk's sorts are done; from then on every slot has a buffer of its own,
+  // because the next batch's sorts overwrite the scratch while this batch's ring ids are still being copied out
+  const bool ring_in_scratch = h.ring == reinterpret_cast<int*>(ctx->buf.sortbuf);
+  auto ring_chunk = [&](int b0) { return h.ring + (size_t)b0 * S * (ring_in_scratch ? 4 : 1); };
+  // the graph holds ctx->buf's pointers, which are slot 0's
+  const bool graphed = slot == 0 && nchunks == 1 && batch <= 8 && !want_l8 && ctx->use_graph && !ctx->profile;
   if (graphed) {
     const int rc = update_graph(ctx, batch, S, want_order);
     if (rc != URF_OK) return rc;
@@ -718,11 +759,11 @@ int process_batch_impl(urf_ctx* ctx, const void* const* data, const int* n, int 
   // for this thread to get through a chunk's kernel launches and result copies
   for (int c = 0; c < nchunks; c++) {
     const int b0 = cb[c], nb = cb[c + 1] - b0;
-    CK(cudaMemcpyAsync(ctx->buf.n + b0, ctx->h_n + b0, sizeof(int) * nb, cudaMemcpyHostToDevice, ctx->s_in));
+    CK(cudaMemcpyAsync(h.n + b0, h.h_n + b0, sizeof(int) * nb, cudaMemcpyHostToDevice, ctx->s_in));
     for (int b = b0; b < b0 + nb; b++) {
       if (n[b] <= 0) continue;
-      if (step == 0) CK(cudaMemcpyAsync(ctx->own_in + (size_t)b * S, data[b], sizeof(float) * 4 * (size_t)n[b], cudaMemcpyHostToDevice, ctx->s_in));
-      else CK(cudaMemcpyAsync(ctx->rawb + (size_t)b * S * step, data[b], (size_t)step * (size_t)n[b], cudaMemcpyHostToDevice, ctx->s_in));
+      if (step == 0) CK(cudaMemcpyAsync(h.in + (size_t)b * S, data[b], sizeof(float) * 4 * (size_t)n[b], cudaMemcpyHostToDevice, ctx->s_in));
+      else CK(cudaMemcpyAsync(h.rawb + (size_t)b * S * step, data[b], (size_t)step * (size_t)n[b], cudaMemcpyHostToDevice, ctx->s_in));
     }
     CK(cudaEventRecord(ctx->ev_in[c], ctx->s_in));
   }
@@ -731,21 +772,21 @@ int process_batch_impl(urf_ctx* ctx, const void* const* data, const int* n, int 
     const int b0 = cb[c], nb = cb[c + 1] - b0;
     CK(cudaStreamWaitEvent(st, ctx->ev_in[c], 0));
     if (step != 0)
-      k_unpack_cloud2_batch<<<dim3((S + 255) / 256, nb), 256, 0, st>>>(ctx->rawb + (size_t)b0 * S * step, ctx->own_in + (size_t)b0 * S, ctx->buf.n + b0, S,
+      k_unpack_cloud2_batch<<<dim3((S + 255) / 256, nb), 256, 0, st>>>(h.rawb + (size_t)b0 * S * step, h.in + (size_t)b0 * S, h.n + b0, S,
                                                                           step, ox, oy, oz, oi);
     const DevBuffers view = offset_view(bufv, b0, S, T, ctx->dp.channels);
     // ev0 / ev1 bracket the kernels of the whole call: before the first chunk's pipeline, after the last one's
     int L = graphed ? ctx->g_launches : 0;
-    int rc = c == 0 ? cuda_rc(ctx, cudaEventRecord(ctx->ev0, st), "cudaEventRecord(ev0)") : URF_OK;
+    int rc = c == 0 ? cuda_rc(ctx, cudaEventRecord(h.ev0, st), "cudaEventRecord(ev0)") : URF_OK;
     if (rc == URF_OK)
       rc = graphed ? cuda_rc(ctx, cudaGraphLaunch(ctx->gexec, st), "cudaGraphLaunch") : launch_pipeline(ctx, view, nb, S, want_order, urf_ctx::kGroups, &L);
-    if (rc == URF_OK && c == nchunks - 1) rc = cuda_rc(ctx, cudaEventRecord(ctx->ev1, st), "cudaEventRecord(ev1)");
+    if (rc == URF_OK && c == nchunks - 1) rc = cuda_rc(ctx, cudaEventRecord(h.ev1, st), "cudaEventRecord(ev1)");
     if (rc != URF_OK) {                                 // nothing of this call may still be writing into the caller's buffers
       cudaStreamSynchronize(ctx->s_in); cudaStreamSynchronize(st); cudaStreamSynchronize(ctx->s_out);
       return rc;
     }
     launches += L;
-    if (want_ring) k_ring32<<<dim3((S + 255) / 256, nb), 256, 0, st>>>(view, ring32 + (size_t)b0 * S * 4, S);
+    if (want_ring) k_ring32<<<dim3((S + 255) / 256, nb), 256, 0, st>>>(view, ring_chunk(b0), S);
     if (clouds) {                                       // batch == 1: pack scan 0, sizes to the host with the results
       const int nt = (std::max(n[0], 1) + kPackTile - 1) / kPackTile;
       k_pack_count<<<nt, 256, 0, st>>>(ctx->buf, ctx->packcnt, nt);
@@ -757,17 +798,32 @@ int process_batch_impl(urf_ctx* ctx, const void* const* data, const int* n, int 
     }
     CK(cudaEventRecord(ctx->ev_comp[c], st));
     CK(cudaStreamWaitEvent(ctx->s_out, ctx->ev_comp[c], 0));
-    CK(cudaMemcpyAsync(ctx->h_out + b0, ctx->buf.out + b0, sizeof(ScanOut) * nb, cudaMemcpyDeviceToHost, ctx->s_out));
+    CK(cudaMemcpyAsync(h.h_out + b0, h.out + b0, sizeof(ScanOut) * nb, cudaMemcpyDeviceToHost, ctx->s_out));
     for (int b = b0; b < b0 + nb; b++) {
       if (n[b] <= 0) continue;
-      if (outs[b].label) CK(cudaMemcpyAsync(outs[b].label, ctx->own_label + (size_t)b * S, sizeof(int) * (size_t)n[b], cudaMemcpyDeviceToHost, ctx->s_out));
-      if (label8 && label8[b]) CK(cudaMemcpyAsync(label8[b], ctx->label8 + (size_t)b * S, (size_t)n[b], cudaMemcpyDeviceToHost, ctx->s_out));
-      if (outs[b].ring) CK(cudaMemcpyAsync(outs[b].ring, ring32 + (size_t)b0 * S * 4 + (size_t)(b - b0) * S, sizeof(int) * (size_t)n[b], cudaMemcpyDeviceToHost, ctx->s_out));
-      if (outs[b].order) CK(cudaMemcpyAsync(outs[b].order, ctx->buf.order + (size_t)b * S, sizeof(int) * (size_t)n[b], cudaMemcpyDeviceToHost, ctx->s_out));
+      if (outs[b].label) CK(cudaMemcpyAsync(outs[b].label, h.label + (size_t)b * S, sizeof(int) * (size_t)n[b], cudaMemcpyDeviceToHost, ctx->s_out));
+      if (label8 && label8[b]) CK(cudaMemcpyAsync(label8[b], h.label8 + (size_t)b * S, (size_t)n[b], cudaMemcpyDeviceToHost, ctx->s_out));
+      if (outs[b].ring) CK(cudaMemcpyAsync(outs[b].ring, ring_chunk(b0) + (size_t)(b - b0) * S, sizeof(int) * (size_t)n[b], cudaMemcpyDeviceToHost, ctx->s_out));
+      if (outs[b].order) CK(cudaMemcpyAsync(outs[b].order, h.order + (size_t)b * S, sizeof(int) * (size_t)n[b], cudaMemcpyDeviceToHost, ctx->s_out));
     }
   }
-  CK(cudaStreamSynchronize(ctx->s_out));
-  CK(cudaStreamSynchronize(st));
+  // s_out waited for the last chunk's kernels: ev_done covers every copy and kernel of the batch
+  CK(cudaEventRecord(h.ev_done, ctx->s_out));
+  h.batch = batch; h.S = S; h.launches = launches; h.outs = outs; h.clouds = clouds;
+  ctx->hs_count++;
+  return URF_OK;
+}
+
+// Waits for the oldest host batch in flight and fills its outs (the slot is free again whatever the outcome).
+int finish_batch(urf_ctx* ctx) {
+  if (!ctx || ctx->hs_count == 0) return URF_ERR_INVALID;
+  urf_ctx::HostSlot& h = ctx->hs[ctx->hs_head];
+  ctx->hs_count--;
+  ctx->hs_head = ctx->hs_count ? 1 - ctx->hs_head : 0;       // idle: the next batch (and every synchronous call) takes slot 0
+  CK(cudaSetDevice(ctx->device));
+  CK(cudaEventSynchronize(h.ev_done));
+  cudaStream_t st = ctx->stream;
+  urf_clouds* clouds = h.clouds;
   if (clouds) {                                              // sizes are known now: copy exactly the records that exist
     const int* t = ctx->h_packtot;
     const float4 *d_rc = ctx->pack, *d_roi = ctx->pack + 2 * (size_t)ctx->max_points, *d_prob = ctx->pack + 4 * (size_t)ctx->max_points;
@@ -779,16 +835,75 @@ int process_batch_impl(urf_ctx* ctx, const void* const* data, const int* n, int 
     if (clouds->road_probably && t[3] > 0) CK(cudaMemcpyAsync(clouds->road_probably, d_prob, rec * t[3], cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
   }
-  ctx->launches = launches;
+  float ms = -1.f;
+  if (cudaEventElapsedTime(&ms, h.ev0, h.ev1) != cudaSuccess) ms = -1.f;
+  ctx->last_ms = ms;
+  ctx->launches = h.launches;
   ctx->timing_valid = true;
-  ctx->last_B = batch; ctx->last_S = S;
-  for (int b = 0; b < batch; b++) {
-    fill_result(ctx->h_out[b], &outs[b], true);
-    if (outs[b].status == URF_TOO_FEW_POINTS && outs[b].ring) for (int i = 0; i < n[b]; i++) outs[b].ring[i] = -1;
+  ctx->timing_host = true;
+  ctx->last_B = h.batch; ctx->last_S = h.S;
+  urf_result* outs = h.outs;
+  for (int b = 0; b < h.batch; b++) {
+    fill_result(h.h_out[b], &outs[b], true);
+    if (outs[b].status == URF_TOO_FEW_POINTS && outs[b].ring) for (int i = 0; i < h.h_n[b]; i++) outs[b].ring[i] = -1;
   }
   return URF_OK;
 }
+
+// The second host slot, and slot 0's own ring-id buffer (include/urf.h: 32 bytes of device memory per point of capacity),
+// on the first asynchronous call (nothing is in flight then).
+int alloc_second_slot(urf_ctx* ctx) {
+  urf_ctx::HostSlot& h = ctx->hs[1];
+  if (h.ev_done) return URF_OK;
+  CK(cudaSetDevice(ctx->device));
+  const size_t P = ctx->P;
+  urf_ctx::HostSlot t;
+  int* ring0 = nullptr;
+  int rc = dalloc(ctx, &t.in, P);
+  if (rc == URF_OK) rc = dalloc(ctx, &t.label, P);
+  if (rc == URF_OK) rc = dalloc(ctx, &t.order, P);
+  if (rc == URF_OK) rc = dalloc(ctx, &t.ring, P);
+  if (rc == URF_OK) rc = dalloc(ctx, &ring0, P);
+  if (rc == URF_OK) rc = dalloc(ctx, &t.n, (size_t)ctx->max_batch);
+  if (rc == URF_OK) rc = dalloc(ctx, &t.out, (size_t)ctx->max_batch);
+  if (rc != URF_OK) return rc;                              // device pieces stay in ctx->allocs until urf_destroy
+  if (!h.h_n) rc = cuda_rc(ctx, cudaMallocHost((void**)&h.h_n, sizeof(int) * ctx->max_batch), "cudaMallocHost");
+  if (rc == URF_OK && !h.h_out) rc = cuda_rc(ctx, cudaMallocHost((void**)&h.h_out, sizeof(ScanOut) * ctx->max_batch), "cudaMallocHost");
+  if (rc == URF_OK && !h.ev0) rc = cuda_rc(ctx, cudaEventCreate(&h.ev0), "cudaEventCreate");
+  if (rc == URF_OK && !h.ev1) rc = cuda_rc(ctx, cudaEventCreate(&h.ev1), "cudaEventCreate");
+  if (rc != URF_OK) return rc;                              // pinned pieces and events are freed by urf_destroy
+  h.in = t.in; h.label = t.label; h.order = t.order; h.ring = t.ring; h.n = t.n; h.out = t.out;
+  ctx->hs[0].ring = ring0;
+  return cuda_rc(ctx, cudaEventCreateWithFlags(&h.ev_done, cudaEventDisableTiming), "cudaEventCreate");   // last: marks the slot complete
+}
+
+// The synchronous entry points: one enqueue and one finish, refused while asynchronous batches are in flight.
+int process_batch_impl(urf_ctx* ctx, const void* const* data, const int* n, int batch, int step, int ox, int oy, int oz, int oi,
+                       urf_result* outs, int8_t* const* label8, urf_clouds* clouds) {
+  if (ctx && ctx->hs_count) return URF_ERR_INVALID;
+  const int rc = enqueue_batch(ctx, data, n, batch, step, ox, oy, oz, oi, outs, label8, clouds);
+  return rc != URF_OK ? rc : finish_batch(ctx);
+}
+
+int enqueue_async(urf_ctx* ctx, const void* const* data, const int* n, int batch, int step, int ox, int oy, int oz, int oi,
+                  urf_result* outs, int8_t* const* label8) {
+  if (!ctx) return URF_ERR_INVALID;
+  const int rc = alloc_second_slot(ctx);
+  return rc != URF_OK ? rc : enqueue_batch(ctx, data, n, batch, step, ox, oy, oz, oi, outs, label8, nullptr);
+}
 }  // namespace
+
+int urf_enqueue_batch(urf_ctx* ctx, const float* const* xyzi, const int* n, int batch, urf_result* outs, int8_t* const* label8) {
+  return enqueue_async(ctx, reinterpret_cast<const void* const*>(xyzi), n, batch, 0, 0, 0, 0, -1, outs, label8);
+}
+
+int urf_enqueue_cloud2_batch(urf_ctx* ctx, const void* const* data, const int* n_points, int batch, int point_step, int off_x, int off_y,
+                             int off_z, int off_intensity, urf_result* outs, int8_t* const* label8) {
+  if (point_step == 0) return URF_ERR_INVALID;
+  return enqueue_async(ctx, data, n_points, batch, point_step, off_x, off_y, off_z, off_intensity, outs, label8);
+}
+
+int urf_finish_batch(urf_ctx* ctx) { return finish_batch(ctx); }
 
 int urf_process_batch(urf_ctx* ctx, const float* const* xyzi, const int* n, int batch, urf_result* outs) {
   return process_batch_impl(ctx, reinterpret_cast<const void* const*>(xyzi), n, batch, 0, 0, 0, 0, -1, outs, nullptr, nullptr);

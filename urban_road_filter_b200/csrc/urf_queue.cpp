@@ -11,13 +11,19 @@
 // consumer waits for the smallest live one. urf_queue_next_batch hands out the whole run of DONE slots that follows it.
 //
 // Label slots are int32, or int8 with URF_QUEUE_LABEL8: the worker then asks the batch body for one-byte labels (float4
-// queues go through urf_process_cloud2_batch with 16-byte records, which has the label8 output urf_process_batch lacks).
+// queues go through urf_enqueue_cloud2_batch with 16-byte records, as the synchronous path went through
+// urf_process_cloud2_batch).
+//
+// On a real context the worker keeps two batches in flight (urf_enqueue_batch / urf_finish_batch): it enqueues what is
+// pending, enqueues the next pending run too if there is one, and only then waits for the oldest batch, so the copies of
+// one batch overlap the kernels of the other and the device does not wait for the host's round trip between batches.
 #include <algorithm>
 #include <chrono>
 #include <condition_variable>
 #include <cstddef>
 #include <cstdlib>
 #include <cstring>
+#include <deque>
 #include <mutex>
 #include <thread>
 #include <vector>
@@ -40,7 +46,10 @@ struct Slot {
 }  // namespace
 
 struct urf_queue {
-  urf_queue_process_fn fn = nullptr;
+  urf_ctx* ctx = nullptr;                  // real queue: batches go through urf_enqueue*_batch / urf_finish_batch
+  urf_queue_process_fn fn = nullptr;       // stand-in, synchronous (urf_queue_create_with)
+  urf_queue_process_fn enq = nullptr;      // stand-in, asynchronous pair (urf_queue_create_with_async)
+  urf_queue_finish_fn fin = nullptr;
   void* user = nullptr;
   bool pinned = false;
   int max_points = 0, max_batch = 1, policy = URF_QUEUE_BLOCK;
@@ -62,82 +71,133 @@ struct urf_queue {
 
 namespace {
 
-int real_process(void* user, const float* const* xyzi, const int* n, int batch, urf_result* outs) {
-  return urf_process_batch(static_cast<urf_ctx*>(user), xyzi, n, batch, outs);
-}
-
 template <class Pred>
 bool wait_for(std::condition_variable& cv, std::unique_lock<std::mutex>& lk, int timeout_ms, Pred pred) {
   if (timeout_ms < 0) { cv.wait(lk, pred); return true; }
   return cv.wait_for(lk, std::chrono::milliseconds(timeout_ms), pred);
 }
 
-void worker_loop(urf_queue* q) {
+// One batch of the worker: the slots it took and the arguments of its batch call (which must outlive an asynchronous
+// batch until its finish).
+struct Run {
   std::vector<int> idx;
   std::vector<const float*> ptrs;
   std::vector<int> ns;
   std::vector<urf_result> outs;
   std::vector<int8_t*> l8;
-  for (;;) {
-    idx.clear();
-    {
-      std::unique_lock<std::mutex> lk(q->mu);
+};
+
+// Takes every pending scan, oldest first, up to max_batch, into r (the slots become RUNNING: from here on they count as
+// started and DROP_OLDEST no longer drops them). wait: first block until a scan is pending or the queue is closed.
+// Returns the number taken; *closed tells whether the queue was closed.
+int take_run(urf_queue* q, Run& r, bool wait, bool* closed) {
+  r.idx.clear();
+  {
+    std::unique_lock<std::mutex> lk(q->mu);
+    if (wait)
       q->cv_pending.wait(lk, [&] {
         if (q->closed) return true;
         for (const Slot& s : q->slots) if (s.state == PENDING) return true;
         return false;
       });
-      // everything pending, oldest first, up to max_batch
-      for (;;) {
-        int best = -1;
-        for (int i = 0; i < (int)q->slots.size(); i++) {
-          const Slot& s = q->slots[i];
-          if (s.state == PENDING && (best < 0 || s.seq < q->slots[best].seq)) best = i;
-        }
-        if (best < 0 || (int)idx.size() >= q->max_batch) break;
-        q->slots[best].state = RUNNING;
-        idx.push_back(best);
+    for (;;) {
+      int best = -1;
+      for (int i = 0; i < (int)q->slots.size(); i++) {
+        const Slot& s = q->slots[i];
+        if (s.state == PENDING && (best < 0 || s.seq < q->slots[best].seq)) best = i;
       }
-      if (idx.empty()) { if (q->closed) return; continue; }
-      q->st.batches++;
-      if ((int)idx.size() > q->st.largest_batch) q->st.largest_batch = (int)idx.size();
+      if (best < 0 || (int)r.idx.size() >= q->max_batch) break;
+      q->slots[best].state = RUNNING;
+      r.idx.push_back(best);
     }
-    const int B = (int)idx.size();
-    ptrs.resize(B); ns.resize(B); l8.resize(B); outs.assign(B, urf_result{});
-    const bool stand_in = q->fn != real_process;
-    for (int j = 0; j < B; j++) {
-      Slot& s = q->slots[idx[j]];
-      ptrs[j] = s.ext ? s.ext : s.in; ns[j] = s.n;
-      outs[j].label = s.label;                          // NULL in a real int8 queue: no int32 label copy is issued
-      l8[j] = s.label8;
-    }
-    int rc;
-    if (stand_in) {
-      rc = q->fn(q->user, ptrs.data(), ns.data(), B, outs.data());
-      if (q->label8 && rc == URF_OK)                    // a stand-in writes int32 labels: the queue narrows them into the slot
-        for (int j = 0; j < B; j++) {
-          const Slot& s = q->slots[idx[j]];
-          for (int i = 0; i < s.n; i++) s.label8[i] = (int8_t)s.label[i];
-        }
-    } else if (q->step == 0 && !q->label8) {
-      rc = q->fn(q->user, ptrs.data(), ns.data(), B, outs.data());
-    } else {
-      // float4 scans with int8 labels are 16-byte records (x, y, z, intensity at 0, 4, 8, 12) to the record body
-      const bool f4 = q->step == 0;
-      rc = urf_process_cloud2_batch(static_cast<urf_ctx*>(q->user), reinterpret_cast<const void* const*>(ptrs.data()), ns.data(), B,
-                                    f4 ? 16 : q->step, f4 ? 0 : q->ox, f4 ? 4 : q->oy, f4 ? 8 : q->oz, f4 ? 12 : q->oi, outs.data(),
-                                    q->label8 ? l8.data() : nullptr);
-    }
-    {
-      std::lock_guard<std::mutex> lk(q->mu);
-      for (int j = 0; j < B; j++) {
-        Slot& s = q->slots[idx[j]];
-        s.res = outs[j]; s.rc = rc; s.state = DONE;
-        q->st.processed++;
-      }
-    }
-    q->cv_done.notify_all();
+    *closed = q->closed;
+    if (r.idx.empty()) return 0;
+    q->st.batches++;
+    if ((int)r.idx.size() > q->st.largest_batch) q->st.largest_batch = (int)r.idx.size();
   }
+  const int B = (int)r.idx.size();
+  r.ptrs.resize(B); r.ns.resize(B); r.l8.resize(B); r.outs.assign(B, urf_result{});
+  for (int j = 0; j < B; j++) {                           // RUNNING slots belong to the worker: read outside the lock
+    const Slot& s = q->slots[r.idx[j]];
+    r.ptrs[j] = s.ext ? s.ext : s.in; r.ns[j] = s.n;
+    r.outs[j].label = s.label;                            // NULL in a real int8 queue: no int32 label copy is issued
+    r.l8[j] = s.label8;
+  }
+  return B;
+}
+
+// Publishes a finished (or failed) run: its slots become DONE with status rc.
+void complete_run(urf_queue* q, const Run& r, int rc) {
+  if (!q->ctx && q->label8 && rc == URF_OK)               // a stand-in writes int32 labels: the queue narrows them into the slot
+    for (int i : r.idx) {
+      const Slot& s = q->slots[i];
+      for (int k = 0; k < s.n; k++) s.label8[k] = (int8_t)s.label[k];
+    }
+  {
+    std::lock_guard<std::mutex> lk(q->mu);
+    for (size_t j = 0; j < r.idx.size(); j++) {
+      Slot& s = q->slots[r.idx[j]];
+      s.res = r.outs[j]; s.rc = rc; s.state = DONE;
+      q->st.processed++;
+    }
+  }
+  q->cv_done.notify_all();
+}
+
+int enqueue_run(urf_queue* q, Run& r) {
+  const int B = (int)r.idx.size();
+  if (q->enq) return q->enq(q->user, r.ptrs.data(), r.ns.data(), B, r.outs.data());
+  if (q->step == 0 && !q->label8) return urf_enqueue_batch(q->ctx, r.ptrs.data(), r.ns.data(), B, r.outs.data(), nullptr);
+  // float4 scans with int8 labels are 16-byte records (x, y, z, intensity at 0, 4, 8, 12) to the record body
+  const bool f4 = q->step == 0;
+  return urf_enqueue_cloud2_batch(q->ctx, reinterpret_cast<const void* const*>(r.ptrs.data()), r.ns.data(), B, f4 ? 16 : q->step,
+                                  f4 ? 0 : q->ox, f4 ? 4 : q->oy, f4 ? 8 : q->oz, f4 ? 12 : q->oi, r.outs.data(),
+                                  q->label8 ? r.l8.data() : nullptr);
+}
+
+void note_in_flight(urf_queue* q, int k) {
+  std::lock_guard<std::mutex> lk(q->mu);
+  if (k > q->st.most_in_flight) q->st.most_in_flight = k;
+}
+
+// Synchronous stand-in (urf_queue_create_with): one batch call at a time.
+void worker_loop_sync(urf_queue* q) {
+  Run r;
+  for (;;) {
+    bool closed = false;
+    if (!take_run(q, r, true, &closed)) { if (closed) return; continue; }
+    note_in_flight(q, 1);
+    complete_run(q, r, q->fn(q->user, r.ptrs.data(), r.ns.data(), (int)r.idx.size(), r.outs.data()));
+  }
+}
+
+// Two batches in flight: enqueue what is pending, enqueue the next pending run while a batch slot is free, then finish the
+// oldest batch. The queue drains what was accepted before a close before the worker returns.
+void worker_loop_async(urf_queue* q) {
+  std::deque<Run> flight;                                 // enqueued, oldest first (at most two)
+  for (;;) {
+    while (flight.size() < 2) {
+      Run r;
+      bool closed = false;
+      if (!take_run(q, r, flight.empty(), &closed)) {
+        if (flight.empty() && closed) return;
+        break;
+      }
+      const int rc = enqueue_run(q, r);
+      if (rc != URF_OK) { complete_run(q, r, rc); continue; }   // nothing of a refused batch is in flight
+      flight.push_back(std::move(r));                     // the vectors' storage, which the batch points at, moves along
+      note_in_flight(q, (int)flight.size());
+    }
+    if (flight.empty()) continue;
+    const int rc = q->fin ? q->fin(q->user) : urf_finish_batch(q->ctx);
+    complete_run(q, flight.front(), rc);
+    flight.pop_front();
+  }
+}
+
+void worker_loop(urf_queue* q) {
+  if (q->fn) worker_loop_sync(q);
+  else worker_loop_async(q);
 }
 
 void free_slot(const urf_queue* q, Slot& s) {
@@ -147,20 +207,24 @@ void free_slot(const urf_queue* q, Slot& s) {
   s.in = nullptr; s.label = nullptr; s.label8 = nullptr;
 }
 
-int create_common(urf_queue** out, urf_queue_process_fn fn, void* user, bool pinned, int max_points, int slots, int max_batch, int policy,
-                  int step = 0, int ox = 0, int oy = 4, int oz = 8, int oi = -1) {
+// Exactly one of ctx (real queue, pinned slots), fn (synchronous stand-in) and enq + fin (asynchronous stand-in) is set.
+int create_common(urf_queue** out, urf_ctx* ctx, urf_queue_process_fn fn, urf_queue_process_fn enq, urf_queue_finish_fn fin, void* user,
+                  int max_points, int slots, int max_batch, int policy, int step = 0, int ox = 0, int oy = 4, int oz = 8, int oi = -1) {
   const bool label8 = (policy & URF_QUEUE_LABEL8) != 0;
   policy &= ~URF_QUEUE_LABEL8;
-  if (!out || !fn || max_points < 1 || slots < 1 || max_batch < 1 || (policy != URF_QUEUE_BLOCK && policy != URF_QUEUE_DROP_OLDEST))
+  if (!out || (!ctx && !fn && !(enq && fin)) || max_points < 1 || slots < 1 || max_batch < 1 ||
+      (policy != URF_QUEUE_BLOCK && policy != URF_QUEUE_DROP_OLDEST))
     return URF_ERR_INVALID;
+  const bool pinned = ctx != nullptr;
   urf_queue* q = new urf_queue;
-  q->fn = fn; q->user = user; q->pinned = pinned; q->max_points = max_points; q->max_batch = max_batch; q->policy = policy;
+  q->ctx = ctx; q->fn = fn; q->enq = enq; q->fin = fin; q->user = user;
+  q->pinned = pinned; q->max_points = max_points; q->max_batch = max_batch; q->policy = policy;
   q->label8 = label8;
   q->step = step; q->ox = ox; q->oy = oy; q->oz = oz; q->oi = oi;
   q->bytes_per_point = step > 0 ? (size_t)step : 16;
   q->slots.resize(slots);
   // int8 slots hold max_points bytes of labels; a stand-in batch function still writes int32 labels, which need a buffer
-  const bool want32 = !label8 || fn != real_process, want8 = label8;
+  const bool want32 = !label8 || !ctx, want8 = label8;
   auto alloc = [pinned](size_t bytes) { return pinned ? urf_pinned_alloc(bytes) : std::malloc(bytes); };
   for (Slot& s : q->slots) {
     const size_t in_bytes = q->bytes_per_point * (size_t)max_points;
@@ -184,7 +248,7 @@ extern "C" {
 
 int urf_queue_create(urf_queue** out, urf_ctx* ctx, int max_points, int slots, int max_batch, int policy) {
   if (!ctx) return URF_ERR_INVALID;
-  return create_common(out, real_process, ctx, true, max_points, slots, max_batch, policy);
+  return create_common(out, ctx, nullptr, nullptr, nullptr, nullptr, max_points, slots, max_batch, policy);
 }
 
 int urf_queue_create_cloud2(urf_queue** out, urf_ctx* ctx, int max_points, int slots, int max_batch, int policy, int point_step, int off_x,
@@ -192,11 +256,19 @@ int urf_queue_create_cloud2(urf_queue** out, urf_ctx* ctx, int max_points, int s
   if (!ctx || point_step < 12 || point_step > URF_MAX_POINT_STEP) return URF_ERR_INVALID;
   for (int o : {off_x, off_y, off_z}) if (o < 0 || o + 4 > point_step) return URF_ERR_INVALID;
   if (off_intensity >= 0 && off_intensity + 4 > point_step) return URF_ERR_INVALID;
-  return create_common(out, real_process, ctx, true, max_points, slots, max_batch, policy, point_step, off_x, off_y, off_z, off_intensity);
+  return create_common(out, ctx, nullptr, nullptr, nullptr, nullptr, max_points, slots, max_batch, policy, point_step, off_x, off_y, off_z,
+                       off_intensity);
 }
 
 int urf_queue_create_with(urf_queue** out, urf_queue_process_fn fn, void* user, int max_points, int slots, int max_batch, int policy) {
-  return create_common(out, fn, user, false, max_points, slots, max_batch, policy);
+  if (!fn) return URF_ERR_INVALID;
+  return create_common(out, nullptr, fn, nullptr, nullptr, user, max_points, slots, max_batch, policy);
+}
+
+int urf_queue_create_with_async(urf_queue** out, urf_queue_process_fn enqueue, urf_queue_finish_fn finish, void* user, int max_points,
+                                int slots, int max_batch, int policy) {
+  if (!enqueue || !finish) return URF_ERR_INVALID;
+  return create_common(out, nullptr, nullptr, enqueue, finish, user, max_points, slots, max_batch, policy);
 }
 
 namespace {

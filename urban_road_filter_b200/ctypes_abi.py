@@ -81,7 +81,7 @@ class UrfClouds(C.Structure):
 
 class UrfQueueStats(C.Structure):
     _fields_ = [("submitted", C.c_uint64), ("processed", C.c_uint64), ("dropped", C.c_uint64), ("delivered", C.c_uint64),
-                ("batches", C.c_uint64), ("largest_batch", C.c_int32), ("pending", C.c_int32), ("reserved", C.c_int32)]
+                ("batches", C.c_uint64), ("largest_batch", C.c_int32), ("pending", C.c_int32), ("most_in_flight", C.c_int32)]
 
 
 URF_MQ_MAX_DEVICES = 16
@@ -98,6 +98,8 @@ URF_QUEUE_LABEL8 = 2          # OR-ed into the policy: int8 label slots
 URF_ERR_TIMEOUT, URF_ERR_CLOSED = -6, -7
 # int (*)(void* user, const float* const* xyzi, const int* n, int batch, urf_result* outs)
 QUEUE_PROCESS_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.c_int, C.POINTER(UrfResult))
+# int (*)(void* user): finishes the oldest batch of an asynchronous stand-in (urf_queue_create_with_async)
+QUEUE_FINISH_FN = C.CFUNCTYPE(C.c_int, C.c_void_p)
 
 
 # cfg/LidarFilters.cfg:10-84 defaults
