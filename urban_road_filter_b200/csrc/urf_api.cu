@@ -33,6 +33,7 @@ struct urf_ctx {
   cudaStream_t s_side[kGroups + 1] = {};
   cudaEvent_t ev_sfork[kGroups + 1] = {}, ev_sjoin[kGroups + 1] = {};
   int sort_ctas = 0;                   // resident CTAs of k_star_sort on the whole device (its grid: the warps walk the sectors)
+  int pts_ctas = 0;                    // resident CTAs of k_points on the whole device (its grid: the scans share them)
   // H100 (400 W), C2 x 128: 1 stream 1.628 ms (one run), 2 streams 1.630 (median of six); 3 and 4 streams slower (DESIGN.md §6).
   // The groups do not hide each other's one-CTA-per-scan stages: descending stream priorities (1.683 ms) and a start
   // staggered by one k_points (1.631) were tried and dropped
@@ -188,7 +189,10 @@ int launch_pipeline(urf_ctx* ctx, const DevBuffers& buf, int B, int S, bool want
     L++;                                                                                     \
   } while (0)
   K("k_reset", k_reset<<<dim3(8, B), 256, 0, st>>>(buf, dp));
-  K("k_points", k_points<<<gpts, 256, 0, st>>>(buf, dp, S));
+  // k_points: at most one resident wave of CTAs over the launch's scans (a second, partial wave would take as long as
+  // the first), a contiguous range of whole tiles each
+  const int gp = std::max(1, std::min(ctx->pts_ctas / B, (S + kPtsTile - 1) / kPtsTile));
+  K("k_points", k_points<<<dim3(gp, B), kPtsThreads, 0, st>>>(buf, dp, S));
   K("k_register", k_register<<<B, 256, 0, st>>>(buf, dp, S));
   K("k_assign", k_assign<<<gchunk, kWarpsPerBlock * 32, 0, st>>>(buf, dp, S, T));
   K("k_scan_offsets", k_scan_offsets<<<B, kScanOffThreads, 0, st>>>(buf, dp, S, T));   // + exact re-registration of refuted scans
@@ -425,6 +429,8 @@ int urf_create(urf_ctx** out, int device, int max_points, int max_batch) {
     CKF(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ctx->device));
     CKF(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_star_sort, kSortWarps * 32, kStarSortSmem));
     ctx->sort_ctas = std::max(1, sms * per_sm);
+    CKF(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_points, kPtsThreads, 0));
+    ctx->pts_ctas = std::max(1, sms * per_sm);
   }
   CKF(cudaFuncSetAttribute(k_star_sort_big, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kStarCtaSmem));
   CKF(cudaFuncSetAttribute(k_star_refine, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kStarCtaSmem));
@@ -958,7 +964,8 @@ int urf_test_math(int device, int which, const float* a, const float* b, float* 
 //         eight-warp sort (nbig) and to the exact fallback (nslow)  10 sectors completed by k_star_refine [i32,1]
 //         (nrefine: their edge search ran off the near-first prefix)  11 Tf, 12 Tb: the blindSpots threshold tables as
 //         k_tab2 left them [f32, kDegBins * channels], degree-major (entry (j, k) at j * channels + k; rows k >= n_rings
-//         are not written)
+//         are not written)  13 firstidx [u32, kElevBins + 1]: the smallest ROI input index per fine elevation bin as
+//         k_points left it (0xffffffff = empty bin)
 int urf_debug_fetch(urf_ctx* ctx, int b, int what, void* dst, size_t bytes) {
   if (!ctx || !dst || b < 0 || b >= ctx->last_B) return URF_ERR_INVALID;
   CK(cudaSetDevice(ctx->device));
@@ -981,6 +988,10 @@ int urf_debug_fetch(urf_ctx* ctx, int b, int what, void* dst, size_t bytes) {
       if (bytes > sizeof(float) * ch * kDegBins) bytes = sizeof(float) * ch * kDegBins;
       break;
     }
+    case 13:
+      src = ctx->buf.firstidx + (size_t)b * (kElevBins + 1);
+      if (bytes > sizeof(unsigned) * (kElevBins + 1)) bytes = sizeof(unsigned) * (kElevBins + 1);
+      break;
     default: return URF_ERR_INVALID;
   }
   CK(cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost));
