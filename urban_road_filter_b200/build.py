@@ -14,8 +14,8 @@ NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-
               "-Xcompiler", "-fPIC"]
 SOURCES = ["urf_api.cu"]
 HOST_SOURCES = ["urf_markers.cpp", "urf_queue.cpp", "urf_mq.cpp"]
-HEADERS = ["urf_kernels.cuh", "urf_logic.cuh", "urf_device.cuh", "urf_math.cuh", "urf_stdsort.cuh", "urf_lomuto.cuh", "urf_host.hpp",
-           "urf_queue_internal.hpp"]
+HEADERS = ["urf_kernels.cuh", "urf_logic.cuh", "urf_device.cuh", "urf_workspace.cuh", "urf_math.cuh", "urf_stdsort.cuh", "urf_lomuto.cuh",
+           "urf_host.hpp", "urf_queue_internal.hpp"]
 
 
 def _nvcc() -> str:
@@ -86,6 +86,11 @@ def build_kat() -> None:
     if _stale(tgt, [os.path.join(kat, "lomuto_check.cpp"), os.path.join(ROOT, "oracle", "urf_oracle.cpp")] + hdrs):
         subprocess.run(["g++", "-std=c++17", "-O2", "-ffp-contract=off", "-I/usr/local/cuda/include", "-o", tgt,
                         os.path.join(kat, "lomuto_check.cpp")], check=True)
+    # the per-scan workspace layout (urf_workspace.cuh): views inside their allocations, sub-batches and host slots apart
+    tgt = os.path.join(bdir, "workspace_check")
+    if _stale(tgt, [os.path.join(kat, "workspace_check.cpp")] + hdrs):
+        subprocess.run(["g++", "-std=c++17", "-O2", "-I/usr/local/cuda/include", "-o", tgt, os.path.join(kat, "workspace_check.cpp")],
+                       check=True)
     # ThreadSanitizer build of the streaming queue around a stand-in batch function (no CUDA involved)
     tgt = os.path.join(bdir, "queue_stress")
     qsrc = [os.path.join(kat, "queue_stress.cpp"), os.path.join(CSRC, "urf_queue.cpp"), os.path.join(CSRC, "urf_mq.cpp"),

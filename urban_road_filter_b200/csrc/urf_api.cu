@@ -5,6 +5,8 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <array>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -16,23 +18,32 @@ using namespace urf;
 
 constexpr int kMaxBatch = 65535;   // scans per context: the largest grid y dimension
 
+// Owners of CUDA resources: each handle is released by its deleter when its owner goes
+template <class T, cudaError_t (*F)(T*)> struct CudaDel { void operator()(T* p) const { F(p); } };
+template <class T> using DevMem = std::unique_ptr<T, CudaDel<void, cudaFree>>;
+template <class T> using HostMem = std::unique_ptr<T, CudaDel<void, cudaFreeHost>>;
+using Stream = std::unique_ptr<CUstream_st, CudaDel<CUstream_st, cudaStreamDestroy>>;
+using Event = std::unique_ptr<CUevent_st, CudaDel<CUevent_st, cudaEventDestroy>>;
+using GraphExec = std::unique_ptr<CUgraphExec_st, CudaDel<CUgraphExec_st, cudaGraphExecDestroy>>;
+using ArrayMem = std::array<DevMem<unsigned char>, kArrays>;   // owners of a DevBuffers' arrays, in for_each_array order
+
 struct urf_ctx {
   int device = 0;
   int max_points = 0;      // per scan, rounded up to kChunk
   int max_batch = 0;
   size_t P = 0;            // max_batch * max_points
   int Tmax = 0;
-  cudaStream_t stream = nullptr;       // compute
-  cudaStream_t s_in = nullptr, s_out = nullptr;   // H2D / D2H copy streams of the pipelined host-buffer path
-  static constexpr int kGroups = 16;               // sub-batches of a device-resident call run on separate streams: scans are
-  cudaStream_t s_grp[kGroups] = {};               // independent, so their (short, partly latency-bound) kernels overlap
-  cudaEvent_t ev_fork = nullptr, ev_join[kGroups] = {};
-  // inside one pipeline the star-shaped search (four kernels) and the ring detector (one kernel) are independent between
-  // k_scatter and k_tab1: the ring detector runs on a side stream of the pipeline's stream
-  // (H100 (400 W), C2 x 128: 1.95 / 2.06 ms per step with, 2.11 / 1.99 without (within noise))
-  cudaStream_t s_side[kGroups + 1] = {};
-  cudaEvent_t ev_sfork[kGroups + 1] = {}, ev_sjoin[kGroups + 1] = {};
-  int sort_ctas = 0;                   // resident CTAs of k_star_sort on the whole device (its grid: the warps walk the sectors)
+  Stream stream;                       // compute
+  Stream s_in, s_out;                  // H2D / D2H copy streams of the pipelined host-buffer path
+  // Sub-batches of a device-resident call run on separate lanes (scans are independent, so their short, partly
+  // latency-bound kernels overlap); lane kGroups is the context's own stream. Between k_scatter and k_tab1 the ring
+  // detector runs on the lane's side stream, next to the star-shaped search
+  // (H100 (400 W), C2 x 128: 1.95 / 2.06 ms per step with, 2.11 / 1.99 without (within noise)).
+  static constexpr int kGroups = 16;
+  struct Lane { cudaStream_t st = nullptr; Stream own, side; Event join, sfork, sjoin; };   // lane kGroups: no own, no join
+  Lane lane[kGroups + 1];
+  Event ev_fork;                       // the context stream's fork to the lanes
+  int sort_ctas = 0;                  // resident CTAs of k_star_sort on the whole device (its grid: the warps walk the sectors)
   int pts_ctas = 0;                    // resident CTAs of k_points on the whole device (its grid: the scans share them)
   // H100 (400 W), C2 x 128: 1 stream 1.628 ms (one run), 2 streams 1.630 (median of six); 3 and 4 streams slower (DESIGN.md §6).
   // The groups do not hide each other's one-CTA-per-scan stages: descending stream priorities (1.683 ms) and a start
@@ -41,33 +52,28 @@ struct urf_ctx {
   // CUDA graph of the kernel sequence for small host-buffer batches (launch latency dominates there); re-captured when
   // the shape, the parameters or an option change
   bool use_graph = true;
-  cudaGraphExec_t gexec = nullptr;
+  GraphExec gexec;
   int g_B = -1, g_S = -1, g_order = -1, g_launches = 0;
   unsigned long long g_version = 0, version = 1;
-  std::vector<cudaEvent_t> ev_in, ev_comp;        // per chunk: input landed / results ready
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;       // the device-resident pair
-  DevBuffers buf{};
+  std::vector<Event> ev_in, ev_comp;   // per chunk: input landed / results ready
+  Event ev0, ev1;                      // the device-resident pair
+  DevBuffers buf{};                    // the workspace, with slot 0's arrays
+  ArrayMem mem;                        // owners of the workspace arrays of buf (slot 0's own theirs)
   // A host-buffer batch between its enqueue and its finish (urf_enqueue_batch / urf_finish_batch; the synchronous entry
   // points are one enqueue and one finish, always in slot 0). A slot holds what the batch's copies touch while the other
   // batch's kernels run; the per-point workspace is shared, and the kernels of both batches queue on `stream`.
   // Slot 0 is the context's own set (from urf_create); slot 1 is allocated by the first asynchronous call.
   struct HostSlot {
-    float4* in = nullptr;
+    DevBuffers dev{};                  // the per-slot arrays (class kSlot); label8 (int8 labels) is allocated when a caller
+    ArrayMem mem;                      // first asks for it
     // record staging of the PointCloud2 / packed-xyz entry points: slot 0 has max_points * URF_MAX_POINT_STEP bytes from
     // urf_create, so single scans never allocate; re-allocated at P * step bytes by the first batch that needs more
-    unsigned char* rawb = nullptr;
+    DevMem<unsigned char> rawb;
     size_t rawb_bytes = 0;
-    int* n = nullptr;
-    int* label = nullptr;
-    signed char* label8 = nullptr;     // int8 labels (P bytes), allocated when a caller first asks for them
-    int* order = nullptr;
-    int* ring = nullptr;               // ring ids for the caller; slot 0 before the first asynchronous call: the sort
-                                       // scratch (buf.sortbuf), see ring_chunk
-    ScanOut* out = nullptr;
-    int* h_n = nullptr;                // pinned
-    ScanOut* h_out = nullptr;          // pinned
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;   // bracket the batch's kernels
-    cudaEvent_t ev_done = nullptr;              // after the batch's last copy to the host
+    DevMem<int> ring;                  // ring ids for the caller; none in slot 0 before the first asynchronous call: the sort
+                                       // scratch (buf.sortbuf) takes them, see ring_chunk
+    HostMem<int> h_n; HostMem<ScanOut> h_out;   // pinned copies of n and out
+    Event ev0, ev1, ev_done;           // bracket the batch's kernels; after its last copy to the host
     // the batch in flight
     int batch = 0, S = 0, launches = 0;
     urf_result* outs = nullptr;
@@ -75,30 +81,28 @@ struct urf_ctx {
   };
   HostSlot hs[2];
   int hs_head = 0, hs_count = 0;       // oldest host batch in flight, number in flight (0..2)
-  float4* pack = nullptr;              // packed output clouds (urf_process_cloud2_packed): 3 * max_points 32-byte records, allocated on first use
-  int* packcnt = nullptr;              // [3][tiles] per-tile counts / offsets
-  int* packtot = nullptr;              // [4] cloud sizes
+  DevMem<float4> pack;                 // packed output clouds (urf_process_cloud2_packed): 3 * max_points 32-byte records, allocated on first use
+  DevMem<int> packcnt, packtot;        // [3][tiles] per-tile counts / offsets, [4] cloud sizes
+  HostMem<int> h_packtot;              // pinned copy
   int tie_order = URF_TIES_INPUT_ORDER;   // urf_set_tie_order; the reference order's buffers (buf.epos, buf.lomuto) are
                                           // allocated by the first switch to it
-  int* h_packtot = nullptr;            // pinned copy
   urf_params params{};
   DevParams dp{};
   // asynchronous enqueues stage their point counts in a ring of pinned rows, each guarded by the event of its H2D copy,
   // so back-to-back enqueues with different counts never overwrite a row whose copy has not run yet
   static constexpr int kNRing = 8;
-  int* h_nring = nullptr;      // pinned, [kNRing][max_batch]
-  cudaEvent_t ev_nring[kNRing] = {};
+  HostMem<int> h_nring;                // [kNRing][max_batch]
+  Event ev_nring[kNRing];
   int nring_pos = 0;
   int last_B = 0, last_S = 0;
   int launches = 0;
   float last_ms = 0.f;                 // device ms of the last finished host batch (timing_host)
   bool timing_valid = false, timing_host = false;
   std::string err;
-  std::vector<void*> allocs;
   // optional per-kernel CUDA-event timing (urf_set_option(ctx, 1, 1)); events live on the ctx stream
   bool profile = false;
   int kslots = 1, kslot = 0;           // event slots: consecutive calls cycle through them so K steps can be timed without syncing
-  std::vector<cudaEvent_t> kev;        // [kslots][kMaxKernels + 1]; the last event of a slot closes the pipeline
+  std::vector<Event> kev;              // [kslots][kMaxKernels + 1]; the last event of a slot closes the pipeline
   std::vector<const char*> knames;
   std::vector<int> kcounts;            // kernels recorded per slot
   int kcount = 0;
@@ -119,59 +123,62 @@ int cuda_rc(urf_ctx* ctx, cudaError_t e, const char* call) {
     if (rc_ != URF_OK) return rc_;                                                                 \
   } while (0)
 
-template <class T> int dalloc(urf_ctx* ctx, T** p, size_t count) {
+template <class T> int dalloc(urf_ctx* ctx, DevMem<T>& owner, size_t count) {
   void* q = nullptr;
   CK(cudaMalloc(&q, count * sizeof(T) + 256));
-  ctx->allocs.push_back(q);
-  // zero once: a few kernels issue loads ahead of the bound they are checked against (the values are dropped), and slots of
-  // a buffer that a call does not fill must read as something defined
-  // (on the context's own stream and waited for: the legacy default stream is not ordered against the non-blocking streams
-  // that use the buffer next)
-  CK(cudaMemsetAsync(q, 0, count * sizeof(T) + 256, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  *p = static_cast<T*>(q);
+  owner.reset(static_cast<T*>(q));
+  // zero once: some kernels load ahead of the bound they check, and slots a call does not fill must read as defined (on the
+  // context's stream, waited for: the legacy default stream is not ordered against the non-blocking streams used next)
+  CK(cudaMemsetAsync(q, 0, count * sizeof(T) + 256, ctx->stream.get()));
+  CK(cudaStreamSynchronize(ctx->stream.get()));
   return URF_OK;
+}
+
+// Hands the arrays allocated in `from`, and their owners, over to `to`
+void adopt(DevBuffers& to, ArrayMem& to_mem, const DevBuffers& from, ArrayMem& from_mem) {
+  for_each_array([&](int i, auto m, Kind, unsigned) { if (from.*m) { to.*m = from.*m; to_mem[i] = std::move(from_mem[i]); } });
+}
+
+// The arrays of `d` that `pick` selects, for max_batch scans at capacity, each owned by its entry of `mem`
+template <class Pick> int alloc_owned(urf_ctx* ctx, DevBuffers& d, ArrayMem& mem, Pick pick) {
+  return alloc_arrays(d, capacity_extent(ctx->max_points), ctx->max_batch, pick, [&](int i, auto& p, size_t count) {
+    const int rc = dalloc(ctx, mem[i], count * sizeof(*p));
+    if (rc == URF_OK) p = reinterpret_cast<std::remove_reference_t<decltype(p)>>(mem[i].get());
+    return rc;
+  });
+}
+
+// a new handle, held by `owner` (empty when the call fails)
+cudaError_t new_stream(Stream& owner) { cudaStream_t h = nullptr; const cudaError_t e = cudaStreamCreateWithFlags(&h, cudaStreamNonBlocking); owner.reset(h); return e; }
+cudaError_t new_event(Event& owner, unsigned flags = cudaEventDisableTiming) { cudaEvent_t h = nullptr; const cudaError_t e = cudaEventCreateWithFlags(&h, flags); owner.reset(h); return e; }
+template <class T> cudaError_t new_pinned(HostMem<T>& owner, size_t count) { void* p = nullptr; const cudaError_t e = cudaMallocHost(&p, sizeof(T) * count); owner.reset(static_cast<T*>(p)); return e; }
+// the pinned result rows and the events of a host slot
+cudaError_t init_slot(urf_ctx* ctx, urf_ctx::HostSlot& h) {
+  cudaError_t e = new_pinned(h.h_n, ctx->max_batch);
+  if (e == cudaSuccess) e = new_pinned(h.h_out, ctx->max_batch);
+  if (e == cudaSuccess) e = new_event(h.ev0, cudaEventDefault);
+  if (e == cudaSuccess) e = new_event(h.ev1, cudaEventDefault);
+  return e == cudaSuccess ? new_event(h.ev_done) : e;
 }
 
 __global__ void k_ring32(DevBuffers buf, int* dst, int S) {
   const int b = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < buf.n[b]) dst[(size_t)b * S + i] = max((int)buf.ringid[(size_t)b * S + i], -1);
-}
-
-// View of `buf` for the sub-batch that starts at scan b0: every per-scan array is advanced by b0 scans (S points of
-// stride, T histogram rows of `channels` counters per scan), so each scan keeps its own slice of the input, the outputs
-// and the workspace.
-DevBuffers offset_view(const DevBuffers& a, int b0, int S, int T, int channels) {
-  DevBuffers v = a;
-  const size_t o = (size_t)b0 * S;
-  v.in += o; v.label += o; v.order += o; v.n += b0; v.out += b0;
-  if (v.epos) { v.epos += o; v.lomuto += (size_t)b0 * (kRingKeys + 1); }
-  if (v.label8) v.label8 += o;
-  v.alpha_v += o; v.mark += o; v.ringid += o; v.sect += o; v.bpt += o;
-  v.sr += o; v.sz += o; v.sidx += o; v.ssrz += o; v.ssl += o;
-  v.az += o; v.d2 += o; v.baz += o; v.roadlist += o; v.roadcnt += (size_t)b0 * ((S + 31) >> 5); v.sortbuf += 2 * o;
-  v.Tf += (size_t)b0 * channels * kTStride; v.Tb += (size_t)b0 * channels * kTStride;
-  v.lut += (size_t)b0 * (kElevBins + 1); v.firstidx += (size_t)b0 * (kElevBins + 1);
-  v.hist += (size_t)b0 * T * channels;
-  v.cmin += (size_t)b0 * channels * kDegBins; v.cmax += (size_t)b0 * channels * kDegBins;
-  v.ne += (size_t)b0 * channels * (kDegBins + 1);
-  v.tab += b0;
-  return v;
+  if (i < buf.n[b]) dst[(size_t)b * point_slice(S) + i] = max((int)buf.ringid[(size_t)b * point_slice(S) + i], -1);
 }
 
 constexpr int kMaxKernels = 32;
 constexpr int kMarkSingleMax = 300000;   // scans above this many points take the multi-CTA marker search
 thread_local std::string g_create_err;
 
-// Enqueues the kernel sequence for B scans of stride S from `buf` on the stream of `group` (0 .. kGroups-1: a group
-// stream, kGroups: the context's own stream) and stores the number of kernels launched in *launched.
-int launch_pipeline(urf_ctx* ctx, const DevBuffers& buf, int B, int S, bool want_order, int group, int* launched) {
+// Enqueues the kernel sequence for B scans of stride S from `buf` on `lane` and stores the number of kernels launched in
+// *launched.
+int launch_pipeline(urf_ctx* ctx, const DevBuffers& buf, int B, int S, bool want_order, const urf_ctx::Lane& lane, int* launched) {
   DevParams dp = ctx->dp;
   // reference tie order: the emission order decides the marker search's scan order, so the ring sort always runs, in
   // front of k_label (into the context's own order buffer when the caller asked for none)
   const bool ref = ctx->tie_order == URF_TIES_REFERENCE;
   dp.want_order = want_order || ref ? 1 : 0;
-  cudaStream_t st = group < urf_ctx::kGroups ? ctx->s_grp[group] : ctx->stream;
+  cudaStream_t st = lane.st;
   const int T = (S + kChunk - 1) / kChunk;
   if (T > ctx->Tmax) return URF_ERR_CAPACITY;
   int L = 0;
@@ -182,7 +189,7 @@ int launch_pipeline(urf_ctx* ctx, const DevBuffers& buf, int B, int S, bool want
   do {                                                                                       \
     if (ctx->profile && ctx->kcount < kMaxKernels) {                                         \
       ctx->knames[ctx->kcount] = name;                                                       \
-      CK(cudaEventRecord(ctx->kev[(size_t)ctx->kslot * (kMaxKernels + 1) + ctx->kcount], st)); \
+      CK(cudaEventRecord(ctx->kev[(size_t)ctx->kslot * (kMaxKernels + 1) + ctx->kcount].get(), st)); \
       ctx->kcount++;                                                                         \
     }                                                                                        \
     __VA_ARGS__;                                                                             \
@@ -201,16 +208,16 @@ int launch_pipeline(urf_ctx* ctx, const DevBuffers& buf, int B, int S, bool want
   // marks, atomic min / max aggregates); k_tab1 is the first reader of the aggregates. Per-kernel timing keeps every
   // kernel on `st`, where K records its events, and without the star-shaped search there is nothing to overlap.
   const bool fork = dp.star && !ctx->profile;
-  cudaStream_t st_ring = fork ? ctx->s_side[group] : st;
+  cudaStream_t st_ring = fork ? lane.side.get() : st;
   if (fork) {
-    CK(cudaEventRecord(ctx->ev_sfork[group], st));
-    CK(cudaStreamWaitEvent(st_ring, ctx->ev_sfork[group], 0));
+    CK(cudaEventRecord(lane.sfork.get(), st));
+    CK(cudaStreamWaitEvent(st_ring, lane.sfork.get(), 0));
   }
   // k_ring_detect never sees curb_points = 5, so it runs the detectors' runtime (<0>) instantiations only
   if (dp.curbPoints == 5)              // four positions per thread (default curb_points only)
     K("k_ring_detect4", k_ring_detect4<<<dim3((S + kTile4 - 1) / kTile4, B), 256, 0, st_ring>>>(buf, dp, S));
   else K("k_ring_detect", k_ring_detect<<<gpts, 256, 0, st_ring>>>(buf, dp, S));
-  if (fork) CK(cudaEventRecord(ctx->ev_sjoin[group], st_ring));
+  if (fork) CK(cudaEventRecord(lane.sjoin.get(), st_ring));
   if (dp.star) {
     const int gbig = std::max(4, std::min(kSectKeys, 2048 / B));
     const dim3 gscan((kSectKeys + kScanWarps * 32 - 1) / (kScanWarps * 32), B);
@@ -225,7 +232,7 @@ int launch_pipeline(urf_ctx* ctx, const DevBuffers& buf, int B, int S, bool want
     if (dp.star_prefix)            // sectors whose edge search ran off the near-first prefix: full sort, search resumed
       K("k_star_refine", k_star_refine<<<dim3(std::max(8, std::min(kSectKeys / 8, 8192 / B)), B), 256, kStarCtaSmem, st>>>(buf, dp, S));
   }
-  if (fork) CK(cudaStreamWaitEvent(st, ctx->ev_sjoin[group], 0));
+  if (fork) CK(cudaStreamWaitEvent(st, lane.sjoin.get(), 0));
   K("k_tab1", k_tab1<<<dim3((dp.channels + 7) / 8, B), 256, 0, st>>>(buf, dp));
   K("k_reach", k_reach<<<dim3((2 * kDegBins + 7) / 8, B), 256, 0, st>>>(buf, dp));
   K("k_tab2", k_tab2<<<dim3((dp.channels + kTab2Rings - 1) / kTab2Rings, B), kTab2Rings * 64, 0, st>>>(buf, dp));
@@ -246,7 +253,7 @@ int launch_pipeline(urf_ctx* ctx, const DevBuffers& buf, int B, int S, bool want
   if (want_order && !ref) K("k_sort_rings", k_sort_rings<false><<<gsort, kSortThreads, kRingSmemKeys * sizeof(unsigned long long), st>>>(buf, S));
 #undef K
   if (ctx->profile) {
-    CK(cudaEventRecord(ctx->kev[(size_t)ctx->kslot * (kMaxKernels + 1) + kMaxKernels], st));
+    CK(cudaEventRecord(ctx->kev[(size_t)ctx->kslot * (kMaxKernels + 1) + kMaxKernels].get(), st));
     ctx->kcounts[ctx->kslot] = ctx->kcount;
     ctx->kslot = (ctx->kslot + 1) % ctx->kslots;
   }
@@ -260,16 +267,17 @@ int launch_pipeline(urf_ctx* ctx, const DevBuffers& buf, int B, int S, bool want
 // the shape, the parameters or an option change.
 int update_graph(urf_ctx* ctx, int B, int S, bool want_order) {
   if (ctx->gexec && ctx->g_B == B && ctx->g_S == S && ctx->g_order == (int)want_order && ctx->g_version == ctx->version) return URF_OK;
-  if (ctx->gexec) { cudaGraphExecDestroy(ctx->gexec); ctx->gexec = nullptr; }
+  ctx->gexec.reset();
   cudaGraph_t graph = nullptr;
-  CK(cudaStreamBeginCapture(ctx->stream, cudaStreamCaptureModeThreadLocal));
+  CK(cudaStreamBeginCapture(ctx->stream.get(), cudaStreamCaptureModeThreadLocal));
   int L = 0;
-  const int rc = launch_pipeline(ctx, ctx->buf, B, S, want_order, urf_ctx::kGroups, &L);
-  const cudaError_t e = cudaStreamEndCapture(ctx->stream, &graph);
+  const int rc = launch_pipeline(ctx, ctx->buf, B, S, want_order, ctx->lane[urf_ctx::kGroups], &L);
+  const cudaError_t e = cudaStreamEndCapture(ctx->stream.get(), &graph);
   if (rc != URF_OK || e != cudaSuccess || !graph) { if (graph) cudaGraphDestroy(graph); ctx->err = "graph capture failed"; return rc != URF_OK ? rc : URF_ERR_CUDA; }
-  const cudaError_t ei = cudaGraphInstantiate(&ctx->gexec, graph, 0);
-  cudaGraphDestroy(graph);
-  if (ei != cudaSuccess) { ctx->gexec = nullptr; ctx->err = cudaGetErrorString(ei); return URF_ERR_CUDA; }
+  cudaGraphExec_t exec = nullptr;
+  const cudaError_t ei = cudaGraphInstantiate(&exec, graph, 0);
+  cudaGraphDestroy(graph); ctx->gexec.reset(exec);
+  if (ei != cudaSuccess) { ctx->err = cudaGetErrorString(ei); return URF_ERR_CUDA; }
   ctx->g_B = B; ctx->g_S = S; ctx->g_order = (int)want_order; ctx->g_version = ctx->version; ctx->g_launches = L;
   return URF_OK;
 }
@@ -349,68 +357,24 @@ int urf_create(urf_ctx** out, int device, int max_points, int max_batch) {
   int rc;
 #define TRY(x) do { rc = (x); if (rc != URF_OK) return fail(rc); } while (0)
 #define CKF(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { ctx->err = cudaGetErrorString(e_); return fail(URF_ERR_CUDA); } } while (0)
-  CKF(cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking));
-  CKF(cudaStreamCreateWithFlags(&ctx->s_in, cudaStreamNonBlocking));
-  CKF(cudaStreamCreateWithFlags(&ctx->s_out, cudaStreamNonBlocking));
-  for (int g = 0; g < urf_ctx::kGroups; g++) {
-    CKF(cudaStreamCreateWithFlags(&ctx->s_grp[g], cudaStreamNonBlocking));
-    CKF(cudaEventCreateWithFlags(&ctx->ev_join[g], cudaEventDisableTiming));
-  }
-  CKF(cudaEventCreateWithFlags(&ctx->ev_fork, cudaEventDisableTiming));
+  for (Stream* s : {&ctx->stream, &ctx->s_in, &ctx->s_out}) CKF(new_stream(*s));
   for (int g = 0; g <= urf_ctx::kGroups; g++) {
-    CKF(cudaStreamCreateWithFlags(&ctx->s_side[g], cudaStreamNonBlocking));
-    CKF(cudaEventCreateWithFlags(&ctx->ev_sfork[g], cudaEventDisableTiming));
-    CKF(cudaEventCreateWithFlags(&ctx->ev_sjoin[g], cudaEventDisableTiming));
+    urf_ctx::Lane& l = ctx->lane[g];
+    if (g < urf_ctx::kGroups) { CKF(new_stream(l.own)); CKF(new_event(l.join)); }
+    l.st = g < urf_ctx::kGroups ? l.own.get() : ctx->stream.get();
+    CKF(new_stream(l.side)); CKF(new_event(l.sfork)); CKF(new_event(l.sjoin));
   }
-  CKF(cudaEventCreate(&ctx->ev0));
-  CKF(cudaEventCreate(&ctx->ev1));
-  const size_t P = ctx->P;
+  CKF(new_event(ctx->ev_fork)); CKF(new_event(ctx->ev0, cudaEventDefault)); CKF(new_event(ctx->ev1, cudaEventDefault));
   DevBuffers& b = ctx->buf;
   urf_ctx::HostSlot& h0 = ctx->hs[0];
-  TRY(dalloc(ctx, &h0.in, P));
-  h0.rawb_bytes = (size_t)ctx->max_points * URF_MAX_POINT_STEP;
-  TRY(dalloc(ctx, &h0.rawb, h0.rawb_bytes));
-  TRY(dalloc(ctx, &b.alpha_v, P));
-  TRY(dalloc(ctx, &b.mark, P));
-  TRY(dalloc(ctx, &b.ringid, P));
-  TRY(dalloc(ctx, &b.sect, P));
-  TRY(dalloc(ctx, &h0.label, P));
-  TRY(dalloc(ctx, &b.bpt, P));
-  TRY(dalloc(ctx, &b.sr, P));
-  TRY(dalloc(ctx, &b.sz, P));
-  TRY(dalloc(ctx, &b.sidx, P));
-  TRY(dalloc(ctx, &b.ssrz, P));
-  TRY(dalloc(ctx, &b.ssl, P));
-  TRY(dalloc(ctx, &b.az, P));
-  TRY(dalloc(ctx, &b.d2, P));
-  TRY(dalloc(ctx, &b.baz, P));
-  TRY(dalloc(ctx, &b.roadlist, P));
-  TRY(dalloc(ctx, &b.roadcnt, P / 32 + (size_t)max_batch + 1));
-  TRY(dalloc(ctx, &b.Tf, (size_t)max_batch * kTStride * URF_MAX_CHANNELS));
-  TRY(dalloc(ctx, &b.Tb, (size_t)max_batch * kTStride * URF_MAX_CHANNELS));
-  TRY(dalloc(ctx, &b.lut, (size_t)max_batch * (kElevBins + 1)));
-  TRY(dalloc(ctx, &b.order, P));
-  TRY(dalloc(ctx, &b.sortbuf, 2 * P));
-  TRY(dalloc(ctx, &b.hist, (size_t)max_batch * ctx->Tmax * kRingKeys));
-  TRY(dalloc(ctx, &b.firstidx, (size_t)max_batch * (kElevBins + 1)));
-  TRY(dalloc(ctx, &b.cmin, (size_t)max_batch * URF_MAX_CHANNELS * kDegBins));
-  TRY(dalloc(ctx, &b.cmax, (size_t)max_batch * URF_MAX_CHANNELS * kDegBins));
-  TRY(dalloc(ctx, &b.ne, (size_t)max_batch * URF_MAX_CHANNELS * (kDegBins + 1)));
-  TRY(dalloc(ctx, &b.newY, (size_t)ctx->max_points));
-  TRY(dalloc(ctx, &b.n, (size_t)max_batch));
-  TRY(dalloc(ctx, &b.out, (size_t)max_batch));
-  TRY(dalloc(ctx, &b.tab, (size_t)max_batch));
-  b.in = h0.in;
-  b.label = h0.label;
-  h0.n = b.n; h0.order = b.order; h0.out = b.out;
-  h0.ring = reinterpret_cast<int*>(b.sortbuf);
-  CKF(cudaMallocHost((void**)&h0.h_n, sizeof(int) * max_batch));
-  CKF(cudaMallocHost((void**)&ctx->h_nring, sizeof(int) * max_batch * urf_ctx::kNRing));
-  for (int r = 0; r < urf_ctx::kNRing; r++) CKF(cudaEventCreateWithFlags(&ctx->ev_nring[r], cudaEventDisableTiming));
-  CKF(cudaMallocHost((void**)&h0.h_out, sizeof(ScanOut) * max_batch));
-  CKF(cudaEventCreate(&h0.ev0));
-  CKF(cudaEventCreate(&h0.ev1));
-  CKF(cudaEventCreateWithFlags(&h0.ev_done, cudaEventDisableTiming));
+  TRY(alloc_owned(ctx, b, ctx->mem, created_with_context));
+  TRY(alloc_owned(ctx, h0.dev, h0.mem, slot_array));
+  b = slot_view(b, h0.dev);
+  h0.rawb_bytes = capacity_elems(Kind::Point, capacity_extent(ctx->max_points), 1) * URF_MAX_POINT_STEP;
+  TRY(dalloc(ctx, h0.rawb, h0.rawb_bytes));
+  CKF(init_slot(ctx, h0));
+  CKF(new_pinned(ctx->h_nring, (size_t)max_batch * urf_ctx::kNRing));
+  for (Event& e : ctx->ev_nring) CKF(new_event(e));
   {
     std::vector<float> ny;
     host_newY(ny, ctx->max_points);
@@ -454,32 +418,7 @@ void urf_destroy(urf_ctx* ctx) {
   if (!ctx) return;
   cudaSetDevice(ctx->device);
   // host batches still in flight copy into the caller's buffers on s_in / s_out: wait for them too
-  for (cudaStream_t s : {ctx->s_in, ctx->stream, ctx->s_out}) if (s) cudaStreamSynchronize(s);
-  for (void* p : ctx->allocs) cudaFree(p);
-  if (ctx->h_nring) cudaFreeHost(ctx->h_nring);
-  for (cudaEvent_t e : ctx->ev_nring) if (e) cudaEventDestroy(e);
-  for (urf_ctx::HostSlot& h : ctx->hs) {
-    if (h.h_n) cudaFreeHost(h.h_n);
-    if (h.h_out) cudaFreeHost(h.h_out);
-    for (cudaEvent_t e : {h.ev0, h.ev1, h.ev_done}) if (e) cudaEventDestroy(e);
-  }
-  if (ctx->h_packtot) cudaFreeHost(ctx->h_packtot);
-  if (ctx->gexec) cudaGraphExecDestroy(ctx->gexec);
-  for (cudaEvent_t e : ctx->kev) cudaEventDestroy(e);
-  for (cudaEvent_t e : ctx->ev_in) cudaEventDestroy(e);
-  for (cudaEvent_t e : ctx->ev_comp) cudaEventDestroy(e);
-  for (int g = 0; g < urf_ctx::kGroups; g++) { if (ctx->s_grp[g]) cudaStreamDestroy(ctx->s_grp[g]); if (ctx->ev_join[g]) cudaEventDestroy(ctx->ev_join[g]); }
-  if (ctx->ev_fork) cudaEventDestroy(ctx->ev_fork);
-  for (int g = 0; g <= urf_ctx::kGroups; g++) {
-    if (ctx->s_side[g]) cudaStreamDestroy(ctx->s_side[g]);
-    if (ctx->ev_sfork[g]) cudaEventDestroy(ctx->ev_sfork[g]);
-    if (ctx->ev_sjoin[g]) cudaEventDestroy(ctx->ev_sjoin[g]);
-  }
-  if (ctx->s_in) cudaStreamDestroy(ctx->s_in);
-  if (ctx->s_out) cudaStreamDestroy(ctx->s_out);
-  if (ctx->ev0) cudaEventDestroy(ctx->ev0);
-  if (ctx->ev1) cudaEventDestroy(ctx->ev1);
-  if (ctx->stream) cudaStreamDestroy(ctx->stream);
+  for (const Stream* s : {&ctx->s_in, &ctx->stream, &ctx->s_out}) if (*s) cudaStreamSynchronize(s->get());
   delete ctx;
 }
 
@@ -523,19 +462,17 @@ int urf_set_option(urf_ctx* ctx, int option, int value) {
   if ((option >= 5 && option <= 9) || option == 11 || option == 12) return URF_OK;
   if (option == 10) { ctx->dp.star_pivot = value < 3 ? 3 : (value > 28 ? 28 : value); return URF_OK; }
   if (option == 1) {                   // value = number of event slots (0 = off)
-    CK(cudaStreamSynchronize(ctx->stream));               // events of the previous setting may still be pending
-    if (ctx->gexec) { cudaGraphExecDestroy(ctx->gexec); ctx->gexec = nullptr; ctx->g_B = -1; }
-    for (cudaEvent_t e : ctx->kev) cudaEventDestroy(e);
+    CK(cudaStreamSynchronize(ctx->stream.get()));         // events of the previous setting may still be pending
+    if (ctx->gexec) { ctx->gexec.reset(); ctx->g_B = -1; }
     ctx->kev.clear();
     ctx->profile = value > 0;
     ctx->kslots = value > 0 ? value : 1;
     ctx->kslot = 0;
     if (ctx->profile) {
-      ctx->kev.assign((size_t)ctx->kslots * (kMaxKernels + 1), nullptr);
-      for (cudaEvent_t& e : ctx->kev) {
-        const cudaError_t ce = cudaEventCreate(&e);
-        if (ce != cudaSuccess) {                           // leave the option off and leak nothing
-          for (cudaEvent_t f : ctx->kev) if (f) cudaEventDestroy(f);
+      ctx->kev.resize((size_t)ctx->kslots * (kMaxKernels + 1));
+      for (Event& e : ctx->kev) {
+        const cudaError_t ce = new_event(e, cudaEventDefault);
+        if (ce != cudaSuccess) {                           // leave the option off
           ctx->kev.clear(); ctx->profile = false; ctx->kslots = 1;
           ctx->err = std::string("cudaEventCreate: ") + cudaGetErrorString(ce);
           return URF_ERR_CUDA;
@@ -553,13 +490,10 @@ int urf_set_tie_order(urf_ctx* ctx, int mode) {
   if (!ctx || ctx->hs_count || (mode != URF_TIES_INPUT_ORDER && mode != URF_TIES_REFERENCE)) return URF_ERR_INVALID;
   CK(cudaSetDevice(ctx->device));
   if (mode == URF_TIES_REFERENCE && !ctx->buf.lomuto) {   // 4 bytes per point of capacity plus one ring list per scan
-    int* epos = nullptr;
-    int* lomuto = nullptr;
-    int rc = dalloc(ctx, &epos, ctx->P);
-    if (rc == URF_OK) rc = dalloc(ctx, &lomuto, (size_t)ctx->max_batch * (kRingKeys + 1));
-    if (rc != URF_OK) return rc;
-    ctx->buf.epos = epos;
-    ctx->buf.lomuto = lomuto;
+    DevBuffers d{};
+    ArrayMem mem;                                          // freed on a failure
+    if (const int rc = alloc_owned(ctx, d, mem, tie_order_array); rc != URF_OK) return rc;
+    adopt(ctx->buf, ctx->mem, d, mem);
   }
   ctx->tie_order = mode;
   ctx->version++;                                          // the captured graph holds the other launch sequence
@@ -577,15 +511,15 @@ int urf_mq_set_tie_order(urf_mq* mq, int mode) {
   return urf_internal::mq_apply_idle(mq, [](urf_ctx* c, const void* m) { return urf_set_tie_order(c, *static_cast<const int*>(m)); }, &mode);
 }
 
-void* urf_stream(urf_ctx* ctx) { return ctx ? (void*)ctx->stream : nullptr; }
+void* urf_stream(urf_ctx* ctx) { return ctx ? (void*)ctx->stream.get() : nullptr; }
 
 float urf_last_device_ms(const urf_ctx* c) {
   urf_ctx* ctx = const_cast<urf_ctx*>(c);
   if (!ctx || !ctx->timing_valid) return -1.f;
   if (ctx->timing_host) return ctx->last_ms;
   float ms = -1.f;
-  if (cudaEventSynchronize(ctx->ev1) != cudaSuccess) return -1.f;
-  if (cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1) != cudaSuccess) return -1.f;
+  if (cudaEventSynchronize(ctx->ev1.get()) != cudaSuccess) return -1.f;
+  if (cudaEventElapsedTime(&ms, ctx->ev0.get(), ctx->ev1.get()) != cudaSuccess) return -1.f;
   return ms;
 }
 
@@ -599,9 +533,9 @@ int urf_profile_slots(const urf_ctx* ctx) { return ctx && ctx->profile ? ctx->ks
 int urf_profile_get(urf_ctx* ctx, int slot, int idx, const char** name, float* ms) {
   if (!ctx || !ctx->profile || slot < 0 || slot >= ctx->kslots || idx < 0 || idx >= ctx->kcounts[slot]) return URF_ERR_INVALID;
   const size_t o = (size_t)slot * (kMaxKernels + 1);
-  cudaEvent_t next = idx + 1 < ctx->kcounts[slot] ? ctx->kev[o + idx + 1] : ctx->kev[o + kMaxKernels];
+  cudaEvent_t next = (idx + 1 < ctx->kcounts[slot] ? ctx->kev[o + idx + 1] : ctx->kev[o + kMaxKernels]).get();
   CK(cudaEventSynchronize(next));
-  CK(cudaEventElapsedTime(ms, ctx->kev[o + idx], next));
+  CK(cudaEventElapsedTime(ms, ctx->kev[o + idx].get(), next));
   if (name) *name = ctx->knames[idx];
   return URF_OK;
 }
@@ -612,42 +546,42 @@ int urf_enqueue_batch_device_ex(urf_ctx* ctx, const float* d_xyzi, int stride_po
   if (batch > ctx->max_batch || (size_t)stride_points * batch > ctx->P || stride_points > ctx->max_points) return URF_ERR_CAPACITY;
   CK(cudaSetDevice(ctx->device));
   for (int b = 0; b < batch; b++) if (n[b] < 0 || n[b] > stride_points) return URF_ERR_INVALID;
-  int* row = ctx->h_nring + (size_t)ctx->nring_pos * ctx->max_batch;
-  CK(cudaEventSynchronize(ctx->ev_nring[ctx->nring_pos]));    // the copy that last used this row (kNRing enqueues ago) is done
+  int* row = ctx->h_nring.get() + (size_t)ctx->nring_pos * ctx->max_batch;
+  CK(cudaEventSynchronize(ctx->ev_nring[ctx->nring_pos].get()));   // the copy that last used this row (kNRing enqueues ago) is done
   std::memcpy(row, n, sizeof(int) * batch);
-  CK(cudaMemcpyAsync(ctx->buf.n, row, sizeof(int) * batch, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaEventRecord(ctx->ev_nring[ctx->nring_pos], ctx->stream));
+  CK(cudaMemcpyAsync(ctx->buf.n, row, sizeof(int) * batch, cudaMemcpyHostToDevice, ctx->stream.get()));
+  CK(cudaEventRecord(ctx->ev_nring[ctx->nring_pos].get(), ctx->stream.get()));
   ctx->nring_pos = (ctx->nring_pos + 1) % urf_ctx::kNRing;
   const bool want_order = d_order != nullptr;
   DevBuffers bufv = ctx->buf;                                 // the caller's buffers instead of the context's own
   bufv.in = reinterpret_cast<float4*>(const_cast<float*>(d_xyzi));
   bufv.label = d_label;
   if (want_order) bufv.order = d_order;
-  const int T = (stride_points + kChunk - 1) / kChunk;
   const int G = (ctx->profile || batch < 2 * ctx->groups) ? 1 : ctx->groups;   // per-kernel event timing needs one stream
   int launches = 0;
-  CK(cudaEventRecord(ctx->ev0, ctx->stream));
+  CK(cudaEventRecord(ctx->ev0.get(), ctx->stream.get()));
   if (G == 1) {
-    const int rc = launch_pipeline(ctx, bufv, batch, stride_points, want_order, urf_ctx::kGroups, &launches);
+    const int rc = launch_pipeline(ctx, bufv, batch, stride_points, want_order, ctx->lane[urf_ctx::kGroups], &launches);
     if (rc != URF_OK) return rc;
   } else {
-    // fork: the ctx stream hands one of G near-equal sub-batches (scans [ceil(g * batch / G), ceil((g + 1) * batch / G)))
-    // to each group stream and joins them again, so callers still see ONE stream. Scans are independent.
-    CK(cudaEventRecord(ctx->ev_fork, ctx->stream));
-    for (int g = 0; g < G; g++) CK(cudaStreamWaitEvent(ctx->s_grp[g], ctx->ev_fork, 0));
+    // fork: the ctx stream hands one of G near-equal sub-batches (group_bounds) to each lane and joins them again, so
+    // callers still see ONE stream. Scans are independent.
+    CK(cudaEventRecord(ctx->ev_fork.get(), ctx->stream.get()));
+    for (int g = 0; g < G; g++) CK(cudaStreamWaitEvent(ctx->lane[g].st, ctx->ev_fork.get(), 0));
+    const Extent e = launch_extent(stride_points, ctx->dp.channels);
     for (int g = 0; g < G; g++) {
-      const int b0 = (g * batch + G - 1) / G, b1 = ((g + 1) * batch + G - 1) / G;
-      int L = 0;
-      const int rc = launch_pipeline(ctx, offset_view(bufv, b0, stride_points, T, ctx->dp.channels), b1 - b0, stride_points, want_order, g, &L);
+      int b0, b1, L = 0;
+      group_bounds(g, G, batch, &b0, &b1);
+      const int rc = launch_pipeline(ctx, scan_view(bufv, b0, e), b1 - b0, stride_points, want_order, ctx->lane[g], &L);
       if (rc != URF_OK) return rc;
       launches += L;
     }
     for (int g = 0; g < G; g++) {
-      CK(cudaEventRecord(ctx->ev_join[g], ctx->s_grp[g]));
-      CK(cudaStreamWaitEvent(ctx->stream, ctx->ev_join[g], 0));
+      CK(cudaEventRecord(ctx->lane[g].join.get(), ctx->lane[g].st));
+      CK(cudaStreamWaitEvent(ctx->stream.get(), ctx->lane[g].join.get(), 0));
     }
   }
-  CK(cudaEventRecord(ctx->ev1, ctx->stream));
+  CK(cudaEventRecord(ctx->ev1.get(), ctx->stream.get()));
   ctx->launches = launches;
   ctx->timing_valid = true;
   ctx->timing_host = false;
@@ -663,9 +597,9 @@ int urf_finish_batch_device(urf_ctx* ctx, urf_result* outs) {
   if (!ctx || ctx->hs_count) return URF_ERR_INVALID;
   CK(cudaSetDevice(ctx->device));
   const int B = ctx->last_B;
-  ScanOut* h_out = ctx->hs[0].h_out;
-  if (outs) CK(cudaMemcpyAsync(h_out, ctx->buf.out, sizeof(ScanOut) * B, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
+  ScanOut* h_out = ctx->hs[0].h_out.get();
+  if (outs) CK(cudaMemcpyAsync(h_out, ctx->buf.out, sizeof(ScanOut) * B, cudaMemcpyDeviceToHost, ctx->stream.get()));
+  CK(cudaStreamSynchronize(ctx->stream.get()));
   if (outs) for (int b = 0; b < B; b++) fill_result(h_out[b], &outs[b], false);
   return URF_OK;
 }
@@ -705,56 +639,52 @@ int enqueue_batch(urf_ctx* ctx, const void* const* data, const int* n, int batch
     want_order |= outs[b].order != nullptr;
     want_ring |= outs[b].ring != nullptr;
     want_l8 |= label8 && label8[b];
-    h.h_n[b] = n[b];
+    h.h_n.get()[b] = n[b];
   }
   const int S = ((nmax + 255) / 256) * 256;
-  const int T = (S + kChunk - 1) / kChunk;
+  const Extent cap = capacity_extent(ctx->max_points), e = launch_extent(S, ctx->dp.channels);
+  const size_t pts = slice_elems(Kind::Point, e);             // per scan: points of the input, ring ids, record staging
   if ((size_t)batch * S * step > h.rawb_bytes) {              // records of a batch beyond the staging buffer: P * step bytes
-    CK(cudaStreamSynchronize(ctx->stream));
-    if (h.rawb) { cudaFree(h.rawb); ctx->allocs.erase(std::find(ctx->allocs.begin(), ctx->allocs.end(), (void*)h.rawb)); h.rawb = nullptr; }
-    h.rawb_bytes = 0;
-    const int rc = dalloc(ctx, &h.rawb, ctx->P * (size_t)step);
-    if (rc != URF_OK) return rc;
-    h.rawb_bytes = ctx->P * (size_t)step;
+    CK(cudaStreamSynchronize(ctx->stream.get()));
+    h.rawb.reset(); h.rawb_bytes = 0;                         // the old buffer goes first
+    const size_t bytes = capacity_elems(Kind::Point, cap, ctx->max_batch) * step;
+    if (const int rc = dalloc(ctx, h.rawb, bytes); rc != URF_OK) return rc;
+    h.rawb_bytes = bytes;
   }
-  if (want_l8 && !h.label8) {
-    const int rc = dalloc(ctx, &h.label8, ctx->P);
-    if (rc != URF_OK) return rc;
-  }
+  if (want_l8 && !h.dev.label8)
+    if (const int rc = alloc_owned(ctx, h.dev, h.mem, label8_array); rc != URF_OK) return rc;
   if (clouds && !ctx->pack) {                                  // first packed call: 96 bytes per point of capacity
     const int tiles = (std::max(ctx->max_points, 1) + kPackTile - 1) / kPackTile;
-    int rc = dalloc(ctx, &ctx->pack, (size_t)6 * ctx->max_points);
-    if (rc == URF_OK) rc = dalloc(ctx, &ctx->packcnt, (size_t)3 * tiles);
-    if (rc == URF_OK) rc = dalloc(ctx, &ctx->packtot, 4);
-    if (rc != URF_OK) { ctx->pack = nullptr; return rc; }
-    CK(cudaMallocHost((void**)&ctx->h_packtot, sizeof(int) * 4));
+    DevMem<float4> pack;                                       // all or nothing: freed on a failure
+    DevMem<int> packcnt, packtot; HostMem<int> h_packtot;
+    int rc = dalloc(ctx, pack, (size_t)6 * ctx->max_points);
+    if (rc == URF_OK) rc = dalloc(ctx, packcnt, (size_t)3 * tiles);
+    if (rc == URF_OK) rc = dalloc(ctx, packtot, 4);
+    if (rc == URF_OK) rc = cuda_rc(ctx, new_pinned(h_packtot, 4), "cudaMallocHost");
+    if (rc != URF_OK) return rc;
+    ctx->pack = std::move(pack); ctx->packcnt = std::move(packcnt); ctx->packtot = std::move(packtot); ctx->h_packtot = std::move(h_packtot);
   }
-  cudaStream_t st = ctx->stream;
-  DevBuffers bufv = ctx->buf;                                 // slot 0: the same pointers as ctx->buf
-  bufv.in = h.in; bufv.n = h.n; bufv.label = h.label; bufv.order = h.order; bufv.out = h.out;
-  bufv.label8 = want_l8 ? h.label8 : nullptr;
+  cudaStream_t st = ctx->stream.get();
+  DevBuffers bufv = slot_view(ctx->buf, h.dev);               // slot 0: the same pointers as ctx->buf
+  if (!want_l8) bufv.label8 = nullptr;
   // Software pipeline over chunks of scans: H2D of chunk c+1 (s_in), kernels of chunk c (stream) and D2H of chunk c-1
   // (s_out) overlap; scans are independent, every chunk owns its slice of every buffer.
   // Chunks of batch / 16 scans. (Tried and dropped: smaller chunks at both ends of the call — a shorter pipeline fill and
   // drain on paper, slower in practice — and copies running only three chunks ahead of the launches.)
   std::vector<int> cb;                                        // chunk c = scans [cb[c], cb[c + 1])
-  {
-    const int chunk = batch >= 16 ? std::max(4, (batch + 15) / 16) : batch;
-    for (int b0 = 0; b0 < batch; b0 += chunk) cb.push_back(b0);
-    cb.push_back(batch);
-  }
+  for (int b0 = 0, chunk = host_chunk(batch); b0 < batch; b0 += chunk) cb.push_back(b0);
+  cb.push_back(batch);
   const int nchunks = (int)cb.size() - 1;
-  while ((int)ctx->ev_in.size() < nchunks) {
-    cudaEvent_t a, c;
-    CK(cudaEventCreateWithFlags(&a, cudaEventDisableTiming));
-    CK(cudaEventCreateWithFlags(&c, cudaEventDisableTiming));
-    ctx->ev_in.push_back(a); ctx->ev_comp.push_back(c);
+  for (int c = (int)ctx->ev_in.size(); c < nchunks; c++) {
+    Event in, comp;
+    CK(new_event(in)); CK(new_event(comp));
+    ctx->ev_in.push_back(std::move(in)); ctx->ev_comp.push_back(std::move(comp));
   }
   // ring ids of chunk c: until the first asynchronous call, slot 0 writes them into the chunk's private slice of the sort
   // scratch (16 bytes per point), free once the chunk's sorts are done; from then on every slot has a buffer of its own,
   // because the next batch's sorts overwrite the scratch while this batch's ring ids are still being copied out
-  const bool ring_in_scratch = h.ring == reinterpret_cast<int*>(ctx->buf.sortbuf);
-  auto ring_chunk = [&](int b0) { return h.ring + (size_t)b0 * S * (ring_in_scratch ? 4 : 1); };
+  const bool ring_in_scratch = !h.ring;
+  auto ring_chunk = [&](const DevBuffers& v, int b0) { return ring_in_scratch ? reinterpret_cast<int*>(v.sortbuf) : h.ring.get() + b0 * pts; };
   // the graph holds ctx->buf's pointers, which are slot 0's
   const bool graphed = slot == 0 && nchunks == 1 && batch <= 8 && !want_l8 && ctx->use_graph && !ctx->profile;
   if (graphed) {
@@ -765,56 +695,59 @@ int enqueue_batch(urf_ctx* ctx, const void* const* data, const int* n, int batch
   // for this thread to get through a chunk's kernel launches and result copies
   for (int c = 0; c < nchunks; c++) {
     const int b0 = cb[c], nb = cb[c + 1] - b0;
-    CK(cudaMemcpyAsync(h.n + b0, h.h_n + b0, sizeof(int) * nb, cudaMemcpyHostToDevice, ctx->s_in));
+    CK(cudaMemcpyAsync(scan_view(bufv, b0, e).n, h.h_n.get() + b0, sizeof(int) * nb, cudaMemcpyHostToDevice, ctx->s_in.get()));
     for (int b = b0; b < b0 + nb; b++) {
       if (n[b] <= 0) continue;
-      if (step == 0) CK(cudaMemcpyAsync(h.in + (size_t)b * S, data[b], sizeof(float) * 4 * (size_t)n[b], cudaMemcpyHostToDevice, ctx->s_in));
-      else CK(cudaMemcpyAsync(h.rawb + (size_t)b * S * step, data[b], (size_t)step * (size_t)n[b], cudaMemcpyHostToDevice, ctx->s_in));
+      if (step == 0) CK(cudaMemcpyAsync(scan_view(bufv, b, e).in, data[b], sizeof(float) * 4 * (size_t)n[b], cudaMemcpyHostToDevice, ctx->s_in.get()));
+      else CK(cudaMemcpyAsync(h.rawb.get() + b * pts * step, data[b], (size_t)step * (size_t)n[b], cudaMemcpyHostToDevice, ctx->s_in.get()));
     }
-    CK(cudaEventRecord(ctx->ev_in[c], ctx->s_in));
+    CK(cudaEventRecord(ctx->ev_in[c].get(), ctx->s_in.get()));
   }
   int launches = 0;
   for (int c = 0; c < nchunks; c++) {
     const int b0 = cb[c], nb = cb[c + 1] - b0;
-    CK(cudaStreamWaitEvent(st, ctx->ev_in[c], 0));
+    CK(cudaStreamWaitEvent(st, ctx->ev_in[c].get(), 0));
+    const DevBuffers view = scan_view(bufv, b0, e);
     if (step != 0)
-      k_unpack_cloud2_batch<<<dim3((S + 255) / 256, nb), 256, 0, st>>>(h.rawb + (size_t)b0 * S * step, h.in + (size_t)b0 * S, h.n + b0, S,
-                                                                          step, ox, oy, oz, oi);
-    const DevBuffers view = offset_view(bufv, b0, S, T, ctx->dp.channels);
+      k_unpack_cloud2_batch<<<dim3((S + 255) / 256, nb), 256, 0, st>>>(h.rawb.get() + b0 * pts * step, view.in, view.n, S, step, ox, oy, oz, oi);
     // ev0 / ev1 bracket the kernels of the whole call: before the first chunk's pipeline, after the last one's
     int L = graphed ? ctx->g_launches : 0;
-    int rc = c == 0 ? cuda_rc(ctx, cudaEventRecord(h.ev0, st), "cudaEventRecord(ev0)") : URF_OK;
+    int rc = c == 0 ? cuda_rc(ctx, cudaEventRecord(h.ev0.get(), st), "cudaEventRecord(ev0)") : URF_OK;
     if (rc == URF_OK)
-      rc = graphed ? cuda_rc(ctx, cudaGraphLaunch(ctx->gexec, st), "cudaGraphLaunch") : launch_pipeline(ctx, view, nb, S, want_order, urf_ctx::kGroups, &L);
-    if (rc == URF_OK && c == nchunks - 1) rc = cuda_rc(ctx, cudaEventRecord(h.ev1, st), "cudaEventRecord(ev1)");
+      rc = graphed ? cuda_rc(ctx, cudaGraphLaunch(ctx->gexec.get(), st), "cudaGraphLaunch")
+                   : launch_pipeline(ctx, view, nb, S, want_order, ctx->lane[urf_ctx::kGroups], &L);
+    if (rc == URF_OK && c == nchunks - 1) rc = cuda_rc(ctx, cudaEventRecord(h.ev1.get(), st), "cudaEventRecord(ev1)");
     if (rc != URF_OK) {                                 // nothing of this call may still be writing into the caller's buffers
-      cudaStreamSynchronize(ctx->s_in); cudaStreamSynchronize(st); cudaStreamSynchronize(ctx->s_out);
+      cudaStreamSynchronize(ctx->s_in.get()); cudaStreamSynchronize(st); cudaStreamSynchronize(ctx->s_out.get());
       return rc;
     }
     launches += L;
-    if (want_ring) k_ring32<<<dim3((S + 255) / 256, nb), 256, 0, st>>>(view, ring_chunk(b0), S);
+    if (want_ring) k_ring32<<<dim3((S + 255) / 256, nb), 256, 0, st>>>(view, ring_chunk(view, b0), S);
     if (clouds) {                                       // batch == 1: pack scan 0, sizes to the host with the results
       const int nt = (std::max(n[0], 1) + kPackTile - 1) / kPackTile;
-      k_pack_count<<<nt, 256, 0, st>>>(ctx->buf, ctx->packcnt, nt);
-      k_pack_scan<<<1, 1024, 0, st>>>(ctx->buf, ctx->packcnt, nt, ctx->packtot);
-      k_pack_write<<<nt, 256, 0, st>>>(ctx->buf, ctx->packcnt, nt, ctx->packtot, ctx->pack, ctx->pack + 2 * (size_t)ctx->max_points,
-                                       ctx->pack + 4 * (size_t)ctx->max_points);
+      float4* pack = ctx->pack.get();
+      k_pack_count<<<nt, 256, 0, st>>>(ctx->buf, ctx->packcnt.get(), nt);
+      k_pack_scan<<<1, 1024, 0, st>>>(ctx->buf, ctx->packcnt.get(), nt, ctx->packtot.get());
+      k_pack_write<<<nt, 256, 0, st>>>(ctx->buf, ctx->packcnt.get(), nt, ctx->packtot.get(), pack, pack + 2 * (size_t)ctx->max_points,
+                                       pack + 4 * (size_t)ctx->max_points);
       launches += 3;
-      CK(cudaMemcpyAsync(ctx->h_packtot, ctx->packtot, sizeof(int) * 4, cudaMemcpyDeviceToHost, st));
+      CK(cudaMemcpyAsync(ctx->h_packtot.get(), ctx->packtot.get(), sizeof(int) * 4, cudaMemcpyDeviceToHost, st));
     }
-    CK(cudaEventRecord(ctx->ev_comp[c], st));
-    CK(cudaStreamWaitEvent(ctx->s_out, ctx->ev_comp[c], 0));
-    CK(cudaMemcpyAsync(h.h_out + b0, h.out + b0, sizeof(ScanOut) * nb, cudaMemcpyDeviceToHost, ctx->s_out));
+    cudaStream_t so = ctx->s_out.get();
+    CK(cudaEventRecord(ctx->ev_comp[c].get(), st));
+    CK(cudaStreamWaitEvent(so, ctx->ev_comp[c].get(), 0));
+    CK(cudaMemcpyAsync(h.h_out.get() + b0, view.out, sizeof(ScanOut) * nb, cudaMemcpyDeviceToHost, so));
     for (int b = b0; b < b0 + nb; b++) {
       if (n[b] <= 0) continue;
-      if (outs[b].label) CK(cudaMemcpyAsync(outs[b].label, h.label + (size_t)b * S, sizeof(int) * (size_t)n[b], cudaMemcpyDeviceToHost, ctx->s_out));
-      if (label8 && label8[b]) CK(cudaMemcpyAsync(label8[b], h.label8 + (size_t)b * S, (size_t)n[b], cudaMemcpyDeviceToHost, ctx->s_out));
-      if (outs[b].ring) CK(cudaMemcpyAsync(outs[b].ring, ring_chunk(b0) + (size_t)(b - b0) * S, sizeof(int) * (size_t)n[b], cudaMemcpyDeviceToHost, ctx->s_out));
-      if (outs[b].order) CK(cudaMemcpyAsync(outs[b].order, h.order + (size_t)b * S, sizeof(int) * (size_t)n[b], cudaMemcpyDeviceToHost, ctx->s_out));
+      const DevBuffers v = scan_view(bufv, b, e);
+      if (outs[b].label) CK(cudaMemcpyAsync(outs[b].label, v.label, sizeof(int) * (size_t)n[b], cudaMemcpyDeviceToHost, so));
+      if (label8 && label8[b]) CK(cudaMemcpyAsync(label8[b], v.label8, (size_t)n[b], cudaMemcpyDeviceToHost, so));
+      if (outs[b].ring) CK(cudaMemcpyAsync(outs[b].ring, ring_chunk(view, b0) + (b - b0) * pts, sizeof(int) * (size_t)n[b], cudaMemcpyDeviceToHost, so));
+      if (outs[b].order) CK(cudaMemcpyAsync(outs[b].order, v.order, sizeof(int) * (size_t)n[b], cudaMemcpyDeviceToHost, so));
     }
   }
   // s_out waited for the last chunk's kernels: ev_done covers every copy and kernel of the batch
-  CK(cudaEventRecord(h.ev_done, ctx->s_out));
+  CK(cudaEventRecord(h.ev_done.get(), ctx->s_out.get()));
   h.batch = batch; h.S = S; h.launches = launches; h.outs = outs; h.clouds = clouds;
   ctx->hs_count++;
   return URF_OK;
@@ -827,12 +760,13 @@ int finish_batch(urf_ctx* ctx) {
   ctx->hs_count--;
   ctx->hs_head = ctx->hs_count ? 1 - ctx->hs_head : 0;       // idle: the next batch (and every synchronous call) takes slot 0
   CK(cudaSetDevice(ctx->device));
-  CK(cudaEventSynchronize(h.ev_done));
-  cudaStream_t st = ctx->stream;
+  CK(cudaEventSynchronize(h.ev_done.get()));
+  cudaStream_t st = ctx->stream.get();
   urf_clouds* clouds = h.clouds;
   if (clouds) {                                              // sizes are known now: copy exactly the records that exist
-    const int* t = ctx->h_packtot;
-    const float4 *d_rc = ctx->pack, *d_roi = ctx->pack + 2 * (size_t)ctx->max_points, *d_prob = ctx->pack + 4 * (size_t)ctx->max_points;
+    const int* t = ctx->h_packtot.get();
+    const float4* d_rc = ctx->pack.get();
+    const float4 *d_roi = d_rc + 2 * (size_t)ctx->max_points, *d_prob = d_rc + 4 * (size_t)ctx->max_points;
     clouds->n_road = t[0]; clouds->n_curb = t[1]; clouds->n_roi = t[2]; clouds->n_road_probably = t[3];
     const size_t rec = sizeof(urf_point_xyzi);
     if (clouds->road && t[0] > 0) CK(cudaMemcpyAsync(clouds->road, d_rc, rec * t[0], cudaMemcpyDeviceToHost, st));
@@ -842,7 +776,7 @@ int finish_batch(urf_ctx* ctx) {
     CK(cudaStreamSynchronize(st));
   }
   float ms = -1.f;
-  if (cudaEventElapsedTime(&ms, h.ev0, h.ev1) != cudaSuccess) ms = -1.f;
+  if (cudaEventElapsedTime(&ms, h.ev0.get(), h.ev1.get()) != cudaSuccess) ms = -1.f;
   ctx->last_ms = ms;
   ctx->launches = h.launches;
   ctx->timing_valid = true;
@@ -850,8 +784,8 @@ int finish_batch(urf_ctx* ctx) {
   ctx->last_B = h.batch; ctx->last_S = h.S;
   urf_result* outs = h.outs;
   for (int b = 0; b < h.batch; b++) {
-    fill_result(h.h_out[b], &outs[b], true);
-    if (outs[b].status == URF_TOO_FEW_POINTS && outs[b].ring) for (int i = 0; i < h.h_n[b]; i++) outs[b].ring[i] = -1;
+    fill_result(h.h_out.get()[b], &outs[b], true);
+    if (outs[b].status == URF_TOO_FEW_POINTS && outs[b].ring) for (int i = 0; i < h.h_n.get()[b]; i++) outs[b].ring[i] = -1;
   }
   return URF_OK;
 }
@@ -859,28 +793,19 @@ int finish_batch(urf_ctx* ctx) {
 // The second host slot, and slot 0's own ring-id buffer (include/urf.h: 32 bytes of device memory per point of capacity),
 // on the first asynchronous call (nothing is in flight then).
 int alloc_second_slot(urf_ctx* ctx) {
-  urf_ctx::HostSlot& h = ctx->hs[1];
-  if (h.ev_done) return URF_OK;
+  if (ctx->hs[1].ev_done) return URF_OK;
   CK(cudaSetDevice(ctx->device));
-  const size_t P = ctx->P;
-  urf_ctx::HostSlot t;
-  int* ring0 = nullptr;
-  int rc = dalloc(ctx, &t.in, P);
-  if (rc == URF_OK) rc = dalloc(ctx, &t.label, P);
-  if (rc == URF_OK) rc = dalloc(ctx, &t.order, P);
-  if (rc == URF_OK) rc = dalloc(ctx, &t.ring, P);
-  if (rc == URF_OK) rc = dalloc(ctx, &ring0, P);
-  if (rc == URF_OK) rc = dalloc(ctx, &t.n, (size_t)ctx->max_batch);
-  if (rc == URF_OK) rc = dalloc(ctx, &t.out, (size_t)ctx->max_batch);
-  if (rc != URF_OK) return rc;                              // device pieces stay in ctx->allocs until urf_destroy
-  if (!h.h_n) rc = cuda_rc(ctx, cudaMallocHost((void**)&h.h_n, sizeof(int) * ctx->max_batch), "cudaMallocHost");
-  if (rc == URF_OK && !h.h_out) rc = cuda_rc(ctx, cudaMallocHost((void**)&h.h_out, sizeof(ScanOut) * ctx->max_batch), "cudaMallocHost");
-  if (rc == URF_OK && !h.ev0) rc = cuda_rc(ctx, cudaEventCreate(&h.ev0), "cudaEventCreate");
-  if (rc == URF_OK && !h.ev1) rc = cuda_rc(ctx, cudaEventCreate(&h.ev1), "cudaEventCreate");
-  if (rc != URF_OK) return rc;                              // pinned pieces and events are freed by urf_destroy
-  h.in = t.in; h.label = t.label; h.order = t.order; h.ring = t.ring; h.n = t.n; h.out = t.out;
-  ctx->hs[0].ring = ring0;
-  return cuda_rc(ctx, cudaEventCreateWithFlags(&h.ev_done, cudaEventDisableTiming), "cudaEventCreate");   // last: marks the slot complete
+  const size_t P = capacity_elems(Kind::Point, capacity_extent(ctx->max_points), ctx->max_batch);
+  urf_ctx::HostSlot t;                                      // all or nothing: freed on a failure
+  DevMem<int> ring0;
+  int rc = alloc_owned(ctx, t.dev, t.mem, slot_array);
+  if (rc == URF_OK) rc = dalloc(ctx, t.ring, P);
+  if (rc == URF_OK) rc = dalloc(ctx, ring0, P);
+  if (rc == URF_OK) rc = cuda_rc(ctx, init_slot(ctx, t), "pinned rows and events of host slot 1");   // ev_done marks it complete
+  if (rc != URF_OK) return rc;
+  ctx->hs[1] = std::move(t);
+  ctx->hs[0].ring = std::move(ring0);
+  return URF_OK;
 }
 
 // The synchronous entry points: one enqueue and one finish, refused while asynchronous batches are in flight.
@@ -969,29 +894,18 @@ int urf_test_math(int device, int which, const float* a, const float* b, float* 
 int urf_debug_fetch(urf_ctx* ctx, int b, int what, void* dst, size_t bytes) {
   if (!ctx || !dst || b < 0 || b >= ctx->last_B) return URF_ERR_INVALID;
   CK(cudaSetDevice(ctx->device));
-  CK(cudaStreamSynchronize(ctx->stream));
-  const size_t off = (size_t)b * ctx->last_S;
+  CK(cudaStreamSynchronize(ctx->stream.get()));
+  const DevBuffers v = scan_view(ctx->buf, b, launch_extent(ctx->last_S, ctx->dp.channels));
   const void* src = nullptr;
+  auto clamp = [&](size_t most) { if (bytes > most) bytes = most; };
   switch (what) {
-    case 0: src = ctx->buf.alpha_v + off; break;
-    case 1: src = ctx->buf.mark + off; break;
-    case 2: src = ctx->buf.ringid + off; break;
-    case 3: src = ctx->buf.sect + off; break;
-    case 4: src = ctx->buf.az + off; break;
-    case 5: src = ctx->buf.d2 + off; break;
-    case 8: src = ctx->buf.tab + b; if (bytes > sizeof(ScanTab)) bytes = sizeof(ScanTab); break;
-    case 9: src = &ctx->buf.tab[b].nbig; if (bytes > 2 * sizeof(int)) bytes = 2 * sizeof(int); break;
-    case 10: src = &ctx->buf.tab[b].nrefine; if (bytes > sizeof(int)) bytes = sizeof(int); break;
-    case 11: case 12: {
-      const size_t ch = (size_t)ctx->dp.channels;
-      src = (what == 11 ? ctx->buf.Tf : ctx->buf.Tb) + (size_t)b * ch * kTStride;
-      if (bytes > sizeof(float) * ch * kDegBins) bytes = sizeof(float) * ch * kDegBins;
-      break;
-    }
-    case 13:
-      src = ctx->buf.firstidx + (size_t)b * (kElevBins + 1);
-      if (bytes > sizeof(unsigned) * (kElevBins + 1)) bytes = sizeof(unsigned) * (kElevBins + 1);
-      break;
+    case 0: src = v.alpha_v; break;  case 1: src = v.mark; break;  case 2: src = v.ringid; break;
+    case 3: src = v.sect; break;     case 4: src = v.az; break;    case 5: src = v.d2; break;
+    case 8: src = v.tab; clamp(sizeof(ScanTab)); break;
+    case 9: src = &v.tab->nbig; clamp(2 * sizeof(int)); break;
+    case 10: src = &v.tab->nrefine; clamp(sizeof(int)); break;
+    case 11: case 12: src = what == 11 ? v.Tf : v.Tb; clamp(sizeof(float) * ctx->dp.channels * kDegBins); break;
+    case 13: src = v.firstidx; clamp(sizeof(unsigned) * kElevSlice); break;
     default: return URF_ERR_INVALID;
   }
   CK(cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost));

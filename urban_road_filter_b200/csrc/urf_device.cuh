@@ -82,7 +82,7 @@ struct ScanTab {
   float resume[kSectKeys][4];      // per refine entry: running mean, deviation, NaN count of the walk over the prefix, its length
 };
 
-// All device buffers of a context. P = max_batch * max_points; T = ceil(max_points / kChunk).
+// All device buffers of a context (urf_workspace.cuh states their layout). P = max_batch * max_points; T = ceil(max_points / kChunk).
 struct DevBuffers {
   float4* in;            // [P]   x, y, z, intensity (input order)
   float* alpha_v;        // [P]   elevation angle in degrees, -1 = outside ROI
@@ -93,20 +93,17 @@ struct DevBuffers {
   signed char* label8;   // [P] or NULL: the same labels as one byte per point (callers that ask for int8 labels)
   float4* bpt;           // [P]   ring buckets (ring-major, input order inside a ring): x, y, z, input index bits
   // sector buckets (unordered inside a sector), in sector-slot order: planar radius (the sort key), height, input index
-  float* sr;             // [P]
-  float* sz;             // [P]
+  float *sr, *sz;        // [P], [P]
   unsigned* sidx;        // [P]
   // sector buckets sorted by r: (r, z), all the edge search reads, and per sorted position the sector slot the point came
   // from (network sorts) or its input index | 0x80000000 (exact fallback); star_input_index resolves either
   float2* ssrz;          // [P]
   unsigned* ssl;         // [P]
-  float* az;             // [P]   azimuth per input point (ROI points only)
-  float* d2;             // [P]   planar range per input point (ROI points only)
+  float *az, *d2;        // [P]   azimuth, planar range per input point (ROI points only)
   uint2* baz;            // [P]   (azimuth bits, input index) per bucket position (written by k_scatter only when the emission order is wanted)
   uint4* roadlist;       // [P]   road points, 32 slots per warp of input points: (bin | ring << 16, azimuth bits, range bits, input index)
   unsigned char* roadcnt; // [B][ceil(S / 32)] road points of each input warp (entries used in its 32 list slots)
-  float* Tf;             // [B][channels][kTStride] forward threshold table (urf_logic.cuh build_T_row)
-  float* Tb;             // [B][channels][kTStride] backward threshold table
+  float *Tf, *Tb;        // [B][channels][kTStride] forward / backward threshold tables (urf_logic.cuh build_T_row)
   unsigned short* lut;   // [B][kElevBins + 1] ring-search start per fine elevation bin
   int* order;            // [P]   emission order (input indices), only when requested
   int* epos;             // [P] or NULL: emission position per input point (reference tie order: the marker search's scan order)
@@ -114,8 +111,7 @@ struct DevBuffers {
   unsigned long long* sortbuf;   // [2P] scratch for segments too large for shared memory
   unsigned* hist;        // [B][T][channels] per-chunk ring histograms, turned into scatter offsets in place
   unsigned* firstidx;    // [B][kElevBins + 1] first input index per fine elevation bin
-  unsigned* cmin;        // [B][channels][kDegBins] float bits: min curb azimuth per (ring, degree bin), +inf = empty
-  unsigned* cmax;        // [B][channels][kDegBins] float bits: max curb azimuth per (ring, degree bin)
+  unsigned *cmin, *cmax; // [B][channels][kDegBins] float bits: min / max curb azimuth per (ring, degree bin), min +inf = empty
   unsigned short* ne;    // [B][channels][kDegBins + 1] prefix count of non-empty curb bins
   float* newY;           // [max_points] x-zero `newY` ramp (x_zero_method.cpp:24-27), depends on the index only
   int* n;                // [B] points per scan

@@ -21,6 +21,7 @@
 #include "urf_logic.cuh"
 #include "urf_lomuto.cuh"
 #include "urf_stdsort.cuh"
+#include "urf_workspace.cuh"
 
 namespace urf {
 
@@ -31,7 +32,7 @@ __constant__ unsigned char c_beam_yx[kSectKeys];
 __device__ __forceinline__ int lane_id() { return threadIdx.x & 31; }
 // 32-bit offset of scan b inside the batch-major arrays (urf_create keeps max_batch * max_points below 2^31): array
 // accesses then cost one IMAD.WIDE instead of 64-bit multiply/add chains
-__device__ __forceinline__ unsigned scan_base(int b, int S) { return (unsigned)b * (unsigned)S; }
+__device__ __forceinline__ unsigned scan_base(int b, int S) { return (unsigned)b * point_slice((unsigned)S); }
 
 // The thread groups that sort together in memory: the whole CTA, or one warp.
 struct CtaGroup {
@@ -75,7 +76,7 @@ __device__ __forceinline__ void curb_hit(const DevBuffers& buf, const DevParams&
   if (k < 0) return;                                   // not in array3D: the mark is never read (lidar_segmentation.cpp:241)
   const float a = buf.az[gb + (unsigned)idx];
   if (a >= 0.0f) {
-    const unsigned o = ((unsigned)b * (unsigned)prm.channels + (unsigned)k) * kDegBins + (unsigned)deg_bin(a);
+    const unsigned o = (unsigned)b * degbin_slice((unsigned)prm.channels) + (unsigned)k * kDegBins + (unsigned)deg_bin(a);
     atomicMin(&buf.cmin[o], fbits(a));
     atomicMax(&buf.cmax[o], fbits(a));
   }
@@ -103,10 +104,10 @@ __global__ void k_reset(DevBuffers buf, DevParams prm) {
   for (int i = tid; i < kDegBins; i += nth) { t.cutbest[i] = ~0ull; t.dmax[i] = 0u; t.best[i] = ~0ull; }
   for (int i = tid; i < kSectKeys; i += nth) t.sect_cnt[i] = 0;
   if (tid == 0) { t.nbig = 0; t.nslow = 0; t.nrefine = 0; }
-  if (tid == 0 && buf.lomuto) buf.lomuto[(size_t)b * (kRingKeys + 1)] = 0;
-  unsigned* fi = buf.firstidx + (size_t)b * (kElevBins + 1);
+  if (tid == 0 && buf.lomuto) buf.lomuto[(size_t)b * kRingListSlice] = 0;
+  unsigned* fi = buf.firstidx + (size_t)b * kElevSlice;
   for (int i = tid; i <= kElevBins; i += nth) fi[i] = 0xffffffffu;
-  const size_t nb = (size_t)prm.channels * kDegBins;
+  const size_t nb = degbin_slice((size_t)prm.channels);
   unsigned* cmin = buf.cmin + (size_t)b * nb;
   unsigned* cmax = buf.cmax + (size_t)b * nb;
   for (size_t i = tid; i < nb; i += nth) { cmin[i] = 0x7f800000u; cmax[i] = 0u; }
@@ -190,7 +191,7 @@ __global__ void __launch_bounds__(kPtsThreads) k_points(DevBuffers buf, DevParam
   roi = __reduce_add_sync(0xffffffffu, roi);
   if (lane_id() == 0 && roi) atomicAdd(&s_roi, roi);
   __syncthreads();
-  unsigned* fi = buf.firstidx + (size_t)b * (kElevBins + 1);
+  unsigned* fi = buf.firstidx + (size_t)b * kElevSlice;
   for (int e = threadIdx.x; e <= kElevBins; e += kPtsThreads) {
     const unsigned v = s_first[e];
     if (v != 0xffffffffu) atomicMin(&fi[e], v);
@@ -275,7 +276,7 @@ __global__ void __launch_bounds__(256) k_register(DevBuffers buf, DevParams prm,
   const int n = buf.n[b];
   ScanOut& out = buf.out[b];
   ScanTab& tab = buf.tab[b];
-  const float* alpha = buf.alpha_v + (size_t)b * S;
+  const float* alpha = buf.alpha_v + (size_t)b * point_slice(S);
   __shared__ unsigned s_cand[kMaxCand];
   __shared__ float s_calpha[kMaxCand];
   __shared__ float s_vis[kRingKeys];
@@ -293,7 +294,7 @@ __global__ void __launch_bounds__(256) k_register(DevBuffers buf, DevParams prm,
   if (!exact) {
     if (threadIdx.x == 0) s_cnt = 0;
     __syncthreads();
-    const unsigned* fi = buf.firstidx + (size_t)b * (kElevBins + 1);
+    const unsigned* fi = buf.firstidx + (size_t)b * kElevSlice;
     for (int t = threadIdx.x; t <= kElevBins; t += blockDim.x) {
       const unsigned v = fi[t];
       if (v != 0xffffffffu) { int s = atomicAdd(&s_cnt, 1); if (s < kMaxCand) s_cand[s] = v; }
@@ -333,7 +334,7 @@ __global__ void __launch_bounds__(256) k_register(DevBuffers buf, DevParams prm,
     if (threadIdx.x == 0) { s_m = m; atomicOr(&out.flags, F_EXACT_REG); }
     __syncthreads();
   }
-  publish_rings_cta(tab, out, buf.lut + (size_t)b * (kElevBins + 1), prm.interval, s_reg, s_idx, s_m, s_keys, s_sorted);
+  publish_rings_cta(tab, out, buf.lut + (size_t)b * kElevSlice, prm.interval, s_reg, s_idx, s_m, s_keys, s_sorted);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -383,7 +384,7 @@ __device__ __forceinline__ bool assign_chunk(const DevBuffers& buf, const DevPar
   __syncwarp();
   // rows are `channels` counters wide: ring ids are below n_rings <= channels
   const int C = prm.channels;
-  unsigned* row = buf.hist + ((size_t)b * T + chunk) * C;
+  unsigned* row = buf.hist + ((size_t)b * chunk_rows(T) + chunk) * C;
   for (int t = lane; t < C; t += 32) row[t] = cnt[t];
   return violation;
 }
@@ -405,7 +406,7 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32) k_assign(DevBuffers buf, 
   __syncthreads();
   if (chunk * kChunk >= n) return;             // whole warp; no block-level sync follows
   const bool violation = assign_chunk(buf, prm, b, S, T, chunk, n, out.n_roi >= 30, !(flags & F_EXACT_REG), s_angle, s_regidx, tab.regorder, R,
-                                      buf.lut + (size_t)b * (kElevBins + 1), s_cnt[warp], lane);
+                                      buf.lut + (size_t)b * kElevSlice, s_cnt[warp], lane);
   if (__any_sync(0xffffffffu, violation) && lane == 0) atomicOr(&out.flags, F_SPEC_VIOLATION);
 }
 
@@ -439,11 +440,11 @@ __global__ void __launch_bounds__(kScanOffThreads, 2) k_scan_offsets(DevBuffers 
       __shared__ int s_red[32];
       __shared__ int s_m;
       int m;
-      register_exact_cta(buf.alpha_v + (size_t)b * S, n, prm.interval, prm.channels, s_vis, s_reg, s_idx, s_red, &m);
+      register_exact_cta(buf.alpha_v + (size_t)b * point_slice(S), n, prm.interval, prm.channels, s_vis, s_reg, s_idx, s_red, &m);
       if (threadIdx.x == 0) s_m = m;
       __syncthreads();
-      const unsigned short* lut = buf.lut + (size_t)b * (kElevBins + 1);
-      publish_rings_cta(buf.tab[b], out, buf.lut + (size_t)b * (kElevBins + 1), prm.interval, s_reg, s_idx, s_m, s_keys, s_sorted);
+      const unsigned short* lut = buf.lut + (size_t)b * kElevSlice;
+      publish_rings_cta(buf.tab[b], out, buf.lut + (size_t)b * kElevSlice, prm.interval, s_reg, s_idx, s_m, s_keys, s_sorted);
       __syncthreads();                                                // s_sorted = the sorted angles, lut written
       const int R = s_m;
       for (int c0 = 0; c0 < rows; c0 += kScanOffWarps) {
@@ -460,7 +461,7 @@ __global__ void __launch_bounds__(kScanOffThreads, 2) k_scan_offsets(DevBuffers 
   const unsigned scnt = threadIdx.x < kSectKeys ? (unsigned)tab.sect_cnt[threadIdx.x] : 0u;   // in flight during the row sums
   const int rpw = (rows + kScanOffWarps - 1) / kScanOffWarps;
   const int r0 = min(rows, warp * rpw), r1 = min(rows, (warp + 1) * rpw);
-  unsigned* hist = buf.hist + (size_t)b * T * C;
+  unsigned* hist = buf.hist + (size_t)b * chunk_rows(T) * C;
   for (int key = lane; key < C; key += 32) {
     unsigned s = 0;
     for (int r = r0; r < r1; r += kScanOffBatch) {
@@ -562,7 +563,7 @@ __global__ void __launch_bounds__(kScatterWarps * 32, 4) k_scatter(DevBuffers bu
   unsigned short* perm = s_perm[warp];
   ScanTab& tab = buf.tab[b];
   const bool live = chunk * kChunk < n;                           // a warp past the end only takes part in the barriers
-  const unsigned* row = buf.hist + ((size_t)b * T + chunk) * prm.channels;
+  const unsigned* row = buf.hist + ((size_t)b * chunk_rows(T) + chunk) * prm.channels;
   const unsigned gb = scan_base(b, S), g0 = gb + (unsigned)chunk * kChunk;
   if (live && lane == 0) {                                        // clipped at the end of the scan
     mbar_init(&s_bar[warp], 1);
@@ -1045,9 +1046,9 @@ __global__ void __launch_bounds__(kSortWarps * 32, 3) k_star_sort(DevBuffers buf
 // by index) and ONE thread runs the restated std::sort (urf_stdsort.cuh) over them.
 template <class G>
 __device__ void slow_sort_sector(const DevBuffers& buf, int b, int S, int base, int n, unsigned long long* s_keys, int cap) {
-  const size_t o = (size_t)b * S + base;
+  const size_t o = (size_t)b * point_slice(S) + base;
   const int npad = next_pow2(n < 2 ? 2 : n);
-  unsigned long long* keys = npad <= cap ? s_keys : buf.sortbuf + 2 * o;
+  unsigned long long* keys = npad <= cap ? s_keys : buf.sortbuf + pair_slice(o);
   G::sync();
   for (int t = G::rank(); t < npad; t += G::size())
     keys[t] = t < n ? (((unsigned long long)fbits(buf.sr[o + t]) << 32) | buf.sidx[o + t]) : ~0ull;
@@ -1068,7 +1069,7 @@ __device__ void slow_sort_sector(const DevBuffers& buf, int b, int S, int base, 
   for (int t = G::rank(); t < n; t += G::size()) {
     const unsigned long long k = keys[t];
     const unsigned idx = (unsigned)k;
-    buf.ssrz[o + t] = make_float2(bitsf((unsigned)(k >> 32)), buf.in[(size_t)b * S + idx].z);
+    buf.ssrz[o + t] = make_float2(bitsf((unsigned)(k >> 32)), buf.in[(size_t)b * point_slice(S) + idx].z);
     buf.ssl[o + t] = idx | kSslIndex;
   }
   G::sync();
@@ -1271,7 +1272,7 @@ __global__ void __launch_bounds__(kScanWarps * 32) k_star_scan(DevBuffers buf, D
     base = tab.sect_start[s]; whole = tab.sect_start[s + 1] - base;
     n = min(whole, tab.sorted_len[s]);               // walk the sorted prefix only
   }
-  const float2* all = buf.ssrz + (size_t)b * S;
+  const float2* all = buf.ssrz + (size_t)b * point_slice(S);
   StarState st;
   star_init(st, 0.f, 0.f);
   bool done = n <= 1;                                                   // star_shaped_search.cpp:112
@@ -1617,9 +1618,9 @@ __global__ void __launch_bounds__(256) k_tab1(DevBuffers buf, DevParams prm) {
   const int warp = threadIdx.x >> 5, lane = lane_id();
   if (blockIdx.x == 0) for (int t = threadIdx.x; t < 2 * kDegBins; t += blockDim.x) tab.reach[t / kDegBins][t % kDegBins] = R;
   if (R <= 0) return;
-  const size_t nb = (size_t)prm.channels * kDegBins;
+  const size_t nb = degbin_slice((size_t)prm.channels);
   const unsigned* cmin = buf.cmin + (size_t)b * nb;
-  unsigned short* ne = buf.ne + (size_t)b * prm.channels * (kDegBins + 1);
+  unsigned short* ne = buf.ne + (size_t)b * degsum_slice((size_t)prm.channels);
   for (int k = blockIdx.x * 8 + warp; k < R; k += gridDim.x * 8) {        // one warp per ring: 12 x 32 bins with a running carry
     unsigned carry = 0;
     for (int c = 0; c < (kDegBins + 31) / 32; c++) {
@@ -1655,8 +1656,8 @@ __global__ void __launch_bounds__(256) k_reach(DevBuffers buf, DevParams prm) {
   if (w >= 2 * kDegBins || R <= 0) return;
   const int dir = w / kDegBins, i = w % kDegBins;
   if (dir == 0 ? i > prm.fwd_last : i < prm.bwd_first) return;          // outside the loop range: never accepted anyway
-  const size_t nb = (size_t)prm.channels * kDegBins;
-  CurbView cv{buf.cmin + (size_t)b * nb, buf.cmax + (size_t)b * nb, buf.ne + (size_t)b * prm.channels * (kDegBins + 1)};
+  const size_t nb = degbin_slice((size_t)prm.channels);
+  CurbView cv{buf.cmin + (size_t)b * nb, buf.cmax + (size_t)b * nb, buf.ne + (size_t)b * degsum_slice((size_t)prm.channels)};
   int reach = R;
   for (int k0 = 0; k0 < R; k0 += 32) {
     const int k = k0 + lane;
@@ -1710,7 +1711,7 @@ __global__ void __launch_bounds__(kTab2Rings * 64) k_tab2(DevBuffers buf, DevPar
   }
   __syncthreads();
   const size_t ch = prm.channels;
-  const size_t o = (size_t)b * ch * kTStride + k0;
+  const size_t o = (size_t)b * ttab_slice(ch) + k0;
   const int nk = min(kTab2Rings, R - k0);
   for (int t = threadIdx.x; t < 2 * kDegBins * kTab2Rings; t += blockDim.x) {
     const int kk = t % kTab2Rings, j = (t / kTab2Rings) % kDegBins, d = t / (kTab2Rings * kDegBins);
@@ -1758,7 +1759,7 @@ __global__ void __launch_bounds__(kLabelThreads) k_label(DevBuffers buf, DevPara
   float tf[G], tb[G];
   unsigned long long cb[G];
   int bin[G];
-  const unsigned ob = (unsigned)b * (unsigned)prm.channels * kTStride;
+  const unsigned ob = (unsigned)b * ttab_slice((unsigned)prm.channels);
 #pragma unroll
   for (int u = 0; u < G; u++) {
     const bool valid = k[u] >= 0 && a[u] >= 0.0f;
@@ -1796,7 +1797,7 @@ __global__ void __launch_bounds__(kLabelThreads) k_label(DevBuffers buf, DevPara
     const unsigned br = __ballot_sync(0xffffffffu, lab == 1), bc = __ballot_sync(0xffffffffu, lab == 2);
     nroad += __popc(br);
     ncurb += __popc(bc);
-    if (lane == 0) buf.roadcnt[(size_t)b * ((S + 31) >> 5) + (unsigned)(i >> 5)] = (unsigned char)__popc(br);
+    if (lane == 0) buf.roadcnt[(size_t)b * warp_slice(S) + (unsigned)(i >> 5)] = (unsigned char)__popc(br);
     if (lab == 1)
       buf.roadlist[gb + (unsigned)(i & ~31) + (unsigned)__popc(br & ((1u << lane) - 1u))] =
           make_uint4((unsigned)bin[u] | ((unsigned)k[u] << 16), fbits(a[u]), fbits(d[u]), (unsigned)pos[u]);
@@ -1881,8 +1882,8 @@ __device__ __forceinline__ void write_vertices(const DevBuffers& buf, int b, int
   if (has) {
     const int slot = off + __popc(bal & ((1u << lane) - 1u));
     int p = (int)(best[i] & 0xffffffull);               // input index of the winner (REF: its emission position)
-    if (REF) p = buf.order[(size_t)b * S + p];
-    const float4 q = buf.in[(size_t)b * S + p];
+    if (REF) p = buf.order[(size_t)b * point_slice(S) + p];
+    const float4 q = buf.in[(size_t)b * point_slice(S) + p];
     out.vert[slot][0] = q.x; out.vert[slot][1] = q.y; out.vert[slot][2] = q.z;
     out.vert[slot][3] = cut[i] != ~0ull ? 1.0f : 0.0f;
   }
@@ -1901,7 +1902,7 @@ __global__ void __launch_bounds__(kMark1Threads) k_markers1(DevBuffers buf, int 
   __syncthreads();
   const int n = buf.n[b];
   const int nseg = (n + 31) >> 5;
-  const unsigned char* cnt = buf.roadcnt + (size_t)b * ((S + 31) >> 5);
+  const unsigned char* cnt = buf.roadcnt + (size_t)b * warp_slice(S);
   const uint4* list = buf.roadlist + scan_base(b, S);
   markers_pass<1>(list, cnt, nseg, s_cut, s_dmax, s_best);
   __syncthreads();
@@ -1928,7 +1929,7 @@ __global__ void __launch_bounds__(kMarkGridThreads) k_markers_grid(DevBuffers bu
   __syncthreads();
   const int n = buf.n[b];
   const int nseg = (n + 31) >> 5;
-  const unsigned char* cnt = buf.roadcnt + (size_t)b * ((S + 31) >> 5);
+  const unsigned char* cnt = buf.roadcnt + (size_t)b * warp_slice(S);
   const uint4* list = buf.roadlist + scan_base(b, S);
   markers_pass<PASS>(list, cnt, nseg, s_cut, s_dmax, s_best);
   __syncthreads();
@@ -1962,7 +1963,7 @@ constexpr int kRingFast = 4096, kRingBins = 4096, kBinCap = 48;
 constexpr int kSortThreads = 512;
 __device__ __forceinline__ void lomuto_enlist(const DevBuffers& buf, int b, int k, bool weird) {
   if (__syncthreads_or(weird) && threadIdx.x == 0) {
-    int* l = buf.lomuto + (size_t)b * (kRingKeys + 1);
+    int* l = buf.lomuto + (size_t)b * kRingListSlice;
     l[1 + atomicAdd(l, 1)] = k;
   }
 }
@@ -1974,7 +1975,7 @@ __global__ void __launch_bounds__(kSortThreads) k_sort_rings(DevBuffers buf, int
   if (k >= out.n_rings) return;
   const int base = out.ring_start[k], n = out.ring_start[k + 1] - base;
   if (n <= 0) return;
-  const size_t gb = (size_t)b * S, g0 = gb + base;
+  const size_t gb = (size_t)b * point_slice(S), g0 = gb + base;
   const int tid = threadIdx.x;
   if (n <= kRingFast) {
     unsigned* s_az = reinterpret_cast<unsigned*>(s_rkeys);            // [kRingFast] azimuth bits by ring position
@@ -2067,7 +2068,7 @@ __global__ void __launch_bounds__(kSortThreads) k_sort_rings(DevBuffers buf, int
     __syncthreads();                                                   // the fallback reuses the shared memory
   }
   const int npad = next_pow2(n < 2 ? 2 : n);
-  unsigned long long* keys = npad <= kRingSmemKeys ? s_rkeys : buf.sortbuf + 2 * g0;
+  unsigned long long* keys = npad <= kRingSmemKeys ? s_rkeys : buf.sortbuf + pair_slice(g0);
   for (int t = tid; t < npad; t += blockDim.x)
     keys[t] = t < n ? (((unsigned long long)buf.baz[g0 + t].x << 32) | (unsigned)t) : ~0ull;
   __syncthreads();
@@ -2122,14 +2123,14 @@ __global__ void __launch_bounds__(kLomutoThreads) k_lomuto_rings(DevBuffers buf,
   extern __shared__ unsigned s_lw[];
   __shared__ LomutoShared sh;
   const int b = blockIdx.y;
-  const int* list = buf.lomuto + (size_t)b * (kRingKeys + 1);
+  const int* list = buf.lomuto + (size_t)b * kRingListSlice;
   if ((int)blockIdx.x >= list[0]) return;
   const int k = list[1 + blockIdx.x];
   const ScanOut& out = buf.out[b];
   const int base = out.ring_start[k], n = out.ring_start[k + 1] - base;
   const unsigned gb = scan_base(b, S), g0 = gb + (unsigned)base;
   const bool smem = n <= kLomutoSmemPts;
-  unsigned* w = smem ? s_lw : reinterpret_cast<unsigned*>(buf.sortbuf + 2 * (size_t)g0);
+  unsigned* w = smem ? s_lw : reinterpret_cast<unsigned*>(buf.sortbuf + pair_slice((size_t)g0));
   for (int t = threadIdx.x; t < n; t += blockDim.x) {
     const uint2 q = buf.baz[g0 + t];
     w[t] = q.x;
@@ -2161,8 +2162,8 @@ __global__ void __launch_bounds__(256) k_unpack_cloud2_batch(const unsigned char
                                                               int off_z, int off_i) {
   const int b = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n[b]) return;
-  const unsigned char* rec = raw + ((size_t)b * S + i) * point_step;
-  dst[(size_t)b * S + i] = make_float4(load_f32_unaligned(rec + off_x), load_f32_unaligned(rec + off_y), load_f32_unaligned(rec + off_z),
+  const unsigned char* rec = raw + ((size_t)b * point_slice(S) + i) * point_step;
+  dst[(size_t)b * point_slice(S) + i] = make_float4(load_f32_unaligned(rec + off_x), load_f32_unaligned(rec + off_y), load_f32_unaligned(rec + off_z),
                                        off_i >= 0 ? load_f32_unaligned(rec + off_i) : 0.f);
 }
 
