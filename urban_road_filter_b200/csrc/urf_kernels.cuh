@@ -34,12 +34,83 @@ __device__ __forceinline__ int lane_id() { return threadIdx.x & 31; }
 // accesses then cost one IMAD.WIDE instead of 64-bit multiply/add chains
 __device__ __forceinline__ unsigned scan_base(int b, int S) { return (unsigned)b * point_slice((unsigned)S); }
 
+// Inclusive prefix sums over the warp's lanes of N values per lane at once (N independent sums, one shuffle ladder).
+// Every lane of the warp calls it.
+template <int N, class T>
+__device__ __forceinline__ void warp_inclusive_sum(T (&x)[N]) {
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    T u[N];
+#pragma unroll
+    for (int i = 0; i < N; i++) u[i] = __shfl_up_sync(0xffffffffu, x[i], d);
+    if (lane_id() >= d)
+#pragma unroll
+      for (int i = 0; i < N; i++) x[i] += u[i];
+  }
+}
+// Append to a list in shared memory: the slot of a flagged lane, in lane order after the *counter entries taken before
+// (one shared atomic per warp). Every lane of the warp calls it; a lane without the flag gets a value it must not use.
+template <class T>
+__device__ __forceinline__ T warp_append(bool flag, T* counter) {
+  const unsigned bal = __ballot_sync(0xffffffffu, flag);
+  T base = 0;
+  if (lane_id() == 0 && bal) base = atomicAdd(counter, (T)__popc(bal));
+  return __shfl_sync(0xffffffffu, base, 0) + (T)__popc(bal & ((1u << lane_id()) - 1u));
+}
+
 // The thread groups that sort together in memory: the whole CTA, or one warp.
+// The CTA-wide helpers (exclusive_sum, count, min) share one contract: every thread of the CTA calls them, the CTA has at
+// most 32 warps, and the scratch is the helper's own function-scope __shared__ array for 32 warps. A helper holds every
+// barrier it needs, the last one after its final read of that scratch, so two calls may follow each other without a
+// barrier of the caller's between them. Shared memory the caller writes after a call still wants the caller's barrier.
 struct CtaGroup {
   static __device__ __forceinline__ unsigned rank() { return threadIdx.x; }
   static __device__ __forceinline__ unsigned size() { return blockDim.x; }
   static __device__ __forceinline__ void sync() { __syncthreads(); }
   static __device__ __forceinline__ bool any(bool p) { return __syncthreads_or(p); }
+  // x[i] becomes the sum of x[i] over the threads before this one (thread order); total[i] = the sum over the CTA
+  template <int N, class T>
+  static __device__ __forceinline__ void exclusive_sum(T (&x)[N], T (&total)[N]) {
+    __shared__ T s_w[N][32];
+    const int lane = lane_id(), warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    T inc[N];
+#pragma unroll
+    for (int i = 0; i < N; i++) inc[i] = x[i];
+    warp_inclusive_sum(inc);
+    if (lane == 31)
+#pragma unroll
+      for (int i = 0; i < N; i++) s_w[i][warp] = inc[i];
+    __syncthreads();
+#pragma unroll
+    for (int i = 0; i < N; i++) {                          // lane w holds warp w's total
+      const T c = lane < nw ? s_w[i][lane] : (T)0;
+      x[i] = __reduce_add_sync(0xffffffffu, lane < warp ? c : (T)0) + inc[i] - x[i];
+      total[i] = __reduce_add_sync(0xffffffffu, c);
+    }
+    __syncthreads();
+  }
+  // exclusive count of p over the threads before this one, and the CTA's total
+  static __device__ __forceinline__ int count(bool p, int* total) {
+    __shared__ int s_w[32];
+    const unsigned bal = __ballot_sync(0xffffffffu, p);
+    const int lane = lane_id(), warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    if (lane == 0) s_w[warp] = __popc(bal);
+    __syncthreads();
+    const int c = lane < nw ? s_w[lane] : 0;
+    const int before = __reduce_add_sync(0xffffffffu, lane < warp ? c : 0);
+    *total = __reduce_add_sync(0xffffffffu, c);
+    __syncthreads();
+    return before + __popc(bal & ((1u << lane) - 1u));
+  }
+  static __device__ __forceinline__ int min(int v) {
+    __shared__ int s_w[32];
+    v = __reduce_min_sync(0xffffffffu, v);
+    if (lane_id() == 0) s_w[threadIdx.x >> 5] = v;
+    __syncthreads();
+    v = __reduce_min_sync(0xffffffffu, lane_id() < (int)(blockDim.x >> 5) ? s_w[lane_id()] : 0x7fffffff);
+    __syncthreads();
+    return v;
+  }
 };
 struct WarpGroup {
   static __device__ __forceinline__ int rank() { return lane_id(); }
@@ -209,8 +280,7 @@ __global__ void __launch_bounds__(kPtsThreads) k_points(DevBuffers buf, DevParam
 //
 // Exact path (any input): rounds of "find the first uncovered point after the last registrant" with a CTA-wide min.
 __device__ void register_exact_cta(const float* __restrict__ alpha, int n, float interval, int channels, float* s_vis,
-                                   float* s_reg, int* s_idx, int* s_red, int* out_m) {
-  __shared__ int s_min;
+                                   float* s_reg, int* s_idx, int* out_m) {
   int m = 0, vis = 0, i_last = -1;
   bool frozen = false;
   while (m < channels) {
@@ -224,17 +294,7 @@ __device__ void register_exact_cta(const float* __restrict__ alpha, int n, float
       }
       if (!cov) { local = i; break; }
     }
-    for (int o = 16; o > 0; o >>= 1) local = min(local, __shfl_xor_sync(0xffffffffu, local, o));
-    if (lane_id() == 0) s_red[threadIdx.x >> 5] = local;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      int v = 0x7fffffff;
-      for (int w = 0; w < (int)(blockDim.x >> 5); w++) v = min(v, s_red[w]);
-      s_min = v;
-    }
-    __syncthreads();
-    const int istar = s_min;
-    __syncthreads();
+    const int istar = CtaGroup::min(local);
     if (istar == 0x7fffffff) break;
     const float a = alpha[istar];
     if (threadIdx.x == 0) { s_reg[m] = a; s_idx[m] = istar; if (!frozen && a != 0.0f) s_vis[vis] = a; }
@@ -284,7 +344,6 @@ __global__ void __launch_bounds__(256) k_register(DevBuffers buf, DevParams prm,
   __shared__ float s_sorted[kRingKeys];
   __shared__ int s_idx[kRingKeys];
   __shared__ unsigned long long s_keys[kRingKeys];
-  __shared__ int s_red[8];
   __shared__ int s_cnt, s_m;
   if (out.n_roi < 30) {                      // lidar_segmentation.cpp:124-126: nothing happens for this scan
     if (threadIdx.x == 0) out.n_rings = 0;
@@ -330,7 +389,7 @@ __global__ void __launch_bounds__(256) k_register(DevBuffers buf, DevParams prm,
   }
   if (exact) {
     int m;
-    register_exact_cta(alpha, n, prm.interval, prm.channels, s_vis, s_reg, s_idx, s_red, &m);
+    register_exact_cta(alpha, n, prm.interval, prm.channels, s_vis, s_reg, s_idx, &m);
     if (threadIdx.x == 0) { s_m = m; atomicOr(&out.flags, F_EXACT_REG); }
     __syncthreads();
   }
@@ -424,7 +483,6 @@ static_assert(kRingKeys < kScanOffThreads && kSectKeys <= kScanOffThreads, "one 
 __global__ void __launch_bounds__(kScanOffThreads, 2) k_scan_offsets(DevBuffers buf, DevParams prm, int S, int T) {
   __shared__ unsigned s_part[kScanOffWarps][kRingKeys];     // per-warp partial sums, then per-warp exclusive prefixes
   __shared__ unsigned s_base[kRingKeys];
-  __shared__ unsigned s_wsum[2][kScanOffWarps];             // per-warp totals of the ring and sector scans
   const int b = blockIdx.x;
   const int n = buf.n[b];
   const int C = prm.channels;
@@ -437,10 +495,9 @@ __global__ void __launch_bounds__(kScanOffThreads, 2) k_scan_offsets(DevBuffers 
       __shared__ float s_vis[kRingKeys], s_reg[kRingKeys], s_sorted[kRingKeys];
       __shared__ int s_idx[kRingKeys];
       __shared__ unsigned long long s_keys[kRingKeys];
-      __shared__ int s_red[32];
       __shared__ int s_m;
       int m;
-      register_exact_cta(buf.alpha_v + (size_t)b * point_slice(S), n, prm.interval, prm.channels, s_vis, s_reg, s_idx, s_red, &m);
+      register_exact_cta(buf.alpha_v + (size_t)b * point_slice(S), n, prm.interval, prm.channels, s_vis, s_reg, s_idx, &m);
       if (threadIdx.x == 0) s_m = m;
       __syncthreads();
       const unsigned short* lut = buf.lut + (size_t)b * kElevSlice;
@@ -478,22 +535,9 @@ __global__ void __launch_bounds__(kScanOffThreads, 2) k_scan_offsets(DevBuffers 
   if (threadIdx.x < C)
     for (int w = 0; w < kScanOffWarps; w++) { const unsigned v = s_part[w][threadIdx.x]; s_part[w][threadIdx.x] = rtot; rtot += v; }
   // CTA-wide exclusive scans of the ring totals (-> ring bases) and of the sector counts (-> sector starts)
-  unsigned xr = rtot, xs = scnt;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    const unsigned ur = __shfl_up_sync(0xffffffffu, xr, d), us = __shfl_up_sync(0xffffffffu, xs, d);
-    if (lane >= d) { xr += ur; xs += us; }
-  }
-  if (lane == 31) { s_wsum[0][warp] = xr; s_wsum[1][warp] = xs; }
-  __syncthreads();
-  unsigned all_r = 0, all_s = 0;
-#pragma unroll
-  for (int w = 0; w < kScanOffWarps; w++) {
-    const unsigned ur = s_wsum[0][w], us = s_wsum[1][w];
-    if (w < warp) { xr += ur; xs += us; }
-    all_r += ur; all_s += us;
-  }
-  xr -= rtot; xs -= scnt;                         // exclusive
+  unsigned x[2] = {rtot, scnt}, all[2];
+  CtaGroup::exclusive_sum(x, all);
+  const unsigned xr = x[0], xs = x[1], all_r = all[0], all_s = all[1];
   ScanOut& o = buf.out[b];
   if (threadIdx.x < C) s_base[threadIdx.x] = xr;
   if (threadIdx.x <= kRingKeys) o.ring_start[threadIdx.x] = (int)(threadIdx.x < C ? xr : all_r);
@@ -635,9 +679,9 @@ __global__ void __launch_bounds__(kScatterWarps * 32, 4) k_scatter(DevBuffers bu
       unsigned v[kRingKeys / 32], sum = 0;
 #pragma unroll
       for (int j = 0; j < kRingKeys / 32; j++) { v[j] = lcnt[lane * (kRingKeys / 32) + j]; sum += v[j]; }
-      unsigned inc = sum;
-      for (int o = 1; o < 32; o <<= 1) { unsigned t = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += t; }
-      unsigned run = inc - sum;
+      unsigned inc[1] = {sum};
+      warp_inclusive_sum(inc);
+      unsigned run = inc[0] - sum;
       __syncwarp();
 #pragma unroll
       for (int j = 0; j < kRingKeys / 32; j++) { lcnt[lane * (kRingKeys / 32) + j] = run; run += v[j]; }
@@ -1096,15 +1140,11 @@ __device__ __forceinline__ int select_near_cta(const float* __restrict__ sr, int
   __syncthreads();
   const unsigned pivot = s_misc[0];
   __syncthreads();                                     // everybody has read the samples: the lists may be overwritten
-  const unsigned lt = (1u << (tid & 31)) - 1u;
 #pragma unroll
   for (int r = 0; r < EPL; r++) {
     const bool sel = key[r] < pivot;                   // padding keys are 0xffffffff: never selected
-    const unsigned bs = __ballot_sync(0xffffffffu, sel);
-    unsigned wb = 0;
-    if ((tid & 31) == 0 && bs) wb = atomicAdd(&s_misc[1], (unsigned)__popc(bs));
-    wb = __shfl_sync(0xffffffffu, wb, 0);
-    if (sel) { const unsigned pos = wb + __popc(bs & lt); s_pk[pos] = key[r]; s_pe[pos] = (unsigned)(r * 256 + tid); }
+    const unsigned pos = warp_append(sel, &s_misc[1]);
+    if (sel) { s_pk[pos] = key[r]; s_pe[pos] = (unsigned)(r * 256 + tid); }
   }
   __syncthreads();
   return (int)s_misc[1];
@@ -1425,16 +1465,9 @@ __global__ void __launch_bounds__(256, 8) k_ring_detect(DevBuffers buf, DevParam
     }
   }
   if (tiled) {
-    const unsigned bx = __ballot_sync(0xffffffffu, need_x), bz = __ballot_sync(0xffffffffu, need_z);
-    const unsigned lt = (1u << lane_id()) - 1u;
-    int ox = 0, oz = 0;
-    if (lane_id() == 0) {
-      if (bx) ox = atomicAdd(&s_nx, __popc(bx));
-      if (bz) oz = atomicAdd(&s_nz, __popc(bz));
-    }
-    ox = __shfl_sync(0xffffffffu, ox, 0); oz = __shfl_sync(0xffffffffu, oz, 0);
-    if (need_x) s_item[ox + __popc(bx & lt)] = (unsigned short)tid;
-    if (need_z) s_item[511 - (oz + __popc(bz & lt))] = (unsigned short)tid;
+    const int ox = warp_append(need_x, &s_nx), oz = warp_append(need_z, &s_nz);
+    if (need_x) s_item[ox] = (unsigned short)tid;
+    if (need_z) s_item[511 - oz] = (unsigned short)tid;
     __syncthreads();
     const int nx = s_nx, nz = s_nz;
     for (int it = tid; it < nx; it += 256) {                            // x-zero angle tests, x_zero_method.cpp:35-61
@@ -1544,12 +1577,9 @@ __global__ void __launch_bounds__(256, 6) k_ring_detect4(DevBuffers buf, DevPara
   // compaction of the gate survivors into the two work lists (one shared counter bump per warp and list)
   {
     const int cx = __popc(nx_mask), cz = __popc(nz_mask);
-    int px = cx, pz = cz;                                 // inclusive warp scans of the per-thread counts
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int ax = __shfl_up_sync(0xffffffffu, px, o), az = __shfl_up_sync(0xffffffffu, pz, o);
-      if (lane_id() >= o) { px += ax; pz += az; }
-    }
+    int pc[2] = {cx, cz};                                 // inclusive warp scans of the per-thread counts
+    warp_inclusive_sum(pc);
+    const int px = pc[0], pz = pc[1];
     int wx = 0, wz = 0;
     if (lane_id() == 31) { if (px) wx = atomicAdd(&s_nx, px); if (pz) wz = atomicAdd(&s_nz, pz); }
     wx = __shfl_sync(0xffffffffu, wx, 31); wz = __shfl_sync(0xffffffffu, wz, 31);
@@ -1829,10 +1859,9 @@ __device__ __forceinline__ void markers_pass(const uint4* __restrict__ list, con
       for (int u = 0; u < 4; u++) { const int sg = seg0 + u * nwarps * 32 + lane; cpre[u] = sg < nseg ? cnt[sg] : 0; }
     }
     const int c = (sw & 3) == 0 ? cpre[0] : (sw & 3) == 1 ? cpre[1] : (sw & 3) == 2 ? cpre[2] : cpre[3];
-    int inc = c;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const int v = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += v; }
-    const int excl = inc - c, total = __shfl_sync(0xffffffffu, inc, 31);
+    int inc[1] = {c};
+    warp_inclusive_sum(inc);
+    const int excl = inc[0] - c, total = __shfl_sync(0xffffffffu, inc[0], 31);
     for (int e0 = 0; e0 < total; e0 += 128) {
       uint4 ent[4];
       bool ok[4];
@@ -1866,21 +1895,16 @@ __device__ __forceinline__ void markers_pass(const uint4* __restrict__ list, con
 }
 // The per-bin winners best[] (~0 = none) compacted in bin order into markerPointsArray (:343-350), with redPoints where
 // the bin has a first non-road point cut[] (:320,348), and a zeroed tail. One bin per thread: the CTA has at least
-// kDegBins threads, and s_wsum one entry per warp.
+// kDegBins threads.
 template <bool REF>
 __device__ __forceinline__ void write_vertices(const DevBuffers& buf, int b, int S, const unsigned long long* best,
-                                               const unsigned long long* cut, int* s_wsum) {
+                                               const unsigned long long* cut) {
   ScanOut& out = buf.out[b];
-  const int i = threadIdx.x, nwarps = blockDim.x >> 5;
+  const int i = threadIdx.x;
   const bool has = i < kDegBins && best[i] != ~0ull;
-  const unsigned bal = __ballot_sync(0xffffffffu, has);
-  const int warp = i >> 5, lane = lane_id();
-  if (lane == 0) s_wsum[warp] = __popc(bal);
-  __syncthreads();
-  const int c = lane < nwarps ? s_wsum[lane] : 0;      // at most 32 warps: lane w reads warp w's count
-  const int off = __reduce_add_sync(0xffffffffu, lane < warp ? c : 0), total = __reduce_add_sync(0xffffffffu, c);
+  int total;
+  const int slot = CtaGroup::count(has, &total);
   if (has) {
-    const int slot = off + __popc(bal & ((1u << lane) - 1u));
     int p = (int)(best[i] & 0xffffffull);               // input index of the winner (REF: its emission position)
     if (REF) p = buf.order[(size_t)b * point_slice(S) + p];
     const float4 q = buf.in[(size_t)b * point_slice(S) + p];
@@ -1896,7 +1920,6 @@ __global__ void __launch_bounds__(kMark1Threads) k_markers1(DevBuffers buf, int 
   const ScanTab& tab = buf.tab[b];
   __shared__ unsigned long long s_cut[kDegBins], s_best[kDegBins];
   __shared__ unsigned s_dmax[kDegBins];
-  __shared__ int s_wsum[kMark1Threads / 32];
   const int tid = threadIdx.x;
   for (int t = tid; t < kDegBins; t += kMark1Threads) { s_cut[t] = tab.cutbest[t]; s_dmax[t] = 0u; s_best[t] = ~0ull; }
   __syncthreads();
@@ -1908,7 +1931,7 @@ __global__ void __launch_bounds__(kMark1Threads) k_markers1(DevBuffers buf, int 
   __syncthreads();
   markers_pass<2>(list, cnt, nseg, s_cut, s_dmax, s_best);
   __syncthreads();
-  write_vertices<REF>(buf, b, S, s_best, s_cut, s_wsum);
+  write_vertices<REF>(buf, b, S, s_best, s_cut);
 }
 
 // The same search for LARGE scans (hundreds of thousands of road points want more than one CTA): a grid of CTAs per scan,
@@ -1943,8 +1966,7 @@ template <bool REF>
 __global__ void __launch_bounds__(384) k_verts(DevBuffers buf, int S) {
   const int b = blockIdx.x;
   const ScanTab& tab = buf.tab[b];
-  __shared__ int s_wsum[12];
-  write_vertices<REF>(buf, b, S, tab.best, tab.cutbest, s_wsum);
+  write_vertices<REF>(buf, b, S, tab.best, tab.cutbest);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -1982,7 +2004,7 @@ __global__ void __launch_bounds__(kSortThreads) k_sort_rings(DevBuffers buf, int
     unsigned* s_cnt = s_az + kRingFast;                               // [kRingBins] bin counts, then exclusive starts
     unsigned short* s_rank = reinterpret_cast<unsigned short*>(s_cnt + kRingBins);   // [kRingFast] arrival rank inside the bin
     unsigned short* s_slot = s_rank + kRingFast;                      // [kRingFast] ring position by sorted position
-    __shared__ unsigned s_lo, s_hi, s_over, s_wsum[kSortThreads / 32];
+    __shared__ unsigned s_lo, s_hi, s_over;
     if (tid == 0) { s_lo = 0xffffffffu; s_hi = 0u; s_over = 0u; }
     for (int t = tid; t < kRingBins; t += kSortThreads) s_cnt[t] = 0u;
     __syncthreads();
@@ -2015,21 +2037,15 @@ __global__ void __launch_bounds__(kSortThreads) k_sort_rings(DevBuffers buf, int
     };
     for (int t = tid; t < n; t += kSortThreads) s_rank[t] = (unsigned short)atomicAdd(&s_cnt[bin_of(s_az[t])], 1u);
     __syncthreads();
-    {   // exclusive scan over the bins: consecutive bins per thread, warp scan, warp totals
+    {   // exclusive scan over the bins: consecutive bins per thread, then the CTA-wide scan of the threads' sums
       constexpr int PER = kRingBins / kSortThreads;
-      unsigned v[PER], sum = 0, mx = 0;
+      unsigned v[PER], run[1] = {0}, all[1], mx = 0;
 #pragma unroll
-      for (int j = 0; j < PER; j++) { v[j] = s_cnt[tid * PER + j]; sum += v[j]; mx = max(mx, v[j]); }
+      for (int j = 0; j < PER; j++) { v[j] = s_cnt[tid * PER + j]; run[0] += v[j]; mx = max(mx, v[j]); }
       if (mx > (unsigned)kBinCap) s_over = 1u;
-      unsigned inc = sum;
+      CtaGroup::exclusive_sum(run, all);
 #pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { const unsigned y = __shfl_up_sync(0xffffffffu, inc, o); if (lane_id() >= o) inc += y; }
-      if (lane_id() == 31) s_wsum[tid >> 5] = inc;
-      __syncthreads();
-      unsigned run = inc - sum;
-      for (int w = 0; w < (tid >> 5); w++) run += s_wsum[w];
-#pragma unroll
-      for (int j = 0; j < PER; j++) { s_cnt[tid * PER + j] = run; run += v[j]; }
+      for (int j = 0; j < PER; j++) { s_cnt[tid * PER + j] = run[0]; run[0] += v[j]; }
     }
     __syncthreads();
     if (!s_over) {
@@ -2091,31 +2107,6 @@ __global__ void __launch_bounds__(kSortThreads) k_sort_rings(DevBuffers buf, int
 // ring's segment of `order` and the emission positions of its points. The work arrays (five words per point) sit in
 // shared memory up to kLomutoSmemPts points, else in the ring's own 16-byte segment of sortbuf plus its slots of
 // roadlist, which k_label only fills afterwards.
-struct CtaLomuto : CtaGroup {
-  static __device__ __forceinline__ int count(bool p, int* total) {
-    __shared__ int s_w[32];
-    const unsigned bal = __ballot_sync(0xffffffffu, p);
-    const int lane = lane_id(), w = threadIdx.x >> 5, nw = blockDim.x >> 5;
-    if (lane == 0) s_w[w] = __popc(bal);
-    __syncthreads();
-    int before = 0, tot = 0;
-    for (int i = 0; i < nw; i++) { const int c = s_w[i]; tot += c; before += i < w ? c : 0; }
-    __syncthreads();
-    *total = tot;
-    return before + __popc(bal & ((1u << lane) - 1u));
-  }
-  static __device__ __forceinline__ int min(int v) {
-    __shared__ int s_m;
-    v = __reduce_min_sync(0xffffffffu, v);
-    if (threadIdx.x == 0) s_m = 0x7fffffff;
-    __syncthreads();
-    if (lane_id() == 0) atomicMin(&s_m, v);
-    __syncthreads();
-    const int r = s_m;
-    __syncthreads();
-    return r;
-  }
-};
 constexpr int kLomutoThreads = 512;
 constexpr int kLomutoSmemPts = 4096;
 constexpr size_t kLomutoSmem = (size_t)5 * kLomutoSmemPts * sizeof(unsigned);   // 80 KB
@@ -2141,7 +2132,7 @@ __global__ void __launch_bounds__(kLomutoThreads) k_lomuto_rings(DevBuffers buf,
   LomutoArrays a;
   a.az = w; a.rk = w + n; a.s0 = w + 2 * n; a.s1 = w + 3 * n;
   a.s2 = smem ? s_lw + 4 * n : reinterpret_cast<unsigned*>(buf.roadlist + g0);
-  lomuto_ring<CtaLomuto>(a, n, sh);
+  lomuto_ring<CtaGroup>(a, n, sh);
   for (int p = threadIdx.x; p < n; p += blockDim.x) {
     const int idx = (int)buf.baz[g0 + a.s0[p]].y;
     buf.order[g0 + p] = idx;
@@ -2181,19 +2172,6 @@ __device__ __forceinline__ void pack_flags(const DevBuffers& buf, const ScanOut&
   if (e < out.n_order) { *idx = buf.order[e]; const int lab = buf.label[*idx]; *road = lab == 1; *curb = lab == 2; }
   if (e < out.n_in) *roi = buf.label[e] >= 0;
 }
-// exclusive rank of `flag` among the CTA's 256 threads (thread order) and the CTA total; all threads must call
-__device__ __forceinline__ int cta_rank(bool flag, int* s_w /* [8] */, int* total) {
-  const unsigned bal = __ballot_sync(0xffffffffu, flag);
-  const int w = threadIdx.x >> 5;
-  __syncthreads();                                                       // s_w free again
-  if (lane_id() == 0) s_w[w] = __popc(bal);
-  __syncthreads();
-  int before = 0, all = 0;
-#pragma unroll
-  for (int j = 0; j < 8; j++) { const int c = s_w[j]; all += c; if (j < w) before += c; }
-  *total = all;
-  return before + __popc(bal & ((1u << lane_id()) - 1u));
-}
 __global__ void __launch_bounds__(256) k_pack_count(DevBuffers buf, int* __restrict__ cnt, int tiles) {
   __shared__ int s_c[3];
   const ScanOut& out = buf.out[0];
@@ -2212,34 +2190,16 @@ __global__ void __launch_bounds__(256) k_pack_count(DevBuffers buf, int* __restr
 }
 // one CTA: exclusive scan of the three per-tile count rows in place; tot[0..3] = road, curb, roi, road_probably counts
 __global__ void __launch_bounds__(1024) k_pack_scan(DevBuffers buf, int* __restrict__ cnt, int tiles, int* __restrict__ tot) {
-  __shared__ int s_w[32];
-  __shared__ int s_carry;
   for (int row = 0; row < 3; row++) {
-    if (threadIdx.x == 0) s_carry = 0;
-    __syncthreads();
+    int carry = 0;                                                       // tiles of the earlier rounds
     for (int t0 = 0; t0 < tiles; t0 += 1024) {
       const int t = t0 + threadIdx.x;
-      const int v = t < tiles ? cnt[row * tiles + t] : 0;
-      int x = v;
-#pragma unroll
-      for (int d = 1; d < 32; d <<= 1) { const int y = __shfl_up_sync(0xffffffffu, x, d); if (lane_id() >= d) x += y; }
-      if (lane_id() == 31) s_w[threadIdx.x >> 5] = x;
-      __syncthreads();
-      if (threadIdx.x < 32) {
-        int wv = s_w[threadIdx.x];
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) { const int y = __shfl_up_sync(0xffffffffu, wv, d); if (lane_id() >= d) wv += y; }
-        s_w[threadIdx.x] = wv;
-      }
-      __syncthreads();
-      const int carry = s_carry, wbase = (threadIdx.x >> 5) ? s_w[(threadIdx.x >> 5) - 1] : 0;
-      if (t < tiles) cnt[row * tiles + t] = carry + wbase + x - v;
-      __syncthreads();
-      if (threadIdx.x == 0) s_carry = carry + s_w[31];
-      __syncthreads();
+      int x[1] = {t < tiles ? cnt[row * tiles + t] : 0}, all[1];
+      CtaGroup::exclusive_sum(x, all);
+      if (t < tiles) cnt[row * tiles + t] = carry + x[0];
+      carry += all[0];
     }
-    if (threadIdx.x == 0) tot[row] = s_carry;
-    __syncthreads();
+    if (threadIdx.x == 0) tot[row] = carry;
   }
   if (threadIdx.x == 0) {
     const ScanOut& out = buf.out[0];
@@ -2252,7 +2212,6 @@ __device__ __forceinline__ void pack_record(float4* __restrict__ dst, int pos, c
 }
 __global__ void __launch_bounds__(256) k_pack_write(DevBuffers buf, const int* __restrict__ cnt, int tiles, const int* __restrict__ tot,
                                                      float4* __restrict__ road_curb, float4* __restrict__ roi_dst, float4* __restrict__ prob) {
-  __shared__ int s_w[8];
   const ScanOut& out = buf.out[0];
   int road_pos = cnt[blockIdx.x], curb_pos = tot[0] + cnt[tiles + blockIdx.x], roi_pos = cnt[2 * tiles + blockIdx.x];
   const int rs10 = out.ring_start[10], rs11 = out.n_roi < 30 ? rs10 : out.ring_start[11];
@@ -2261,13 +2220,13 @@ __global__ void __launch_bounds__(256) k_pack_write(DevBuffers buf, const int* _
     bool road, curb, roi; int idx;
     pack_flags(buf, out, e, &road, &curb, &roi, &idx);
     int total;
-    const int r0 = cta_rank(road, s_w, &total);
+    const int r0 = CtaGroup::count(road, &total);
     if (road) pack_record(road_curb, road_pos + r0, buf.in[idx]);
     road_pos += total;
-    const int r1 = cta_rank(curb, s_w, &total);
+    const int r1 = CtaGroup::count(curb, &total);
     if (curb) pack_record(road_curb, curb_pos + r1, buf.in[idx]);
     curb_pos += total;
-    const int r2 = cta_rank(roi, s_w, &total);
+    const int r2 = CtaGroup::count(roi, &total);
     if (roi) pack_record(roi_dst, roi_pos + r2, buf.in[e]);
     roi_pos += total;
     if (e >= rs10 && e < rs11) pack_record(prob, e - rs10, buf.in[idx]);

@@ -17,7 +17,7 @@
 // less + [pivot] + window[1:] + [window[0]]. (Stored by scan position, entry f + h sits at low + lr, lr = elements < p in
 // [low, j), and the window's front at the pivot's final position.)
 //
-// The same template runs on the device (CtaLomuto: one CTA) and sequentially on the host (SeqLomuto), where
+// The same template runs on the device (CtaGroup: one CTA) and sequentially on the host (SeqLomuto), where
 // tests/kat/lomuto_check.cpp compares it with the restated quicksort of the CPU oracle.
 #pragma once
 #include <stdint.h>
