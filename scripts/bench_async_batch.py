@@ -4,8 +4,9 @@ worker did before it kept two batches in flight) against a urf_enqueue_batch / u
 flight (what it does now). Per shape: scans/s of both loops, alternated `--repeats` times (medians), and the device's idle
 time between consecutive batches = (wall time - the sum of the batches' kernel spans, CUDA events) / batches. The labels
 of both loops are compared byte for byte.
-With --old-lib DIR (a liburf_b200.so of another build): tools/mq_bench (urf_mq at one GPU, urf_mq_next_batch on int8
-slots, the settings of scripts/bench_mq_batch.py) alternately against that library and this tree's, medians.
+With --old-lib DIR (a liburf_b200.so of another build): tools/mq_bench (urf_mq at one GPU, the settings of
+scripts/bench_mq_batch.py: urf_mq_next_view on int32 slots and urf_mq_next_batch on int8 slots) alternately against that
+library and this tree's, medians and every run.
 usage: python scripts/bench_async_batch.py [--shapes C2,C4] [--batch 16] [--steps 100] [--repeats 3] [--old-lib DIR]"""
 import argparse, ctypes as C, json, os, statistics, subprocess, sys, tempfile, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -119,15 +120,16 @@ if args.old_lib:
         for k in range(K):
             f.write(np.ascontiguousarray(make_scan("C4", 500 + k), np.float32).tobytes())
     libs = {"old": os.path.abspath(args.old_lib), "new": os.path.join(ROOT, "urban_road_filter_b200")}
-    runs = {k: [] for k in libs}
-    for r in range(args.repeats):
-        for k in (("old", "new") if r % 2 == 0 else ("new", "old")):
-            out = subprocess.run([exe, path, str(n), str(K), "1", "4", str(args.mq_scans), "24", "16", "1", str(sh.channels), str(sh.interval),
-                                  "3", "64"], check=True, capture_output=True, text=True,
-                                 env={**os.environ, "LD_LIBRARY_PATH": libs[k]}).stdout
-            runs[k].append(json.loads(out.strip().splitlines()[-1])["scans_per_sec"])
-    med = {k: statistics.median(v) for k, v in runs.items()}
-    print(json.dumps({"mq_1gpu_C4_next_batch_int8": {k: {"scans_per_sec": round(med[k], 1), "runs": [round(x, 1) for x in runs[k]]}
-                                                       for k in libs}}), flush=True)
+    for mode, name in ((2, "next_view_int32"), (3, "next_batch_int8")):      # tools/mq_bench modes
+        runs = {k: [] for k in libs}
+        for r in range(args.repeats):
+            for k in (("old", "new") if r % 2 == 0 else ("new", "old")):
+                out = subprocess.run([exe, path, str(n), str(K), "1", "4", str(args.mq_scans), "24", "16", "1", str(sh.channels),
+                                      str(sh.interval), str(mode), "64"], check=True, capture_output=True, text=True,
+                                     env={**os.environ, "LD_LIBRARY_PATH": libs[k]}).stdout
+                runs[k].append(json.loads(out.strip().splitlines()[-1])["scans_per_sec"])
+        med = {k: statistics.median(v) for k, v in runs.items()}
+        print(json.dumps({"mq_1gpu_C4_" + name: {k: {"scans_per_sec": round(med[k], 1), "runs": [round(x, 1) for x in runs[k]]}
+                                                 for k in libs}}), flush=True)
     os.remove(path)
     os.rmdir(tmp)

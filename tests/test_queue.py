@@ -69,6 +69,7 @@ def test_queue_orders_and_batches():
     st = q.stats()
     assert (st["submitted"], st["processed"], st["delivered"], st["dropped"], st["pending"]) == (50, 50, 50, 0, 0)
     assert 1 <= st["largest_batch"] <= 4 and sum(fb.batches) == 50 and max(fb.batches) <= 4
+    assert st["most_in_flight"] == 1                              # a synchronous stand-in: one batch call at a time
     q.destroy()
 
 

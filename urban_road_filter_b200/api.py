@@ -191,10 +191,10 @@ class BatchHandle:
     batch's copies run asynchronously; a copy from or to pageable memory makes the enqueue wait for it. Allocating
     page-locked memory can wait for the device: build handles before enqueueing if batches are to overlap. A handle can be
     enqueued again once it is finished (collect copies the results out); its page-locked memory is freed by free() or when
-    the handle is dropped."""
+    the handle is dropped. want_label=False: no label buffers (a call whose caller does not read the labels)."""
 
     def __init__(self, inputs, ns, want_ring: bool, want_order: bool, label8: bool, step: int = 0, offs=(0, 4, 8, -1),
-                 pinned: bool = False):
+                 pinned: bool = False, want_label: bool = True):
         B = len(inputs)
         self.lib = load_library()
         self.step, self.offs, self.pinned = step, tuple(offs), pinned
@@ -208,11 +208,13 @@ class BatchHandle:
         self.results = None
         for b, n in enumerate(ns):
             m = max(n, 1)
-            lab = self._array(np.full(m, -1, np.int8 if label8 else np.int32))
+            lab = self._array(np.full(m, -1, np.int8 if label8 else np.int32)) if want_label else None
             ring = self._array(np.full(m, -1, np.int32)) if want_ring else None
             order = self._array(np.zeros(m, np.int32)) if want_order else None
             rs = self._array(np.zeros(URF_MAX_CHANNELS + 1, np.int32))
-            if label8:
+            if lab is None:
+                pass
+            elif label8:
                 self.l8[b] = lab.ctypes.data
             else:
                 self.res[b].label = lab.ctypes.data_as(C.POINTER(C.c_int32))
@@ -253,10 +255,11 @@ class BatchHandle:
         out = []
         for b, n in enumerate(self.ns):
             lab, ring, order, rs = self.bufs[b]
-            lab = lab[:n].astype(np.int32) if self.l8 is not None else lab[:n]
+            if lab is not None:
+                lab = lab[:n].astype(np.int32) if self.l8 is not None else lab[:n]
             ring = None if ring is None else ring[:n]
             if self.pinned:
-                lab = lab.copy()
+                lab = None if lab is None else lab.copy()
                 ring = None if ring is None else ring.copy()
             out.append(_scan_result(self.res[b], lab, ring, order, rs))
         self.results = out
@@ -382,42 +385,31 @@ class Detector:
         hb.collect()
         return hb
 
+    def _one_record_scan(self, data, n_points: int, point_step: int, offs, want_ring: bool, want_order: bool, want_label: bool) -> BatchHandle:
+        """Input and result buffers of one scan given as raw PointCloud2 bytes, of which n_points records count."""
+        raw = np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray)) else np.ascontiguousarray(data).view(np.uint8).reshape(-1)
+        return BatchHandle([raw], [n_points], want_ring, want_order, False, point_step, offs, want_label=want_label)
+
     def filtered_cloud2(self, data: bytes | np.ndarray, n_points: int, point_step: int, off_x: int, off_y: int, off_z: int) -> ScanResult:
         """One scan from the raw `data` bytes of a sensor_msgs/PointCloud2 (unpacked on the device)."""
-        raw = np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray)) else np.ascontiguousarray(data).view(np.uint8).reshape(-1)
-        m = max(n_points, 1)
-        lab, ring, order = np.full(m, -1, np.int32), np.full(m, -1, np.int32), np.zeros(m, np.int32)
-        rs = np.zeros(URF_MAX_CHANNELS + 1, np.int32)
-        res = UrfResult()
-        res.label = lab.ctypes.data_as(C.POINTER(C.c_int32)); res.ring = ring.ctypes.data_as(C.POINTER(C.c_int32))
-        res.order = order.ctypes.data_as(C.POINTER(C.c_int32)); res.ring_start = rs.ctypes.data_as(C.POINTER(C.c_int32))
-        self._check(self.lib.urf_process_cloud2(self._ctx, raw.ctypes.data, n_points, point_step, off_x, off_y, off_z, C.byref(res)),
-                    "urf_process_cloud2")
-        return _scan_result(res, lab[:n_points], ring[:n_points], order, rs)
+        hb = self._one_record_scan(data, n_points, point_step, (off_x, off_y, off_z, -1), True, True, True)
+        self._check(self.lib.urf_process_cloud2(self._ctx, hb.ptrs[0], n_points, point_step, off_x, off_y, off_z, hb.res), "urf_process_cloud2")
+        return hb.collect()[0]
 
     def filtered_cloud2_packed(self, data, n_points: int, point_step: int, off_x: int, off_y: int, off_z: int,
                                off_intensity: int = -1, want_labels: bool = False):
         """One scan from raw PointCloud2 bytes; returns (ScanResult, clouds) where clouds maps "road" / "curb" / "roi" /
         "road_probably" to float32 arrays [count, 8] of 32-byte pcl::PointXYZI records packed on the device in the
         reference's emission order (include/urf.h urf_clouds). Labels / order are only fetched with want_labels."""
-        raw = np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray)) else np.ascontiguousarray(data).view(np.uint8).reshape(-1)
-        m = max(n_points, 1)
-        bufs = {k: np.empty((m, 8), np.float32) for k in ("road", "curb", "roi", "road_probably")}
+        hb = self._one_record_scan(data, n_points, point_step, (off_x, off_y, off_z, off_intensity), False, want_labels, want_labels)
+        bufs = {k: np.empty((max(n_points, 1), 8), np.float32) for k in ("road", "curb", "roi", "road_probably")}
         cl = UrfClouds()
         for k, a in bufs.items():
             setattr(cl, k, a.ctypes.data)
-        rs = np.zeros(URF_MAX_CHANNELS + 1, np.int32)
-        res = UrfResult()
-        res.ring_start = rs.ctypes.data_as(C.POINTER(C.c_int32))
-        lab = order = None
-        if want_labels:
-            lab, order = np.full(m, -1, np.int32), np.zeros(m, np.int32)
-            res.label = lab.ctypes.data_as(C.POINTER(C.c_int32)); res.order = order.ctypes.data_as(C.POINTER(C.c_int32))
-        self._check(self.lib.urf_process_cloud2_packed(self._ctx, raw.ctypes.data, n_points, point_step, off_x, off_y, off_z,
-                                                       off_intensity, C.byref(res), C.byref(cl)), "urf_process_cloud2_packed")
-        r = _scan_result(res, lab[:n_points] if want_labels else None, None, order, rs)
+        self._check(self.lib.urf_process_cloud2_packed(self._ctx, hb.ptrs[0], n_points, point_step, off_x, off_y, off_z,
+                                                       off_intensity, hb.res, C.byref(cl)), "urf_process_cloud2_packed")
         counts = dict(road=cl.n_road, curb=cl.n_curb, roi=cl.n_roi, road_probably=cl.n_road_probably)
-        return r, {k: bufs[k][: counts[k]] for k in bufs}
+        return hb.collect()[0], {k: bufs[k][: counts[k]] for k in bufs}
 
     def filtered(self, cloud, **kw) -> ScanResult:
         """One Detector::filtered() call."""
@@ -483,153 +475,33 @@ class _BatchBuffers:
         return out
 
 
-def _next_batch(fn, handle, bufs: "_BatchBuffers | None", max_results: int, timeout_ms: int, label8: bool, copy: bool, where: str):
-    if max_results < 1:
-        raise ValueError("max_results must be >= 1")
-    if bufs is None or bufs.cap < max_results:
-        bufs = _BatchBuffers(max_results)
-    k = fn(handle, max_results, bufs.tags, bufs.rcs, bufs.outs, bufs.views, timeout_ms)
-    if k in (URF_ERR_TIMEOUT, URF_ERR_CLOSED):
-        return bufs, []
-    if k < 0:
-        raise UrfError(k, where)
-    return bufs, bufs.results(k, label8, copy)
+class _StreamQueue:
+    """What ScanQueue and MultiGpuQueue share: the library handle `_h`, the arrays of by-reference submits, the reused
+    batch buffers, and submit / next / next_batch / close / destroy, written against the library functions
+    `_PREFIX` + name (urf_queue_* or urf_mq_*), which have the same arguments in both families."""
+    _PREFIX = ""
 
-
-class MultiGpuQueue:
-    """One ingest stream over several GPUs (include/urf.h urf_mq, BASELINE config 4): a context + streaming queue per device,
-    every scan goes to the device with the fewest scans in flight, results come back in submission order. Any number of
-    producer threads, one consumer. `by_reference` submits hand the array to the library without a copy: keep it alive and
-    unchanged until its result has come back. label8: int8 label slots on every device (see ScanQueue)."""
-
-    def __init__(self, devices, max_points: int, slots_per_device: int = 8, max_batch: int = 4, params: UrfParams | None = None,
-                 process_fn=None, label8: bool = False):
+    def __init__(self, max_points: int, label8: bool):
         self.lib = load_library()
-        self._m = C.c_void_p()
+        self._h = C.c_void_p()
         self.max_points = max_points
         self.label8 = label8
-        self._cb = None
-        self._bufs = None
-        if process_fn is not None:                      # tests: stand-in devices, no GPU
-            self._cb = QUEUE_PROCESS_FN(process_fn)
-            create = self.lib.urf_mq_create_with_label8 if label8 else self.lib.urf_mq_create_with
-            rc = create(C.byref(self._m), self._cb, None, len(devices), max_points, slots_per_device, max_batch)
-        else:
-            dv = (C.c_int * len(devices))(*devices)
-            create = self.lib.urf_mq_create_label8 if label8 else self.lib.urf_mq_create
-            rc = create(C.byref(self._m), dv, len(devices), max_points, slots_per_device, max_batch,
-                        C.byref(params) if params is not None else None)
-        if rc != URF_OK:
-            raise UrfError(rc, "urf_mq_create", self.lib.urf_last_cuda_error(None).decode())
-        self._keep = {}
-
-    def set_params(self, prm: UrfParams):
-        rc = self.lib.urf_mq_set_params(self._m, C.byref(prm))
-        if rc != URF_OK:
-            raise UrfError(rc, "urf_mq_set_params")
-
-    def set_tie_order(self, mode: str):
-        """Detector.set_tie_order on every device; like set_params, only while nothing is in flight."""
-        if mode not in TIE_ORDERS:
-            raise ValueError(f"tie order {mode!r}: expected one of {sorted(TIE_ORDERS)}")
-        rc = self.lib.urf_mq_set_tie_order(self._m, TIE_ORDERS[mode])
-        if rc != URF_OK:
-            raise UrfError(rc, "urf_mq_set_tie_order")
-
-    def submit(self, cloud: np.ndarray, tag: int = 0, timeout_ms: int = -1, by_reference: bool = False) -> int:
-        pts = np.ascontiguousarray(cloud, np.float32)
-        if by_reference:
-            self._keep[tag] = pts
-            rc = self.lib.urf_mq_submit_ref(self._m, pts.ctypes.data, pts.shape[0], tag, timeout_ms)
-        else:
-            rc = self.lib.urf_mq_submit(self._m, pts.ctypes.data, pts.shape[0], tag, timeout_ms)
-        if rc not in (URF_OK, URF_ERR_TIMEOUT, URF_ERR_CLOSED):
-            raise UrfError(rc, "urf_mq_submit")
-        return rc
-
-    def next(self, timeout_ms: int = -1):
-        """(tag, ScanResult) of the oldest scan, or None on timeout / when the closed queue is drained."""
-        lab = np.full(self.max_points, -1, np.int32)
-        res = UrfResult()
-        res.label = lab.ctypes.data_as(C.POINTER(C.c_int32))
-        tag = C.c_uint64()
-        rc = self.lib.urf_mq_next(self._m, C.byref(tag), C.byref(res), timeout_ms)
-        if rc in (URF_ERR_TIMEOUT, URF_ERR_CLOSED):
-            return None
-        if rc != URF_OK:
-            raise UrfError(rc, "urf_mq_next")
-        self._keep.pop(tag.value, None)
-        return tag.value, _scan_result(res, lab[: res.n_in].copy())
-
-    def next_batch(self, max_results: int, timeout_ms: int = -1, copy: bool = False) -> list:
-        """[(tag, ScanResult)] of the run of finished scans at the front of the global order (urf_mq_next_batch), at most
-        max_results; [] on timeout / when the closed queue is drained. Labels are views of the lent slots (int8 with
-        label8), valid until the next next* call, unless `copy`. A scan whose batch failed has status < 0 and label None."""
-        self._bufs, out = _next_batch(self.lib.urf_mq_next_batch, self._m, self._bufs, max_results, timeout_ms, self.label8, copy,
-                                      "urf_mq_next_batch")
-        for t, _ in out:
-            self._keep.pop(t, None)
-        return out
-
-    def stats(self) -> dict:
-        st = UrfMqStats()
-        self.lib.urf_mq_get_stats(self._m, C.byref(st))
-        n = st.n_devices
-        return dict(n_devices=n, pending=st.pending, submitted=list(st.submitted[:n]), delivered=list(st.delivered[:n]),
-                    batches=list(st.batches[:n]), largest_batch=list(st.largest_batch[:n]))
-
-    def close(self):
-        if self._m:
-            self.lib.urf_mq_close(self._m)
-
-    def destroy(self):
-        if self._m:
-            self.lib.urf_mq_destroy(self._m)
-            self._m = C.c_void_p()
-
-
-class ScanQueue:
-    """Streaming ingest (include/urf.h urf_queue, SURVEY.md §8 f4): producers `submit` scans from any thread, one worker
-    thread batches whatever is pending through the detector, `next` returns results in submission order and `next_batch`
-    every result that is ready at once. With `process_fn` (a Python callable with urf_process_batch's arguments) the queue
-    runs without a GPU — tests only; with `enqueue_fn` and `finish_fn` instead (urf_enqueue_batch's arguments / none) it
-    runs the real queue's two-batches-in-flight schedule around them. label8: int8 label slots (URF_QUEUE_LABEL8) — a
-    quarter of the label traffic and memory; `next` still returns int32 labels, `next_batch` int8 ones."""
-
-    def __init__(self, detector: "Detector | None", max_points: int, slots: int = 8, max_batch: int = 4,
-                 policy: int = URF_QUEUE_BLOCK, process_fn=None, label8: bool = False, enqueue_fn=None, finish_fn=None):
-        self.lib = load_library()
-        self._q = C.c_void_p()
-        self.max_points = max_points
-        self.label8 = label8
-        if label8:
-            policy |= URF_QUEUE_LABEL8
-        self._cb = None
+        self._cb = None                   # ctypes callbacks of a stand-in, kept alive with the queue
         self._bufs = None
         self._keep = {}                   # arrays of by-reference submits, until their results come back
-        if enqueue_fn is not None:
-            self._cb = (QUEUE_PROCESS_FN(enqueue_fn), QUEUE_FINISH_FN(lambda user: finish_fn()))
-            rc = self.lib.urf_queue_create_with_async(C.byref(self._q), *self._cb, None, max_points, slots, max_batch, policy)
-        elif process_fn is not None:
-            self._cb = QUEUE_PROCESS_FN(process_fn)
-            rc = self.lib.urf_queue_create_with(C.byref(self._q), self._cb, None, max_points, slots, max_batch, policy)
-        else:
-            assert detector is not None and detector.max_batch >= max_batch and detector.max_points >= max_points
-            self._det = detector          # keeps the ctx alive; nobody else may use it while the queue exists
-            rc = self.lib.urf_queue_create(C.byref(self._q), detector._ctx, max_points, slots, max_batch, policy)
-        if rc != URF_OK:
-            raise UrfError(rc, "urf_queue_create")
+
+    def _call(self, name: str, *args) -> int:
+        return getattr(self.lib, self._PREFIX + name)(self._h, *args)
 
     def submit(self, cloud: np.ndarray, tag: int = 0, timeout_ms: int = -1, by_reference: bool = False) -> int:
         """Returns URF_OK, URF_ERR_TIMEOUT or URF_ERR_CLOSED; raises on anything else. by_reference: no copy
-        (urf_queue_submit_ref): keep the array alive and unchanged until its result has come back."""
+        (urf_queue_submit_ref / urf_mq_submit_ref): keep the array alive and unchanged until its result has come back."""
         pts = np.ascontiguousarray(cloud, np.float32)
         if by_reference:
             self._keep[tag] = pts
-        submit = self.lib.urf_queue_submit_ref if by_reference else self.lib.urf_queue_submit
-        rc = submit(self._q, pts.ctypes.data, pts.shape[0], tag, timeout_ms)
+        rc = self._call("submit_ref" if by_reference else "submit", pts.ctypes.data, pts.shape[0], tag, timeout_ms)
         if rc not in (URF_OK, URF_ERR_TIMEOUT, URF_ERR_CLOSED):
-            raise UrfError(rc, "urf_queue_submit")
+            raise UrfError(rc, self._PREFIX + "submit")
         return rc
 
     def next(self, timeout_ms: int = -1):
@@ -638,38 +510,121 @@ class ScanQueue:
         res = UrfResult()
         res.label = lab.ctypes.data_as(C.POINTER(C.c_int32))
         tag = C.c_uint64()
-        rc = self.lib.urf_queue_next(self._q, C.byref(tag), C.byref(res), timeout_ms)
+        rc = self._call("next", C.byref(tag), C.byref(res), timeout_ms)
         if rc in (URF_ERR_TIMEOUT, URF_ERR_CLOSED):
             return None
         if rc != URF_OK:
-            raise UrfError(rc, "urf_queue_next")
+            raise UrfError(rc, self._PREFIX + "next")
         self._keep.pop(tag.value, None)
-        return int(tag.value), _scan_result(res, lab[: res.n_in].copy())
+        return tag.value, _scan_result(res, lab[: res.n_in].copy())
 
     def next_batch(self, max_results: int, timeout_ms: int = -1, copy: bool = False) -> list:
-        """[(tag, ScanResult)] of the run of finished scans that starts with the oldest one (urf_queue_next_batch), at most
-        max_results; [] on timeout / when the closed queue is drained. Labels are views of the lent slots (int8 with
-        label8), valid until the next next* call, unless `copy`. A scan whose batch failed has status < 0 and label None."""
-        self._bufs, out = _next_batch(self.lib.urf_queue_next_batch, self._q, self._bufs, max_results, timeout_ms, self.label8, copy,
-                                      "urf_queue_next_batch")
+        """[(tag, ScanResult)] of the run of finished scans that starts with the oldest one (urf_queue_next_batch /
+        urf_mq_next_batch), at most max_results; [] on timeout / when the closed queue is drained. Labels are views of the
+        lent slots (int8 with label8), valid until the next next* call, unless `copy`. A scan whose batch failed has
+        status < 0 and label None."""
+        if max_results < 1:
+            raise ValueError("max_results must be >= 1")
+        if self._bufs is None or self._bufs.cap < max_results:
+            self._bufs = _BatchBuffers(max_results)
+        b = self._bufs
+        k = self._call("next_batch", max_results, b.tags, b.rcs, b.outs, b.views, timeout_ms)
+        if k in (URF_ERR_TIMEOUT, URF_ERR_CLOSED):
+            return []
+        if k < 0:
+            raise UrfError(k, self._PREFIX + "next_batch")
+        out = b.results(k, self.label8, copy)
         for t, _ in out:
             self._keep.pop(t, None)
         return out
 
+    def close(self):
+        if self._h:
+            self._call("close")
+
+    def destroy(self):
+        if self._h:
+            self._call("destroy")
+            self._h = C.c_void_p()
+
+
+class MultiGpuQueue(_StreamQueue):
+    """One ingest stream over several GPUs (include/urf.h urf_mq, BASELINE config 4): a context + streaming queue per device,
+    every scan goes to the device with the fewest scans in flight, results come back in submission order. Any number of
+    producer threads, one consumer. `by_reference` submits hand the array to the library without a copy: keep it alive and
+    unchanged until its result has come back. label8: int8 label slots on every device (see ScanQueue)."""
+    _PREFIX = "urf_mq_"
+    _m = property(lambda self: self._h)      # the library handle, under the name this class has always had for it
+
+    def __init__(self, devices, max_points: int, slots_per_device: int = 8, max_batch: int = 4, params: UrfParams | None = None,
+                 process_fn=None, label8: bool = False):
+        super().__init__(max_points, label8)
+        if process_fn is not None:                      # tests: stand-in devices, no GPU
+            self._cb = QUEUE_PROCESS_FN(process_fn)
+            create = self.lib.urf_mq_create_with_label8 if label8 else self.lib.urf_mq_create_with
+            rc = create(C.byref(self._h), self._cb, None, len(devices), max_points, slots_per_device, max_batch)
+        else:
+            dv = (C.c_int * len(devices))(*devices)
+            create = self.lib.urf_mq_create_label8 if label8 else self.lib.urf_mq_create
+            rc = create(C.byref(self._h), dv, len(devices), max_points, slots_per_device, max_batch,
+                        C.byref(params) if params is not None else None)
+        if rc != URF_OK:
+            raise UrfError(rc, "urf_mq_create", self.lib.urf_last_cuda_error(None).decode())
+
+    def set_params(self, prm: UrfParams):
+        rc = self._call("set_params", C.byref(prm))
+        if rc != URF_OK:
+            raise UrfError(rc, "urf_mq_set_params")
+
+    def set_tie_order(self, mode: str):
+        """Detector.set_tie_order on every device; like set_params, only while nothing is in flight."""
+        if mode not in TIE_ORDERS:
+            raise ValueError(f"tie order {mode!r}: expected one of {sorted(TIE_ORDERS)}")
+        rc = self._call("set_tie_order", TIE_ORDERS[mode])
+        if rc != URF_OK:
+            raise UrfError(rc, "urf_mq_set_tie_order")
+
+    def stats(self) -> dict:
+        st = UrfMqStats()
+        self._call("get_stats", C.byref(st))
+        n = st.n_devices
+        return dict(n_devices=n, pending=st.pending, submitted=list(st.submitted[:n]), delivered=list(st.delivered[:n]),
+                    batches=list(st.batches[:n]), largest_batch=list(st.largest_batch[:n]))
+
+
+class ScanQueue(_StreamQueue):
+    """Streaming ingest (include/urf.h urf_queue, SURVEY.md §8 f4): producers `submit` scans from any thread, one worker
+    thread batches whatever is pending through the detector, `next` returns results in submission order and `next_batch`
+    every result that is ready at once. With `process_fn` (a Python callable with urf_process_batch's arguments) the queue
+    runs without a GPU — tests only; with `enqueue_fn` and `finish_fn` instead (urf_enqueue_batch's arguments / none) it
+    runs the real queue's two-batches-in-flight schedule around them. label8: int8 label slots (URF_QUEUE_LABEL8) — a
+    quarter of the label traffic and memory; `next` still returns int32 labels, `next_batch` int8 ones."""
+    _PREFIX = "urf_queue_"
+    _q = property(lambda self: self._h)      # the library handle, under the name this class has always had for it
+
+    def __init__(self, detector: "Detector | None", max_points: int, slots: int = 8, max_batch: int = 4,
+                 policy: int = URF_QUEUE_BLOCK, process_fn=None, label8: bool = False, enqueue_fn=None, finish_fn=None):
+        super().__init__(max_points, label8)
+        if label8:
+            policy |= URF_QUEUE_LABEL8
+        if enqueue_fn is not None:
+            self._cb = (QUEUE_PROCESS_FN(enqueue_fn), QUEUE_FINISH_FN(lambda user: finish_fn()))
+            rc = self.lib.urf_queue_create_with_async(C.byref(self._h), *self._cb, None, max_points, slots, max_batch, policy)
+        elif process_fn is not None:
+            self._cb = QUEUE_PROCESS_FN(process_fn)
+            rc = self.lib.urf_queue_create_with(C.byref(self._h), self._cb, None, max_points, slots, max_batch, policy)
+        else:
+            assert detector is not None and detector.max_batch >= max_batch and detector.max_points >= max_points
+            self._det = detector          # keeps the ctx alive; nobody else may use it while the queue exists
+            rc = self.lib.urf_queue_create(C.byref(self._h), detector._ctx, max_points, slots, max_batch, policy)
+        if rc != URF_OK:
+            raise UrfError(rc, "urf_queue_create")
+
     def release(self):
         """Gives the slots lent by next_batch back before the next call (urf_queue_release_view)."""
-        self.lib.urf_queue_release_view(self._q)
+        self._call("release_view")
 
     def stats(self) -> dict:
         st = UrfQueueStats()
-        self.lib.urf_queue_get_stats(self._q, C.byref(st))
+        self._call("get_stats", C.byref(st))
         return {k: int(getattr(st, k)) for k, _ in UrfQueueStats._fields_}
-
-    def close(self):
-        if self._q:
-            self.lib.urf_queue_close(self._q)
-
-    def destroy(self):
-        if self._q:
-            self.lib.urf_queue_destroy(self._q)
-            self._q = C.c_void_p()

@@ -4,22 +4,22 @@
 // The reference is a single subscriber with queue depth 1 (`nh->subscribe(params::topicName, 1, &Detector::filtered, this)`,
 // lidar_segmentation.cpp:53); the demo graph feeds four LiDAR topics (config/demo1.rviz:91,121,151,181). urf_mq keeps one
 // submit/next interface in front of N devices: every device owns a context and a streaming queue (urf_queue: pinned
-// staging slots + one worker thread that batches whatever is pending through urf_process_batch); a scan goes to the device
-// with the fewest scans in flight (ties: round-robin), and results come back in the order the submissions completed.
+// staging slots + one worker thread that takes whatever is pending as one batch and keeps two batches in flight); a scan
+// goes to the device with the fewest scans in flight (ties: round-robin), and results come back in the order the
+// submissions completed.
 // Scans are independent units, so there is nothing to exchange between devices (no collective on this path).
 //
 // Ordering: urf_queue delivers each device's scans in the order their submit calls completed, so the global order only
 // has to remember WHICH device holds the next scan: a FIFO of device indices, appended after a device accepted a scan
 // (under that device's submit mutex, so that the k-th entry naming a device is the k-th scan its queue accepted).
 //
-// Batched delivery (urf_mq_next_batch) cuts the front of that FIFO at the first scan that is not done yet: every device
-// queue involved reports how many of its oldest scans are done, and then lends exactly the ones before the cut.
+// Delivery (take_front_run, behind urf_mq_next / _next_view / _next_batch) cuts the front of that FIFO at the first scan
+// that is not done yet: every device queue involved reports how many of its oldest scans are done, and then lends exactly
+// the ones before the cut.
 #include <algorithm>
 #include <cstring>
 #include <deque>
 #include <mutex>
-#include <condition_variable>
-#include <chrono>
 #include <vector>
 
 #include "../../include/urf.h"
@@ -32,7 +32,6 @@ struct urf_mq {
     urf_queue* q = nullptr;
     uint64_t submitted = 0, delivered = 0;
     int inflight = 0;                // accepted or being copied, not yet delivered
-    bool lent = false;               // consumer side only: this device's queue has slots lent out by urf_mq_next_view / _batch
     std::mutex submit_mu;            // held from the device queue's submit to the append to `order`: one device's entries
                                      // enter `order` in the order its queue accepted them (copies to DIFFERENT devices overlap)
   };
@@ -44,6 +43,11 @@ struct urf_mq {
   int submitting = 0;                // submit calls between device choice and order append
   bool closed = false;
   bool label8 = false;               // int8 label slots on every device (urf_mq_create_label8)
+  // Scratch of take_front_run. The header allows ONE consumer thread, so it needs no lock.
+  std::vector<int> ds;               // devices of the first scans in the global order (a snapshot of `order`'s front)
+  std::vector<int> want, done, used; // per device: its entries in ds / how many of them are done (-1: not asked yet) /
+                                     // how many the last call lent, which are still lent when the next call begins
+  std::vector<std::vector<int>> dst; // per device: output positions of its share, in its queue's order
 };
 
 namespace {
@@ -83,40 +87,73 @@ int submit_common(urf_mq* m, const float* xyzi, int n, uint64_t tag, int timeout
   return rc;
 }
 
-int create_real(urf_mq** out, const int* devices, int n_devices, int max_points, int slots_per_device, int max_batch,
-                const urf_params* params, int policy) {
-  if (!out || !devices || n_devices < 1 || max_points < 1 || slots_per_device < 1 || max_batch < 1) return URF_ERR_INVALID;
+// fn == NULL: a context (with `params`, if given) and a pinned queue on each of `devices`; otherwise stand-in devices
+// around fn, which gets users[j] for device j. The first device that cannot be made ends the attempt.
+int create(urf_mq** out, const int* devices, urf_queue_process_fn fn, void* const* users, int n_devices, int max_points,
+           int slots_per_device, int max_batch, const urf_params* params, int policy) {
+  if (!out || (!devices && !fn) || n_devices < 1 || max_points < 1 || slots_per_device < 1 || max_batch < 1) return URF_ERR_INVALID;
   *out = nullptr;
   urf_mq* m = new urf_mq;
   m->label8 = (policy & URF_QUEUE_LABEL8) != 0;
   for (int j = 0; j < n_devices; j++) m->dev.emplace_back();
-  int rc = URF_OK;
-  for (int j = 0; j < n_devices && rc == URF_OK; j++) {
-    urf_mq::Dev& d = m->dev[j];
-    d.device = devices[j];
-    rc = urf_create(&d.ctx, d.device, max_points, max_batch);
-    if (rc == URF_OK && params) rc = urf_set_params(d.ctx, params);
-    if (rc == URF_OK) rc = urf_queue_create(&d.q, d.ctx, max_points, slots_per_device, max_batch, policy);
-  }
-  if (rc != URF_OK) { urf_mq_destroy(m); return rc; }
-  *out = m;
-  return URF_OK;
-}
-
-int create_stand_in(urf_mq** out, urf_queue_process_fn fn, void* const* users, int n_devices, int max_points, int slots_per_device,
-                    int max_batch, int policy) {
-  if (!out || !fn || n_devices < 1) return URF_ERR_INVALID;
-  *out = nullptr;
-  urf_mq* m = new urf_mq;
-  m->label8 = (policy & URF_QUEUE_LABEL8) != 0;
-  for (int j = 0; j < n_devices; j++) m->dev.emplace_back();
+  m->want.resize(n_devices); m->done.resize(n_devices); m->used.resize(n_devices); m->dst.resize(n_devices);
   for (int j = 0; j < n_devices; j++) {
-    m->dev[j].device = j;
-    const int rc = urf_queue_create_with(&m->dev[j].q, fn, users ? users[j] : nullptr, max_points, slots_per_device, max_batch, policy);
+    urf_mq::Dev& d = m->dev[j];
+    d.device = fn ? j : devices[j];
+    int rc = URF_OK;
+    if (fn) rc = urf_queue_create_with(&d.q, fn, users ? users[j] : nullptr, max_points, slots_per_device, max_batch, policy);
+    else {
+      rc = urf_create(&d.ctx, d.device, max_points, max_batch);
+      if (rc == URF_OK && params) rc = urf_set_params(d.ctx, params);
+      if (rc == URF_OK) rc = urf_queue_create(&d.q, d.ctx, max_points, slots_per_device, max_batch, policy);
+    }
     if (rc != URF_OK) { urf_mq_destroy(m); return rc; }
   }
   *out = m;
   return URF_OK;
+}
+
+// The one delivery routine: lends the run of finished scans at the front of the global order, at most max_results of
+// them, and returns its length (>= 1), or URF_ERR_TIMEOUT (the oldest scan's entry stays at the front) / URF_ERR_CLOSED.
+// Outputs as urf_mq_next_batch.
+int take_front_run(urf_mq* m, int max_results, uint64_t* tags, int32_t* rcs, urf_result* outs, const void** label_views, int timeout_ms) {
+  const int D = (int)m->dev.size();
+  // slots lent by the previous call belong to device queues: they go back before this call waits for producers, who may
+  // need them, and before a queue lends new ones
+  for (int d = 0; d < D; d++)
+    if (m->used[d]) { urf_queue_release_view(m->dev[d].q); m->used[d] = 0; }
+  {
+    std::unique_lock<std::mutex> lk(m->mu);
+    if (!urf_internal::wait_for(m->cv, lk, timeout_ms, [&] { return !m->order.empty() || (m->closed && m->submitting == 0); }))
+      return URF_ERR_TIMEOUT;
+    if (m->order.empty()) return URF_ERR_CLOSED;          // closed and drained
+    m->ds.assign(m->order.begin(), m->order.begin() + std::min<size_t>((size_t)max_results, m->order.size()));
+  }
+  // Only this consumer takes entries out of `order` and scans out of the queues, so the snapshot's front stays valid and
+  // a scan seen done stays done. The k-th entry naming device d is the k-th oldest scan in d's queue.
+  const std::vector<int>& ds = m->ds;
+  std::vector<int>& want = m->want, & done = m->done, & used = m->used;
+  for (int d = 0; d < D; d++) { want[d] = 0; done[d] = -1; m->dst[d].clear(); }
+  for (int d : ds) want[d]++;
+  const int r = urf_internal::queue_done_run(m->dev[ds[0]].q, want[ds[0]], timeout_ms);   // waits for the oldest scan
+  if (r < 0) return r;
+  done[ds[0]] = r;
+  int k = 0;
+  for (; k < (int)ds.size(); k++) {                       // the run ends at the first scan that is not done on its device
+    const int d = ds[k];
+    if (done[d] < 0) done[d] = std::max(0, urf_internal::queue_done_run(m->dev[d].q, want[d], 0));
+    if (used[d] == done[d]) break;
+    used[d]++;
+    m->dst[d].push_back(k);
+  }
+  for (int d = 0; d < D; d++)
+    if (used[d]) urf_internal::queue_lend_run(m->dev[d].q, used[d], m->dst[d].data(), tags, rcs, outs, label_views);
+  {
+    std::lock_guard<std::mutex> lk(m->mu);
+    m->order.erase(m->order.begin(), m->order.begin() + k);
+    for (int d = 0; d < D; d++) { m->dev[d].inflight -= used[d]; m->dev[d].delivered += (uint64_t)used[d]; }
+  }
+  return k;
 }
 
 }  // namespace
@@ -139,22 +176,22 @@ extern "C" {
 
 int urf_mq_create(urf_mq** out, const int* devices, int n_devices, int max_points, int slots_per_device, int max_batch,
                   const urf_params* params) {
-  return create_real(out, devices, n_devices, max_points, slots_per_device, max_batch, params, URF_QUEUE_BLOCK);
+  return create(out, devices, nullptr, nullptr, n_devices, max_points, slots_per_device, max_batch, params, URF_QUEUE_BLOCK);
 }
 
 int urf_mq_create_label8(urf_mq** out, const int* devices, int n_devices, int max_points, int slots_per_device, int max_batch,
                          const urf_params* params) {
-  return create_real(out, devices, n_devices, max_points, slots_per_device, max_batch, params, URF_QUEUE_BLOCK | URF_QUEUE_LABEL8);
+  return create(out, devices, nullptr, nullptr, n_devices, max_points, slots_per_device, max_batch, params, URF_QUEUE_BLOCK | URF_QUEUE_LABEL8);
 }
 
 int urf_mq_create_with(urf_mq** out, urf_queue_process_fn fn, void* const* users, int n_devices, int max_points, int slots_per_device,
                        int max_batch) {
-  return create_stand_in(out, fn, users, n_devices, max_points, slots_per_device, max_batch, URF_QUEUE_BLOCK);
+  return create(out, nullptr, fn, users, n_devices, max_points, slots_per_device, max_batch, nullptr, URF_QUEUE_BLOCK);
 }
 
 int urf_mq_create_with_label8(urf_mq** out, urf_queue_process_fn fn, void* const* users, int n_devices, int max_points,
                               int slots_per_device, int max_batch) {
-  return create_stand_in(out, fn, users, n_devices, max_points, slots_per_device, max_batch, URF_QUEUE_BLOCK | URF_QUEUE_LABEL8);
+  return create(out, nullptr, fn, users, n_devices, max_points, slots_per_device, max_batch, nullptr, URF_QUEUE_BLOCK | URF_QUEUE_LABEL8);
 }
 
 int urf_mq_set_params(urf_mq* m, const urf_params* p) {
@@ -165,88 +202,34 @@ int urf_mq_set_params(urf_mq* m, const urf_params* p) {
 int urf_mq_submit(urf_mq* m, const float* xyzi, int n, uint64_t tag, int timeout_ms) { return submit_common(m, xyzi, n, tag, timeout_ms, false); }
 int urf_mq_submit_ref(urf_mq* m, const float* xyzi, int n, uint64_t tag, int timeout_ms) { return submit_common(m, xyzi, n, tag, timeout_ms, true); }
 
-namespace {
-int mq_next_common(urf_mq* m, uint64_t* tag, urf_result* out, const int32_t** label_view, int timeout_ms);
-}
-int urf_mq_next(urf_mq* m, uint64_t* tag, urf_result* out, int timeout_ms) { return mq_next_common(m, tag, out, nullptr, timeout_ms); }
-int urf_mq_next_view(urf_mq* m, uint64_t* tag, urf_result* out, const int32_t** label_view, int timeout_ms) {
-  if (!label_view || (m && m->label8)) return URF_ERR_INVALID;
-  return mq_next_common(m, tag, out, label_view, timeout_ms);
-}
-namespace {
-// Consumer side: gives back the slots lent by the previous call on every device except `keep` (whose own queue call does it).
-void release_mq_lent(urf_mq* m, int keep) {
-  for (int d = 0; d < (int)m->dev.size(); d++)
-    if (m->dev[d].lent) { if (d != keep) urf_queue_release_view(m->dev[d].q); m->dev[d].lent = false; }
-}
-
-int mq_next_common(urf_mq* m, uint64_t* tag, urf_result* out, const int32_t** label_view, int timeout_ms) {
-  if (!m || !out) return URF_ERR_INVALID;
-  int d;
-  {
-    std::unique_lock<std::mutex> lk(m->mu);
-    auto ready = [&] { return !m->order.empty() || (m->closed && m->submitting == 0); };
-    if (timeout_ms < 0) m->cv.wait(lk, ready);
-    else if (!m->cv.wait_for(lk, std::chrono::milliseconds(timeout_ms), ready)) return URF_ERR_TIMEOUT;
-    if (m->order.empty()) return URF_ERR_CLOSED;          // closed and drained
-    d = m->order.front();
-  }
-  // views lent by the previous call belong to device queues: give them back before a queue lends a new one
-  release_mq_lent(m, d);
-  const int rc = label_view ? urf_queue_next_view(m->dev[d].q, tag, out, label_view, timeout_ms) : urf_queue_next(m->dev[d].q, tag, out, timeout_ms);
-  if (rc == URF_ERR_TIMEOUT) return rc;                   // still the oldest scan: the entry stays at the front
-  if (label_view) m->dev[d].lent = true;
-  {
-    std::lock_guard<std::mutex> lk(m->mu);
-    m->order.pop_front();
-    m->dev[d].inflight--;
-    m->dev[d].delivered++;
-  }
-  return rc;
-}
-}  // namespace
-
 int urf_mq_next_batch(urf_mq* m, int max_results, uint64_t* tags, int32_t* rcs, urf_result* outs, const void** label_views,
                       int timeout_ms) {
   if (!m || !outs || max_results < 1) return URF_ERR_INVALID;
-  release_mq_lent(m, -1);
-  std::vector<int> ds;                                    // devices of the first scans in the global order
-  {
-    std::unique_lock<std::mutex> lk(m->mu);
-    auto ready = [&] { return !m->order.empty() || (m->closed && m->submitting == 0); };
-    if (timeout_ms < 0) m->cv.wait(lk, ready);
-    else if (!m->cv.wait_for(lk, std::chrono::milliseconds(timeout_ms), ready)) return URF_ERR_TIMEOUT;
-    if (m->order.empty()) return URF_ERR_CLOSED;          // closed and drained
-    ds.assign(m->order.begin(), m->order.begin() + std::min<size_t>((size_t)max_results, m->order.size()));
-  }
-  // Only this consumer takes entries out of `order` and scans out of the queues, so the snapshot's front stays valid and
-  // a scan seen done stays done. The k-th entry naming device d is the k-th oldest scan in d's queue.
-  const int D = (int)m->dev.size(), n = (int)ds.size();
-  std::vector<int> want(D, 0), done(D, -1), used(D, 0);
-  for (int d : ds) want[d]++;
-  const int r = urf_internal::queue_done_run(m->dev[ds[0]].q, want[ds[0]], timeout_ms);   // waits for the oldest scan
-  if (r < 0) return r;                                    // URF_ERR_TIMEOUT: the entry stays at the front
-  done[ds[0]] = r;
-  int k = 0;
-  for (; k < n; k++) {                                    // the run ends at the first scan that is not done on its device
-    const int d = ds[k];
-    if (done[d] < 0) done[d] = std::max(0, urf_internal::queue_done_run(m->dev[d].q, want[d], 0));
-    if (used[d] == done[d]) break;
-    used[d]++;
-  }
-  std::vector<std::vector<int>> dst(D);                   // output positions of each device's share, in its queue's order
-  for (int j = 0; j < k; j++) dst[ds[j]].push_back(j);
-  for (int d = 0; d < D; d++) {
-    if (!used[d]) continue;
-    urf_internal::queue_lend_run(m->dev[d].q, used[d], dst[d].data(), tags, rcs, outs, label_views);
-    m->dev[d].lent = true;
-  }
-  {
-    std::lock_guard<std::mutex> lk(m->mu);
-    m->order.erase(m->order.begin(), m->order.begin() + k);
-    for (int d = 0; d < D; d++) { m->dev[d].inflight -= used[d]; m->dev[d].delivered += (uint64_t)used[d]; }
-  }
-  return k;
+  return take_front_run(m, max_results, tags, rcs, outs, label_views, timeout_ms);
+}
+
+int urf_mq_next_view(urf_mq* m, uint64_t* tag, urf_result* out, const int32_t** label_view, int timeout_ms) {
+  if (!m || !out || !label_view || m->label8) return URF_ERR_INVALID;
+  int32_t rc = URF_OK;
+  const void* view = nullptr;
+  const int k = take_front_run(m, 1, tag, &rc, out, &view, timeout_ms);
+  if (k < 0) return k;
+  *label_view = static_cast<const int32_t*>(view);
+  return rc;
+}
+
+int urf_mq_next(urf_mq* m, uint64_t* tag, urf_result* out, int timeout_ms) {
+  if (!m || !out) return URF_ERR_INVALID;
+  int32_t* user_label = out->label;
+  int32_t rc = URF_OK;
+  const int k = take_front_run(m, 1, tag, &rc, out, nullptr, timeout_ms);
+  if (k < 0) return k;
+  out->label = user_label;
+  const int d = m->ds[0];
+  urf_internal::queue_copy_lent_labels(m->dev[d].q, user_label);
+  urf_queue_release_view(m->dev[d].q);                    // nothing stays lent: the slot goes back to the producers at once
+  m->used[d] = 0;
+  return rc;
 }
 
 int urf_mq_get_stats(urf_mq* m, urf_mq_stats* st) {

@@ -2,24 +2,24 @@
 //
 // Replaces the reference's depth-1 subscriber (`nh->subscribe(params::topicName, 1, &Detector::filtered, this)`,
 // lidar_segmentation.cpp:53): scans that arrive while a scan is being processed are staged instead of dropped, and the
-// worker hands everything that is pending to one batched call.
+// worker takes everything that is pending (up to max_batch scans) as one batch.
 //
 // Slot life cycle (all transitions under one mutex):
 //   FREE -> FILLING (producer copies the scan, lock released) -> PENDING -> RUNNING (worker) -> DONE -> FREE (consumer)
 //   PENDING -> FREE when URF_QUEUE_DROP_OLDEST needs room (the scan is counted as dropped, never delivered).
 // Results are delivered in submission order: every accepted scan gets a sequence number when it becomes PENDING and the
-// consumer waits for the smallest live one. urf_queue_next_batch hands out the whole run of DONE slots that follows it.
+// consumer waits for the smallest live one. Every delivery call (urf_queue_next / _next_view / _next_batch, and the mq's)
+// takes the run of DONE slots that starts there through take_done_run and hands it out through hand_out.
 //
 // Label slots are int32, or int8 with URF_QUEUE_LABEL8: the worker then asks the batch body for one-byte labels (float4
 // queues go through urf_enqueue_cloud2_batch with 16-byte records, as the synchronous path went through
 // urf_process_cloud2_batch).
 //
-// On a real context the worker keeps two batches in flight (urf_enqueue_batch / urf_finish_batch): it enqueues what is
-// pending, enqueues the next pending run too if there is one, and only then waits for the oldest batch, so the copies of
-// one batch overlap the kernels of the other and the device does not wait for the host's round trip between batches.
+// The worker is one loop with a depth. On a real context it keeps two batches in flight (urf_enqueue_batch /
+// urf_finish_batch): it enqueues what is pending, enqueues the next pending run too if there is one, and only then waits
+// for the oldest batch, so the copies of one batch overlap the kernels of the other and the device does not wait for the
+// host's round trip between batches. A synchronous stand-in (urf_queue_create_with) is the same loop at depth 1.
 #include <algorithm>
-#include <chrono>
-#include <condition_variable>
 #include <cstddef>
 #include <cstdlib>
 #include <cstring>
@@ -47,12 +47,12 @@ struct Slot {
 
 struct urf_queue {
   urf_ctx* ctx = nullptr;                  // real queue: batches go through urf_enqueue*_batch / urf_finish_batch
-  urf_queue_process_fn fn = nullptr;       // stand-in, synchronous (urf_queue_create_with)
-  urf_queue_process_fn enq = nullptr;      // stand-in, asynchronous pair (urf_queue_create_with_async)
-  urf_queue_finish_fn fin = nullptr;
+  urf_queue_process_fn enq = nullptr;      // stand-in: with fin the asynchronous pair (urf_queue_create_with_async), alone
+  urf_queue_finish_fn fin = nullptr;       // the synchronous batch function (urf_queue_create_with), which does it all
   void* user = nullptr;
   bool pinned = false;
   int max_points = 0, max_batch = 1, policy = URF_QUEUE_BLOCK;
+  int depth = 2;               // batches the worker keeps in flight: 2, or 1 around a synchronous stand-in
   bool label8 = false;         // URF_QUEUE_LABEL8: int8 label slots
   // record format of the scans: step == 0: (x, y, z, intensity) float4 points; step > 0: raw PointCloud2 records of `step`
   // bytes (urf_queue_create_cloud2), handed to urf_process_cloud2_batch and unpacked on the device
@@ -62,8 +62,10 @@ struct urf_queue {
   std::mutex mu;
   std::condition_variable cv_free, cv_pending, cv_done;
   uint64_t next_seq = 1;       // sequence number of the next accepted scan
-  std::vector<int> lent;       // slots lent out by urf_queue_next_view / _next_batch, given back on the consumer's next call
-  std::vector<std::pair<uint64_t, int>> live;   // consumer scratch (under mu): live slots in submission order
+  // Consumer side. The header allows one consumer at a time, so only that thread changes `lent`, and it may read it
+  // outside the lock: after a delivery call `lent` is exactly the run that call took, in submission order.
+  std::vector<int> lent;       // slots lent out by the last delivery call, given back on the consumer's next call
+  std::vector<std::pair<uint64_t, int>> live;   // scratch (under mu): live slots in submission order
   bool closed = false;
   urf_queue_stats st{};
   std::thread worker;
@@ -71,11 +73,7 @@ struct urf_queue {
 
 namespace {
 
-template <class Pred>
-bool wait_for(std::condition_variable& cv, std::unique_lock<std::mutex>& lk, int timeout_ms, Pred pred) {
-  if (timeout_ms < 0) { cv.wait(lk, pred); return true; }
-  return cv.wait_for(lk, std::chrono::milliseconds(timeout_ms), pred);
-}
+using urf_internal::wait_for;
 
 // One batch of the worker: the slots it took and the arguments of its batch call (which must outlive an asynchronous
 // batch until its finish).
@@ -85,6 +83,7 @@ struct Run {
   std::vector<int> ns;
   std::vector<urf_result> outs;
   std::vector<int8_t*> l8;
+  int rc = URF_OK;             // synchronous stand-in: what the batch function returned, reported by finish_run
 };
 
 // Takes every pending scan, oldest first, up to max_batch, into r (the slots become RUNNING: from here on they count as
@@ -144,9 +143,15 @@ void complete_run(urf_queue* q, const Run& r, int rc) {
   q->cv_done.notify_all();
 }
 
+// Starts run r. A synchronous stand-in does all its work here, and that counts as accepted: finish_run reports how it went.
 int enqueue_run(urf_queue* q, Run& r) {
   const int B = (int)r.idx.size();
-  if (q->enq) return q->enq(q->user, r.ptrs.data(), r.ns.data(), B, r.outs.data());
+  if (q->enq) {
+    const int rc = q->enq(q->user, r.ptrs.data(), r.ns.data(), B, r.outs.data());
+    if (q->fin) return rc;
+    r.rc = rc;
+    return URF_OK;
+  }
   if (q->step == 0 && !q->label8) return urf_enqueue_batch(q->ctx, r.ptrs.data(), r.ns.data(), B, r.outs.data(), nullptr);
   // float4 scans with int8 labels are 16-byte records (x, y, z, intensity at 0, 4, 8, 12) to the record body
   const bool f4 = q->step == 0;
@@ -155,28 +160,16 @@ int enqueue_run(urf_queue* q, Run& r) {
                                   q->label8 ? r.l8.data() : nullptr);
 }
 
-void note_in_flight(urf_queue* q, int k) {
-  std::lock_guard<std::mutex> lk(q->mu);
-  if (k > q->st.most_in_flight) q->st.most_in_flight = k;
-}
+// Waits for the oldest run in flight, r.
+int finish_run(urf_queue* q, const Run& r) { return q->ctx ? urf_finish_batch(q->ctx) : q->fin ? q->fin(q->user) : r.rc; }
 
-// Synchronous stand-in (urf_queue_create_with): one batch call at a time.
-void worker_loop_sync(urf_queue* q) {
-  Run r;
+// q->depth batches in flight: enqueue what is pending, enqueue the next pending run while a batch slot is free, then finish
+// the oldest batch. At depth 1 no second run is taken before the first is published. The queue drains what was accepted
+// before a close before the worker returns.
+void worker_loop(urf_queue* q) {
+  std::deque<Run> flight;                                 // enqueued, oldest first (at most q->depth)
   for (;;) {
-    bool closed = false;
-    if (!take_run(q, r, true, &closed)) { if (closed) return; continue; }
-    note_in_flight(q, 1);
-    complete_run(q, r, q->fn(q->user, r.ptrs.data(), r.ns.data(), (int)r.idx.size(), r.outs.data()));
-  }
-}
-
-// Two batches in flight: enqueue what is pending, enqueue the next pending run while a batch slot is free, then finish the
-// oldest batch. The queue drains what was accepted before a close before the worker returns.
-void worker_loop_async(urf_queue* q) {
-  std::deque<Run> flight;                                 // enqueued, oldest first (at most two)
-  for (;;) {
-    while (flight.size() < 2) {
+    while ((int)flight.size() < q->depth) {
       Run r;
       bool closed = false;
       if (!take_run(q, r, flight.empty(), &closed)) {
@@ -186,18 +179,13 @@ void worker_loop_async(urf_queue* q) {
       const int rc = enqueue_run(q, r);
       if (rc != URF_OK) { complete_run(q, r, rc); continue; }   // nothing of a refused batch is in flight
       flight.push_back(std::move(r));                     // the vectors' storage, which the batch points at, moves along
-      note_in_flight(q, (int)flight.size());
+      std::lock_guard<std::mutex> lk(q->mu);
+      q->st.most_in_flight = std::max(q->st.most_in_flight, (int32_t)flight.size());
     }
     if (flight.empty()) continue;
-    const int rc = q->fin ? q->fin(q->user) : urf_finish_batch(q->ctx);
-    complete_run(q, flight.front(), rc);
+    complete_run(q, flight.front(), finish_run(q, flight.front()));
     flight.pop_front();
   }
-}
-
-void worker_loop(urf_queue* q) {
-  if (q->fn) worker_loop_sync(q);
-  else worker_loop_async(q);
 }
 
 void free_slot(const urf_queue* q, Slot& s) {
@@ -207,22 +195,22 @@ void free_slot(const urf_queue* q, Slot& s) {
   s.in = nullptr; s.label = nullptr; s.label8 = nullptr;
 }
 
-// Exactly one of ctx (real queue, pinned slots), fn (synchronous stand-in) and enq + fin (asynchronous stand-in) is set.
-int create_common(urf_queue** out, urf_ctx* ctx, urf_queue_process_fn fn, urf_queue_process_fn enq, urf_queue_finish_fn fin, void* user,
+// Either ctx (real queue, pinned slots) or enq (stand-in; synchronous, and the worker's depth 1, without fin) is set.
+int create_common(urf_queue** out, urf_ctx* ctx, urf_queue_process_fn enq, urf_queue_finish_fn fin, void* user,
                   int max_points, int slots, int max_batch, int policy, int step = 0, int ox = 0, int oy = 4, int oz = 8, int oi = -1) {
   const bool label8 = (policy & URF_QUEUE_LABEL8) != 0;
   policy &= ~URF_QUEUE_LABEL8;
-  if (!out || (!ctx && !fn && !(enq && fin)) || max_points < 1 || slots < 1 || max_batch < 1 ||
+  if (!out || (!ctx && !enq) || max_points < 1 || slots < 1 || max_batch < 1 ||
       (policy != URF_QUEUE_BLOCK && policy != URF_QUEUE_DROP_OLDEST))
     return URF_ERR_INVALID;
   const bool pinned = ctx != nullptr;
   urf_queue* q = new urf_queue;
-  q->ctx = ctx; q->fn = fn; q->enq = enq; q->fin = fin; q->user = user;
+  q->ctx = ctx; q->enq = enq; q->fin = fin; q->user = user;
   q->pinned = pinned; q->max_points = max_points; q->max_batch = max_batch; q->policy = policy;
-  q->label8 = label8;
+  q->label8 = label8; q->depth = ctx || fin ? 2 : 1;
   q->step = step; q->ox = ox; q->oy = oy; q->oz = oz; q->oi = oi;
   q->bytes_per_point = step > 0 ? (size_t)step : 16;
-  q->slots.resize(slots);
+  q->slots.resize(slots); q->lent.reserve(slots); q->live.reserve(slots);
   // int8 slots hold max_points bytes of labels; a stand-in batch function still writes int32 labels, which need a buffer
   const bool want32 = !label8 || !ctx, want8 = label8;
   auto alloc = [pinned](size_t bytes) { return pinned ? urf_pinned_alloc(bytes) : std::malloc(bytes); };
@@ -248,7 +236,7 @@ extern "C" {
 
 int urf_queue_create(urf_queue** out, urf_ctx* ctx, int max_points, int slots, int max_batch, int policy) {
   if (!ctx) return URF_ERR_INVALID;
-  return create_common(out, ctx, nullptr, nullptr, nullptr, nullptr, max_points, slots, max_batch, policy);
+  return create_common(out, ctx, nullptr, nullptr, nullptr, max_points, slots, max_batch, policy);
 }
 
 int urf_queue_create_cloud2(urf_queue** out, urf_ctx* ctx, int max_points, int slots, int max_batch, int policy, int point_step, int off_x,
@@ -256,19 +244,19 @@ int urf_queue_create_cloud2(urf_queue** out, urf_ctx* ctx, int max_points, int s
   if (!ctx || point_step < 12 || point_step > URF_MAX_POINT_STEP) return URF_ERR_INVALID;
   for (int o : {off_x, off_y, off_z}) if (o < 0 || o + 4 > point_step) return URF_ERR_INVALID;
   if (off_intensity >= 0 && off_intensity + 4 > point_step) return URF_ERR_INVALID;
-  return create_common(out, ctx, nullptr, nullptr, nullptr, nullptr, max_points, slots, max_batch, policy, point_step, off_x, off_y, off_z,
+  return create_common(out, ctx, nullptr, nullptr, nullptr, max_points, slots, max_batch, policy, point_step, off_x, off_y, off_z,
                        off_intensity);
 }
 
 int urf_queue_create_with(urf_queue** out, urf_queue_process_fn fn, void* user, int max_points, int slots, int max_batch, int policy) {
   if (!fn) return URF_ERR_INVALID;
-  return create_common(out, nullptr, fn, nullptr, nullptr, user, max_points, slots, max_batch, policy);
+  return create_common(out, nullptr, fn, nullptr, user, max_points, slots, max_batch, policy);
 }
 
 int urf_queue_create_with_async(urf_queue** out, urf_queue_process_fn enqueue, urf_queue_finish_fn finish, void* user, int max_points,
                                 int slots, int max_batch, int policy) {
   if (!enqueue || !finish) return URF_ERR_INVALID;
-  return create_common(out, nullptr, nullptr, enqueue, finish, user, max_points, slots, max_batch, policy);
+  return create_common(out, nullptr, enqueue, finish, user, max_points, slots, max_batch, policy);
 }
 
 namespace {
@@ -340,17 +328,6 @@ int urf_queue_submit_cloud2(urf_queue* q, const void* data, int n_points, uint64
 }
 
 namespace {
-int next_common(urf_queue* q, uint64_t* tag, urf_result* out, const int32_t** label_view, int timeout_ms);
-}
-
-int urf_queue_next(urf_queue* q, uint64_t* tag, urf_result* out, int timeout_ms) { return next_common(q, tag, out, nullptr, timeout_ms); }
-
-int urf_queue_next_view(urf_queue* q, uint64_t* tag, urf_result* out, const int32_t** label_view, int timeout_ms) {
-  if (!label_view || (q && q->label8)) return URF_ERR_INVALID;         // int8 slots have no int32 view: urf_queue_next_batch
-  return next_common(q, tag, out, label_view, timeout_ms);
-}
-
-namespace {
 // Gives the slots lent by the previous urf_queue_next_view / _next_batch call back to the producers (mu held).
 void release_lent(urf_queue* q) {
   if (q->lent.empty()) return;
@@ -359,36 +336,19 @@ void release_lent(urf_queue* q) {
   q->cv_free.notify_all();
 }
 
-// The oldest live scan (smallest sequence number among PENDING / RUNNING / DONE slots): 1 and *slot when it is DONE,
-// 2 when the queue is closed and drained, 0 otherwise (mu held).
-int front_state(const urf_queue* q, int* slot) {
-  int best = -1;
-  bool filling = false;
-  for (int i = 0; i < (int)q->slots.size(); i++) {
-    const Slot& s = q->slots[i];
-    if (s.state == FILLING) filling = true;
-    if ((s.state == PENDING || s.state == RUNNING || s.state == DONE) && (best < 0 || s.seq < q->slots[best].seq)) best = i;
-  }
-  if (best >= 0 && q->slots[best].state == DONE) { *slot = best; return 1; }
-  if (best < 0 && !filling && q->closed) return 2;
-  return 0;
-}
-
-// Waits up to timeout_ms until the oldest live scan is done: URF_OK, URF_ERR_TIMEOUT or URF_ERR_CLOSED (mu held).
-int wait_front(urf_queue* q, std::unique_lock<std::mutex>& lk, int timeout_ms, int* slot) {
-  int state = 0;
-  if (!wait_for(q->cv_done, lk, timeout_ms, [&] { return (state = front_state(q, slot)) != 0; })) return URF_ERR_TIMEOUT;
-  return state == 2 ? (int)URF_ERR_CLOSED : (int)URF_OK;
-}
-
-// The run of DONE slots at the front, in submission order, at most max_results of them, into q->live (mu held).
-// A dropped scan's slot was reused and carries a new sequence number, so it is skipped like in urf_queue_next.
+// The run of DONE slots that starts with the oldest live scan (smallest sequence number among PENDING / RUNNING / DONE
+// slots), in submission order, at most max_results of them, into q->live: its length, 0 while the oldest live scan is not
+// done, URF_ERR_CLOSED when the queue is closed and drained (mu held). A dropped scan's slot was reused and carries a new
+// sequence number, so it is skipped.
 int done_run(urf_queue* q, int max_results) {
   q->live.clear();
+  bool filling = false;
   for (int i = 0; i < (int)q->slots.size(); i++) {
     const SlotState st = q->slots[i].state;
+    if (st == FILLING) filling = true;
     if (st == PENDING || st == RUNNING || st == DONE) q->live.emplace_back(q->slots[i].seq, i);
   }
+  if (q->live.empty()) return q->closed && !filling ? (int)URF_ERR_CLOSED : 0;
   std::sort(q->live.begin(), q->live.end());
   int k = 0;
   while (k < (int)q->live.size() && k < max_results && q->slots[q->live[k].second].state == DONE) k++;
@@ -396,10 +356,28 @@ int done_run(urf_queue* q, int max_results) {
   return k;
 }
 
-// Marks the k slots of q->live as lent (invisible to producers and the worker until release_lent) (mu held).
-void lend(urf_queue* q, int k) {
+// The first half of every delivery call (mu held): the slots lent by the previous call come back, then waits up to
+// timeout_ms for done_run to find a run (>= 1) or the drained queue (URF_ERR_CLOSED); URF_ERR_TIMEOUT otherwise.
+int wait_done_run(urf_queue* q, std::unique_lock<std::mutex>& lk, int max_results, int timeout_ms) {
+  release_lent(q);
+  int k = 0;
+  if (!wait_for(q->cv_done, lk, timeout_ms, [&] { return (k = done_run(q, max_results)) != 0; })) return URF_ERR_TIMEOUT;
+  return k;
+}
+
+// The second half (mu held): the first k slots of q->live become lent: VIEWED slots are invisible to producers and the
+// worker until release_lent, so the consumer reads them outside the lock.
+int lend(urf_queue* q, int k) {
   for (int j = 0; j < k; j++) { q->slots[q->live[j].second].state = VIEWED; q->lent.push_back(q->live[j].second); }
   q->st.delivered += (uint64_t)k;
+  return k;
+}
+
+// Both halves in the one lock round of a urf_queue_next* call: the number of slots now in q->lent, or the error code.
+int take_done_run(urf_queue* q, int max_results, int timeout_ms) {
+  std::unique_lock<std::mutex> lk(q->mu);
+  const int k = wait_done_run(q, lk, max_results, timeout_ms);
+  return k < 0 ? k : lend(q, k);
 }
 
 // The fields of a finished scan the consumer gets: counts and flags, and only the n_vert vertices that exist.
@@ -410,11 +388,10 @@ void copy_result(urf_result* dst, const urf_result& src) {
   std::memcpy(dst->vert, src.vert, sizeof(src.vert[0]) * (size_t)nv);
 }
 
-// Hands out the slots lent by lend(): slot[j] goes to index dst ? dst[j] : j. Runs outside the lock (the slots are ours).
-void hand_out(const urf_queue* q, const int* slot, int k, const int* dst, uint64_t* tags, int32_t* rcs, urf_result* outs,
-              const void** label_views) {
-  for (int j = 0; j < k; j++) {
-    const Slot& s = q->slots[slot[j]];
+// Hands out the slots of q->lent: the j-th goes to index dst ? dst[j] : j. Runs outside the lock (the slots are ours).
+void hand_out(const urf_queue* q, const int* dst, uint64_t* tags, int32_t* rcs, urf_result* outs, const void** label_views) {
+  for (int j = 0; j < (int)q->lent.size(); j++) {
+    const Slot& s = q->slots[q->lent[j]];
     const int o = dst ? dst[j] : j;
     if (tags) tags[o] = s.tag;
     if (rcs) rcs[o] = s.rc;
@@ -422,60 +399,38 @@ void hand_out(const urf_queue* q, const int* slot, int k, const int* dst, uint64
     if (label_views) label_views[o] = s.rc != URF_OK ? nullptr : q->label8 ? (const void*)s.label8 : (const void*)s.label;
   }
 }
-
-// label_view != NULL: no copy — *label_view points at the labels inside the queue's staging slot, which stays reserved
-// (not reusable by producers) until this consumer's next urf_queue_next* call on the queue.
-int next_common(urf_queue* q, uint64_t* tag, urf_result* out, const int32_t** label_view, int timeout_ms) {
-  if (!q || !out) return URF_ERR_INVALID;
-  std::unique_lock<std::mutex> lk(q->mu);
-  release_lent(q);                                        // the slots lent out by the previous call come back now
-  int slot = -1;
-  const int wrc = wait_front(q, lk, timeout_ms, &slot);
-  if (wrc != URF_OK) return wrc;
-  Slot& s = q->slots[slot];
-  int32_t* user_label = out->label;
-  const int rc = s.rc;
-  *out = s.res;
-  out->label = user_label; out->ring = nullptr; out->order = nullptr; out->ring_start = nullptr;
-  if (tag) *tag = s.tag;
-  q->st.delivered++;
-  if (label_view) {                                       // lend the slot: DONE slots are invisible to producers and the worker
-    *label_view = rc == URF_OK ? s.label : nullptr;
-    s.state = VIEWED;
-    q->lent.push_back(slot);
-    return rc;
-  }
-  const int n = s.n;
-  s.state = VIEWED;                                       // ours: invisible to producers, the worker and other consumers
-  lk.unlock();                                            // the copy runs outside the lock
-  if (user_label && rc == URF_OK && n > 0) {
-    if (q->label8) for (int i = 0; i < n; i++) user_label[i] = s.label8[i];      // int8 slot: widened for the caller
-    else std::memcpy(user_label, s.label, sizeof(int32_t) * (size_t)n);
-  }
-  lk.lock();
-  s.state = FREE;
-  lk.unlock();
-  q->cv_free.notify_one();
-  return rc;
-}
 }  // namespace
 
 int urf_queue_next_batch(urf_queue* q, int max_results, uint64_t* tags, int32_t* rcs, urf_result* outs, const void** label_views,
                          int timeout_ms) {
   if (!q || !outs || max_results < 1) return URF_ERR_INVALID;
-  std::vector<int> idx;
-  {
-    std::unique_lock<std::mutex> lk(q->mu);               // the only lock round of the call
-    release_lent(q);
-    int front = -1;
-    const int wrc = wait_front(q, lk, timeout_ms, &front);
-    if (wrc != URF_OK) return wrc;
-    const int k = done_run(q, max_results);               // >= 1: the front is done
-    for (int j = 0; j < k; j++) idx.push_back(q->live[j].second);
-    lend(q, k);
-  }
-  hand_out(q, idx.data(), (int)idx.size(), nullptr, tags, rcs, outs, label_views);
-  return (int)idx.size();
+  const int k = take_done_run(q, max_results, timeout_ms);
+  if (k > 0) hand_out(q, nullptr, tags, rcs, outs, label_views);
+  return k;
+}
+
+// No copy: *label_view points at the labels inside the queue's staging slot, which stays reserved (not reusable by
+// producers) until this consumer's next urf_queue_next* call on the queue.
+int urf_queue_next_view(urf_queue* q, uint64_t* tag, urf_result* out, const int32_t** label_view, int timeout_ms) {
+  if (!q || !out || !label_view || q->label8) return URF_ERR_INVALID;  // int8 slots have no int32 view: urf_queue_next_batch
+  int32_t rc = URF_OK;
+  const void* view = nullptr;
+  const int k = urf_queue_next_batch(q, 1, tag, &rc, out, &view, timeout_ms);
+  if (k < 0) return k;
+  *label_view = static_cast<const int32_t*>(view);
+  return rc;
+}
+
+int urf_queue_next(urf_queue* q, uint64_t* tag, urf_result* out, int timeout_ms) {
+  if (!q || !out) return URF_ERR_INVALID;
+  int32_t* user_label = out->label;
+  int32_t rc = URF_OK;
+  const int k = urf_queue_next_batch(q, 1, tag, &rc, out, nullptr, timeout_ms);
+  if (k < 0) return k;
+  out->label = user_label;
+  urf_internal::queue_copy_lent_labels(q, user_label);    // outside the lock
+  urf_queue_release_view(q);                              // nothing stays lent: the slot goes back to the producers at once
+  return rc;
 }
 
 void urf_queue_release_view(urf_queue* q) {
@@ -518,25 +473,25 @@ namespace urf_internal {
 
 int queue_done_run(urf_queue* q, int max_results, int timeout_ms) {
   std::unique_lock<std::mutex> lk(q->mu);
-  release_lent(q);
-  int front = -1;
-  const int wrc = wait_front(q, lk, timeout_ms, &front);
-  if (wrc == URF_ERR_TIMEOUT && timeout_ms == 0) return 0;
-  if (wrc != URF_OK) return wrc;
-  return done_run(q, max_results);
+  const int k = wait_done_run(q, lk, max_results, timeout_ms);
+  return k == URF_ERR_TIMEOUT && timeout_ms == 0 ? 0 : k;
 }
 
 int queue_lend_run(urf_queue* q, int count, const int* dst, uint64_t* tags, int32_t* rcs, urf_result* outs, const void** label_views) {
-  std::vector<int> idx;
   {
     std::lock_guard<std::mutex> lk(q->mu);
-    // a run that was done stays done (only this consumer takes scans out), so this is the run queue_done_run counted
-    const int k = done_run(q, count);
-    for (int j = 0; j < k; j++) idx.push_back(q->live[j].second);
-    lend(q, k);
+    // only this consumer takes scans out and rebuilds q->live, so the run queue_done_run left there is still done
+    lend(q, std::min(count, (int)q->live.size()));
   }
-  hand_out(q, idx.data(), (int)idx.size(), dst, tags, rcs, outs, label_views);
-  return (int)idx.size();
+  hand_out(q, dst, tags, rcs, outs, label_views);
+  return (int)q->lent.size();
+}
+
+void queue_copy_lent_labels(const urf_queue* q, int32_t* dst) {
+  const Slot& s = q->slots[q->lent.front()];
+  if (!dst || s.rc != URF_OK || s.n < 1) return;
+  if (q->label8) for (int i = 0; i < s.n; i++) dst[i] = s.label8[i];   // int8 slot: widened for the caller
+  else std::memcpy(dst, s.label, sizeof(int32_t) * (size_t)s.n);
 }
 
 }  // namespace urf_internal

@@ -1,23 +1,38 @@
-// urf_queue_internal.hpp — the two pieces of urf_queue_next_batch that urf_mq_next_batch needs separately, and the idle
-// rule of the mq's settings (host code, C++ linkage, not part of include/urf.h). urf_mq first asks every device queue how far its run of finished scans reaches,
-// cuts the global order at the first scan that is not done, and only then has each queue lend exactly its share.
+// urf_queue_internal.hpp — what urf_queue.cpp and urf_mq.cpp share (host code, C++ linkage, not part of include/urf.h):
+// the timed wait, the two halves of a delivery call, which urf_mq needs separately, the copy of a lent scan's labels, and
+// the idle rule of the mq's settings. urf_mq first asks every device queue how far its run of finished scans reaches, cuts
+// the global order at the first scan that is not done, and only then has each queue lend exactly its share.
 #pragma once
 
+#include <chrono>
+#include <condition_variable>
 #include <cstdint>
+#include <mutex>
 
 #include "../../include/urf.h"
 
 namespace urf_internal {
 
-// Gives back the slots lent by earlier urf_queue_next* calls, waits up to timeout_ms (< 0: forever, 0: no wait) until the
+// cv.wait(lk, pred) for up to timeout_ms (< 0: forever): false when the time ran out with pred still false.
+template <class Pred>
+bool wait_for(std::condition_variable& cv, std::unique_lock<std::mutex>& lk, int timeout_ms, Pred pred) {
+  if (timeout_ms < 0) { cv.wait(lk, pred); return true; }
+  return cv.wait_for(lk, std::chrono::milliseconds(timeout_ms), pred);
+}
+
+// Gives back the slots lent by earlier delivery calls, waits up to timeout_ms (< 0: forever, 0: no wait) until the
 // oldest live scan is done, and returns how many consecutive scans from the oldest on are done (at most max_results).
 // URF_ERR_TIMEOUT / URF_ERR_CLOSED as for urf_queue_next; with timeout_ms == 0 a queue whose oldest scan is not done
 // returns 0 instead of URF_ERR_TIMEOUT.
 int queue_done_run(urf_queue* q, int max_results, int timeout_ms);
 
-// Lends the next `count` scans, which queue_done_run has seen done, in submission order: scan j goes to index dst[j] of
-// tags / rcs / outs / label_views (each may be NULL except outs). Returns the number lent.
+// Lends the next `count` scans, which queue_done_run has just seen done, in submission order: scan j goes to index dst[j]
+// of tags / rcs / outs / label_views (each may be NULL except outs). Returns the number lent.
 int queue_lend_run(urf_queue* q, int count, const int* dst, uint64_t* tags, int32_t* rcs, urf_result* outs, const void** label_views);
+
+// Copies the labels of the oldest scan the last delivery call lent into the caller's n_in int32 labels, widening them
+// from an int8 slot. Nothing is copied for a failed scan or with dst == NULL.
+void queue_copy_lent_labels(const urf_queue* q, int32_t* dst);
 
 // Runs fn(ctx, arg) on the context of every device of the mq, in device order, while nothing is in flight (everything
 // submitted has been collected): URF_ERR_INVALID otherwise. Stops at the first error and returns it. Stand-in devices
