@@ -10,7 +10,7 @@ import os
 
 import numpy as np
 
-from .ctypes_abi import (UrfMqStats, QUEUE_FINISH_FN, QUEUE_PROCESS_FN, URF_ERR_CLOSED, URF_ERR_TIMEOUT, URF_MAX_CHANNELS, URF_MAX_VERTS, URF_OK, URF_QUEUE_BLOCK,
+from .ctypes_abi import (UrfMqStats, QUEUE_FINISH_FN, QUEUE_PARAMS_FN, QUEUE_PROCESS_FN, URF_ERR_CLOSED, URF_ERR_TIMEOUT, URF_MAX_CHANNELS, URF_MAX_VERTS, URF_OK, URF_QUEUE_BLOCK,
                          URF_QUEUE_DROP_OLDEST, URF_QUEUE_LABEL8, URF_TOO_FEW_POINTS, UrfClouds, UrfParams, UrfQueueStats, UrfResult,
                          UrfStrip, make_params)
 
@@ -24,7 +24,9 @@ EXPORTS = ["urf_queue_next_batch", "urf_mq_next_batch", "urf_mq_create_label8", 
            "urf_set_params", "urf_get_params", "urf_process", "urf_process_batch", "urf_process_batch_device",
            "urf_process_batch_xyz", "urf_process_cloud2_batch", "urf_enqueue_batch_device", "urf_enqueue_batch_device_ex", "urf_finish_batch_device", "urf_stream", "urf_last_device_ms",
            "urf_last_launch_count", "urf_build_markers", "urf_set_tie_order", "urf_get_tie_order", "urf_mq_set_tie_order",
-           "urf_enqueue_batch", "urf_enqueue_cloud2_batch", "urf_finish_batch", "urf_queue_create_with_async"]
+           "urf_enqueue_batch", "urf_enqueue_cloud2_batch", "urf_finish_batch", "urf_queue_create_with_async",
+           "urf_set_params_next", "urf_queue_update_params", "urf_mq_update_params", "urf_queue_set_params_hook",
+           "urf_mq_set_params_hook"]
 
 # urf_set_tie_order modes (include/urf.h): equal azimuths inside a ring in input order, or in the reference's Lomuto order
 TIE_ORDERS = {"input": 0, "reference": 1}
@@ -57,6 +59,7 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
     lib.urf_create.argtypes = [C.POINTER(vp), ip, ip, ip]
     lib.urf_destroy.argtypes = [vp]
     lib.urf_set_params.argtypes = [vp, C.POINTER(UrfParams)]
+    lib.urf_set_params_next.argtypes = [vp, C.POINTER(UrfParams)]
     lib.urf_get_params.argtypes = [vp, C.POINTER(UrfParams)]
     lib.urf_set_option.argtypes = [vp, ip, ip]
     lib.urf_set_tie_order.argtypes = [vp, ip]
@@ -102,6 +105,10 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
     lib.urf_mq_create.argtypes = [C.POINTER(vp), C.POINTER(ip), ip, ip, ip, ip, C.POINTER(UrfParams)]
     lib.urf_mq_create_with.argtypes = [C.POINTER(vp), QUEUE_PROCESS_FN, C.POINTER(vp), ip, ip, ip, ip]
     lib.urf_mq_set_params.argtypes = [vp, C.POINTER(UrfParams)]
+    lib.urf_queue_update_params.argtypes = [vp, C.POINTER(UrfParams)]
+    lib.urf_mq_update_params.argtypes = [vp, C.POINTER(UrfParams)]
+    lib.urf_queue_set_params_hook.argtypes = [vp, QUEUE_PARAMS_FN]
+    lib.urf_mq_set_params_hook.argtypes = [vp, QUEUE_PARAMS_FN]
     lib.urf_mq_submit.argtypes = [vp, vp, ip, C.c_uint64, ip]
     lib.urf_mq_submit_ref.argtypes = [vp, vp, ip, C.c_uint64, ip]
     lib.urf_mq_next.argtypes = [vp, C.POINTER(C.c_uint64), C.POINTER(UrfResult), ip]
@@ -132,7 +139,7 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
 
 class ScanResult:
     """Per-scan output of the path (urf_result, include/urf.h)."""
-    __slots__ = ("status", "n_in", "n_roi", "n_rings", "n_order", "n_road", "n_curb", "n_vert", "flags", "label",
+    __slots__ = ("status", "n_in", "n_roi", "n_rings", "n_order", "n_road", "n_curb", "n_vert", "flags", "params_gen", "label",
                  "ring", "order", "ring_start", "vert")
 
     @property
@@ -158,7 +165,7 @@ def _scan_result(res: UrfResult, label, ring=None, order=None, ring_start=None) 
     """ScanResult of a filled urf_result: `label` and `ring` as given, `order` / `ring_start` (the caller's whole buffers, or
     None) cut to n_order / n_rings + 1 entries and copied, the vertices copied."""
     r = ScanResult()
-    for f in ("status", "n_in", "n_roi", "n_rings", "n_order", "n_road", "n_curb", "n_vert", "flags"):
+    for f in ("status", "n_in", "n_roi", "n_rings", "n_order", "n_road", "n_curb", "n_vert", "flags", "params_gen"):
         setattr(r, f, int(getattr(res, f)))
     r.label, r.ring = label, ring
     r.order = None if order is None else order[: r.n_order].copy()
@@ -317,6 +324,15 @@ class Detector:
         self._check(self.lib.urf_set_params(self._ctx, C.byref(prm)), "urf_set_params")
         self.params = prm
 
+    def set_params_next(self, prm: UrfParams) -> int:
+        """paramsCallback while batches are in flight (urf_set_params_next): `prm` applies from the next enqueue / filtered
+        call on, batches already enqueued keep the set they were enqueued with. Returns the new parameter generation, which
+        the results of later calls report as `params_gen`."""
+        gen = self.lib.urf_set_params_next(self._ctx, C.byref(prm))
+        self._check(gen, "urf_set_params_next")
+        self.params = prm
+        return gen
+
     def set_option(self, option: int, value: int):
         self._check(self.lib.urf_set_option(self._ctx, option, value), "urf_set_option")
 
@@ -356,7 +372,8 @@ class Detector:
         """Enqueues a prepared batch (BatchHandle.of_clouds / of_records; urf_enqueue_batch / urf_enqueue_cloud2_batch) and
         returns at once when its buffers are pinned. finish_batch fills its `results`. At most two batches are in flight;
         the detector keeps the handle alive until then. While batches are in flight every other compute call and
-        set_params / set_tie_order / set_option raise (URF_ERR_INVALID)."""
+        set_params / set_tie_order / set_option raise (URF_ERR_INVALID); set_params_next changes the set of the next
+        enqueue."""
         B = len(hb.ns)
         if hb.step == 0:
             rc, where = self.lib.urf_enqueue_batch(self._ctx, hb.ptrs, hb.ns, B, hb.res, hb.l8), "urf_enqueue_batch"
@@ -481,17 +498,42 @@ class _StreamQueue:
     `_PREFIX` + name (urf_queue_* or urf_mq_*), which have the same arguments in both families."""
     _PREFIX = ""
 
-    def __init__(self, max_points: int, label8: bool):
+    def __init__(self, max_points: int, label8: bool, params: UrfParams | None = None):
         self.lib = load_library()
         self._h = C.c_void_p()
         self.max_points = max_points
         self.label8 = label8
         self._cb = None                   # ctypes callbacks of a stand-in, kept alive with the queue
+        self._params_cb = None            # the parameter hook of a stand-in
         self._bufs = None
         self._keep = {}                   # arrays of by-reference submits, until their results come back
+        self._sets = {0: params}          # parameter generation -> set (0: the set in force at creation, None if unknown)
 
     def _call(self, name: str, *args) -> int:
         return getattr(self.lib, self._PREFIX + name)(self._h, *args)
+
+    def update_params(self, prm: UrfParams) -> int:
+        """New parameters for a running queue, with no drain (urf_queue_update_params / urf_mq_update_params): every scan
+        submitted after this returns runs with `prm`, every scan before with the earlier sets, and no batch mixes them.
+        Returns the new generation; results report theirs as `params_gen`, and params_of(gen) gives its set back."""
+        gen = self._call("update_params", C.byref(prm))
+        if gen < 0:
+            raise UrfError(gen, self._PREFIX + "update_params")
+        self._sets[gen] = UrfParams.from_buffer_copy(prm)   # a copy: the caller may change its own set afterwards
+        return gen
+
+    def params_of(self, gen: int) -> UrfParams | None:
+        """The set of generation `gen` (for build_markers of a result with that params_gen); None for generation 0 when the
+        queue does not know it (stand-in devices). One entry is kept per update."""
+        return self._sets[gen]
+
+    def set_params_hook(self, fn):
+        """Stand-in queues only (tests): fn(user, params pointer, generation) -> int is called where a real queue's worker
+        calls urf_set_params_next (urf_queue_set_params_hook / urf_mq_set_params_hook)."""
+        self._params_cb = QUEUE_PARAMS_FN(fn)
+        rc = self._call("set_params_hook", self._params_cb)
+        if rc != URF_OK:
+            raise UrfError(rc, self._PREFIX + "set_params_hook")
 
     def submit(self, cloud: np.ndarray, tag: int = 0, timeout_ms: int = -1, by_reference: bool = False) -> int:
         """Returns URF_OK, URF_ERR_TIMEOUT or URF_ERR_CLOSED; raises on anything else. by_reference: no copy
@@ -558,7 +600,7 @@ class MultiGpuQueue(_StreamQueue):
 
     def __init__(self, devices, max_points: int, slots_per_device: int = 8, max_batch: int = 4, params: UrfParams | None = None,
                  process_fn=None, label8: bool = False):
-        super().__init__(max_points, label8)
+        super().__init__(max_points, label8, None if process_fn is not None else params if params is not None else make_params())
         if process_fn is not None:                      # tests: stand-in devices, no GPU
             self._cb = QUEUE_PROCESS_FN(process_fn)
             create = self.lib.urf_mq_create_with_label8 if label8 else self.lib.urf_mq_create_with
@@ -604,7 +646,7 @@ class ScanQueue(_StreamQueue):
 
     def __init__(self, detector: "Detector | None", max_points: int, slots: int = 8, max_batch: int = 4,
                  policy: int = URF_QUEUE_BLOCK, process_fn=None, label8: bool = False, enqueue_fn=None, finish_fn=None):
-        super().__init__(max_points, label8)
+        super().__init__(max_points, label8, detector.params if detector is not None else None)
         if label8:
             policy |= URF_QUEUE_LABEL8
         if enqueue_fn is not None:

@@ -15,7 +15,7 @@ NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-
 SOURCES = ["urf_api.cu"]
 HOST_SOURCES = ["urf_markers.cpp", "urf_queue.cpp", "urf_mq.cpp"]
 HEADERS = ["urf_kernels.cuh", "urf_logic.cuh", "urf_device.cuh", "urf_workspace.cuh", "urf_math.cuh", "urf_stdsort.cuh", "urf_lomuto.cuh",
-           "urf_host.hpp", "urf_queue_internal.hpp"]
+           "urf_host.hpp", "urf_params.hpp", "urf_queue_internal.hpp"]
 
 
 def _nvcc() -> str:
@@ -94,13 +94,13 @@ def build_kat() -> None:
     # ThreadSanitizer build of the streaming queue around a stand-in batch function (no CUDA involved)
     tgt = os.path.join(bdir, "queue_stress")
     qsrc = [os.path.join(kat, "queue_stress.cpp"), os.path.join(CSRC, "urf_queue.cpp"), os.path.join(CSRC, "urf_mq.cpp"),
-            os.path.join(kat, "queue_async_stubs.cpp")]
-    qdeps = [os.path.join(ROOT, "include", "urf.h"), os.path.join(CSRC, "urf_queue_internal.hpp")]
+            os.path.join(kat, "queue_async_stubs.cpp"), os.path.join(kat, "queue_params_stubs.cpp")]
+    qdeps = [os.path.join(ROOT, "include", "urf.h"), os.path.join(CSRC, "urf_queue_internal.hpp"), os.path.join(CSRC, "urf_params.hpp")]
     if _stale(tgt, qsrc + qdeps):
         subprocess.run(["g++", "-std=c++17", "-O1", "-g", "-fsanitize=thread", "-pthread", "-o", tgt, *qsrc], check=True)
-    # the same for batched delivery (urf_queue_next_batch / urf_mq_next_batch) and int8 label slots, and for the worker's
-    # two-batches-in-flight schedule around an asynchronous stand-in
-    for name in ("queue_batch_stress", "queue_async_stress"):
+    # the same for batched delivery (urf_queue_next_batch / urf_mq_next_batch) and int8 label slots, for the worker's
+    # two-batches-in-flight schedule around an asynchronous stand-in, and for parameter updates on a running queue
+    for name in ("queue_batch_stress", "queue_async_stress", "queue_params_stress"):
         tgt = os.path.join(bdir, name)
         src = [os.path.join(kat, name + ".cpp")] + qsrc[1:]
         if _stale(tgt, src + qdeps):

@@ -74,8 +74,10 @@ struct urf_ctx {
                                        // scratch (buf.sortbuf) takes them, see ring_chunk
     HostMem<int> h_n; HostMem<ScanOut> h_out;   // pinned copies of n and out
     Event ev0, ev1, ev_done;           // bracket the batch's kernels; after its last copy to the host
-    // the batch in flight
-    int batch = 0, S = 0, launches = 0;
+    // the batch in flight; gen and C are the parameter generation and `channels` it was enqueued with (urf_set_params_next
+    // may change the context's while it runs)
+    int batch = 0, S = 0, launches = 0, C = 0;
+    int32_t gen = 0;
     urf_result* outs = nullptr;
     urf_clouds* clouds = nullptr;
   };
@@ -87,14 +89,16 @@ struct urf_ctx {
   int tie_order = URF_TIES_INPUT_ORDER;   // urf_set_tie_order; the reference order's buffers (buf.epos, buf.lomuto) are
                                           // allocated by the first switch to it
   urf_params params{};
-  DevParams dp{};
+  DevParams dp{};                      // copied by value into every launch: a batch keeps the parameters it was enqueued with
+  int32_t gen = 0;                     // parameter generation (urf_set_params_next); 0 until the first one
+  int32_t dev_gen = 0;                 // generation of the device-resident batch (urf_enqueue_batch_device*)
   // asynchronous enqueues stage their point counts in a ring of pinned rows, each guarded by the event of its H2D copy,
   // so back-to-back enqueues with different counts never overwrite a row whose copy has not run yet
   static constexpr int kNRing = 8;
   HostMem<int> h_nring;                // [kNRing][max_batch]
   Event ev_nring[kNRing];
   int nring_pos = 0;
-  int last_B = 0, last_S = 0;
+  int last_B = 0, last_S = 0, last_C = 0;   // scans, stride and channels of the last finished call (urf_debug_fetch)
   int launches = 0;
   float last_ms = 0.f;                 // device ms of the last finished host batch (timing_host)
   bool timing_valid = false, timing_host = false;
@@ -282,10 +286,10 @@ int update_graph(urf_ctx* ctx, int B, int S, bool want_order) {
   return URF_OK;
 }
 
-// with_ring_start = false leaves the caller's ring_start untouched
-void fill_result(const ScanOut& o, urf_result* r, bool with_ring_start) {
+// with_ring_start = false leaves the caller's ring_start untouched; gen: the parameter generation the scan ran with
+void fill_result(const ScanOut& o, urf_result* r, bool with_ring_start, int32_t gen) {
   r->n_in = o.n_in; r->n_roi = o.n_roi;
-  r->flags = o.flags & F_PUBLIC_MASK; r->reserved = 0;
+  r->flags = o.flags & F_PUBLIC_MASK; r->params_gen = gen;
   if (o.n_roi < 30) {                       // lidar_segmentation.cpp:124-126
     r->status = URF_TOO_FEW_POINTS;
     r->n_rings = 0; r->n_order = 0; r->n_road = 0; r->n_curb = 0; r->n_vert = 0;
@@ -406,6 +410,7 @@ int urf_create(urf_ctx** out, int device, int max_points, int max_batch) {
   urf_default_params(&ctx->params);
   const char* fe = std::getenv("URF_FORCE_EXACT_REGISTRATION");
   narrow_params(&ctx->params, &ctx->dp, ctx->dp.Kfi, fe && fe[0] == '1', 0);
+  ctx->last_C = ctx->dp.channels;
   ctx->dp.star_prefix = 1;                                  // near-first star sort (option 4 turns it off)
   ctx->dp.star_pivot = 17;
 #undef TRY
@@ -437,6 +442,20 @@ int urf_set_params(urf_ctx* ctx, const urf_params* p) {
   narrow_params(p, &ctx->dp, ctx->dp.Kfi, ctx->dp.force_exact, 0);
   ctx->version++;
   return URF_OK;
+}
+
+// Nothing between an enqueue and its finish reads ctx->params or ctx->dp: launch_pipeline copies dp into the kernels'
+// arguments, the strides of the batch's copies are fixed at the enqueue, and what the finish needs is in its HostSlot. A
+// changed set bumps `version`, so the next graphed batch re-captures; that can only be a slot-0 batch, whose previous graph
+// launch was finished with slot 0's last batch, so the old executable graph is no longer running when it is replaced.
+int urf_set_params_next(urf_ctx* ctx, const urf_params* p) {
+  if (!ctx || !p) return URF_ERR_INVALID;
+  const int rc = validate_params(p);
+  if (rc != URF_OK) return rc;
+  ctx->params = *p;
+  narrow_params(p, &ctx->dp, ctx->dp.Kfi, ctx->dp.force_exact, 0);
+  ctx->version++;
+  return ++ctx->gen;
 }
 
 int urf_get_params(const urf_ctx* ctx, urf_params* p) {
@@ -585,7 +604,8 @@ int urf_enqueue_batch_device_ex(urf_ctx* ctx, const float* d_xyzi, int stride_po
   ctx->launches = launches;
   ctx->timing_valid = true;
   ctx->timing_host = false;
-  ctx->last_B = batch; ctx->last_S = stride_points;
+  ctx->last_B = batch; ctx->last_S = stride_points; ctx->last_C = ctx->dp.channels;
+  ctx->dev_gen = ctx->gen;
   return URF_OK;
 }
 
@@ -600,7 +620,7 @@ int urf_finish_batch_device(urf_ctx* ctx, urf_result* outs) {
   ScanOut* h_out = ctx->hs[0].h_out.get();
   if (outs) CK(cudaMemcpyAsync(h_out, ctx->buf.out, sizeof(ScanOut) * B, cudaMemcpyDeviceToHost, ctx->stream.get()));
   CK(cudaStreamSynchronize(ctx->stream.get()));
-  if (outs) for (int b = 0; b < B; b++) fill_result(h_out[b], &outs[b], false);
+  if (outs) for (int b = 0; b < B; b++) fill_result(h_out[b], &outs[b], false, ctx->dev_gen);
   return URF_OK;
 }
 
@@ -749,6 +769,7 @@ int enqueue_batch(urf_ctx* ctx, const void* const* data, const int* n, int batch
   // s_out waited for the last chunk's kernels: ev_done covers every copy and kernel of the batch
   CK(cudaEventRecord(h.ev_done.get(), ctx->s_out.get()));
   h.batch = batch; h.S = S; h.launches = launches; h.outs = outs; h.clouds = clouds;
+  h.C = ctx->dp.channels; h.gen = ctx->gen;
   ctx->hs_count++;
   return URF_OK;
 }
@@ -781,10 +802,10 @@ int finish_batch(urf_ctx* ctx) {
   ctx->launches = h.launches;
   ctx->timing_valid = true;
   ctx->timing_host = true;
-  ctx->last_B = h.batch; ctx->last_S = h.S;
+  ctx->last_B = h.batch; ctx->last_S = h.S; ctx->last_C = h.C;
   urf_result* outs = h.outs;
   for (int b = 0; b < h.batch; b++) {
-    fill_result(h.h_out.get()[b], &outs[b], true);
+    fill_result(h.h_out.get()[b], &outs[b], true, h.gen);
     if (outs[b].status == URF_TOO_FEW_POINTS && outs[b].ring) for (int i = 0; i < h.h_n.get()[b]; i++) outs[b].ring[i] = -1;
   }
   return URF_OK;
@@ -895,7 +916,7 @@ int urf_debug_fetch(urf_ctx* ctx, int b, int what, void* dst, size_t bytes) {
   if (!ctx || !dst || b < 0 || b >= ctx->last_B) return URF_ERR_INVALID;
   CK(cudaSetDevice(ctx->device));
   CK(cudaStreamSynchronize(ctx->stream.get()));
-  const DevBuffers v = scan_view(ctx->buf, b, launch_extent(ctx->last_S, ctx->dp.channels));
+  const DevBuffers v = scan_view(ctx->buf, b, launch_extent(ctx->last_S, ctx->last_C));
   const void* src = nullptr;
   auto clamp = [&](size_t most) { if (bytes > most) bytes = most; };
   switch (what) {
@@ -904,7 +925,7 @@ int urf_debug_fetch(urf_ctx* ctx, int b, int what, void* dst, size_t bytes) {
     case 8: src = v.tab; clamp(sizeof(ScanTab)); break;
     case 9: src = &v.tab->nbig; clamp(2 * sizeof(int)); break;
     case 10: src = &v.tab->nrefine; clamp(sizeof(int)); break;
-    case 11: case 12: src = what == 11 ? v.Tf : v.Tb; clamp(sizeof(float) * ctx->dp.channels * kDegBins); break;
+    case 11: case 12: src = what == 11 ? v.Tf : v.Tb; clamp(sizeof(float) * ctx->last_C * kDegBins); break;
     case 13: src = v.firstidx; clamp(sizeof(unsigned) * kElevSlice); break;
     default: return URF_ERR_INVALID;
   }

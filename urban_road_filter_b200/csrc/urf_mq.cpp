@@ -16,6 +16,10 @@
 // Delivery (take_front_run, behind urf_mq_next / _next_view / _next_batch) cuts the front of that FIFO at the first scan
 // that is not done yet: every device queue involved reports how many of its oldest scans are done, and then lends exactly
 // the ones before the cut.
+//
+// Parameter updates (urf_mq_update_params) take every device's submit mutex, in device order, and then give each device
+// queue the mq's next generation. No scan can then be between its queue's acceptance and its entry in `order`, so the
+// update falls at one point of the global order on every device at once.
 #include <algorithm>
 #include <cstring>
 #include <deque>
@@ -23,6 +27,7 @@
 #include <vector>
 
 #include "../../include/urf.h"
+#include "urf_params.hpp"
 #include "urf_queue_internal.hpp"
 
 struct urf_mq {
@@ -43,6 +48,7 @@ struct urf_mq {
   int submitting = 0;                // submit calls between device choice and order append
   bool closed = false;
   bool label8 = false;               // int8 label slots on every device (urf_mq_create_label8)
+  int32_t gen = 0;                   // last parameter generation; changed only with every device's submit_mu held
   // Scratch of take_front_run. The header allows ONE consumer thread, so it needs no lock.
   std::vector<int> ds;               // devices of the first scans in the global order (a snapshot of `order`'s front)
   std::vector<int> want, done, used; // per device: its entries in ds / how many of them are done (-1: not asked yet) /
@@ -197,6 +203,30 @@ int urf_mq_create_with_label8(urf_mq** out, urf_queue_process_fn fn, void* const
 int urf_mq_set_params(urf_mq* m, const urf_params* p) {
   if (!m || !p) return URF_ERR_INVALID;
   return urf_internal::mq_apply_idle(m, [](urf_ctx* c, const void* q) { return urf_set_params(c, static_cast<const urf_params*>(q)); }, p);
+}
+
+int urf_mq_update_params(urf_mq* m, const urf_params* p) {
+  if (!m || !p || urf::validate_params(p) != URF_OK) return URF_ERR_INVALID;
+  std::vector<std::unique_lock<std::mutex>> held;         // device order: two updates cannot each hold what the other waits for
+  held.reserve(m->dev.size());
+  for (urf_mq::Dev& d : m->dev) held.emplace_back(d.submit_mu);
+  {
+    std::lock_guard<std::mutex> lk(m->mu);
+    if (m->closed) return URF_ERR_CLOSED;
+  }
+  const int32_t g = ++m->gen;
+  for (urf_mq::Dev& d : m->dev) {
+    const int rc = urf_internal::queue_update_params(d.q, p, g);
+    if (rc < 0) return rc;                                // closed meanwhile: no scan is accepted any more anyway
+  }
+  return g;
+}
+
+int urf_mq_set_params_hook(urf_mq* m, urf_queue_params_fn fn) {
+  if (!m) return URF_ERR_INVALID;
+  for (urf_mq::Dev& d : m->dev) if (d.ctx) return URF_ERR_INVALID;
+  for (urf_mq::Dev& d : m->dev) urf_queue_set_params_hook(d.q, fn);
+  return URF_OK;
 }
 
 int urf_mq_submit(urf_mq* m, const float* xyzi, int n, uint64_t tag, int timeout_ms) { return submit_common(m, xyzi, n, tag, timeout_ms, false); }

@@ -19,16 +19,23 @@
 // urf_finish_batch): it enqueues what is pending, enqueues the next pending run too if there is one, and only then waits
 // for the oldest batch, so the copies of one batch overlap the kernels of the other and the device does not wait for the
 // host's round trip between batches. A synchronous stand-in (urf_queue_create_with) is the same loop at depth 1.
+//
+// Parameter generations (urf_queue_update_params): a scan is stamped with the queue's generation when it becomes PENDING,
+// under the same lock that gives it its sequence number. Generations therefore never decrease along the sequence numbers,
+// a run taken oldest-first ends at the first scan of another generation, and the worker applies a run's set to the context
+// just before it enqueues the run. `sets` holds the set of each generation a pending scan or the next submit may carry.
 #include <algorithm>
 #include <cstddef>
 #include <cstdlib>
 #include <cstring>
 #include <deque>
+#include <map>
 #include <mutex>
 #include <thread>
 #include <vector>
 
 #include "../../include/urf.h"
+#include "urf_params.hpp"
 #include "urf_queue_internal.hpp"
 
 namespace {
@@ -36,6 +43,7 @@ enum SlotState { FREE = 0, FILLING, PENDING, RUNNING, DONE, VIEWED };   // VIEWE
 struct Slot {
   SlotState state = FREE;
   uint64_t seq = 0, tag = 0;
+  int32_t gen = 0;           // parameter generation in force when the scan became PENDING
   int n = 0, rc = URF_OK;
   float* in = nullptr;       // max_points * bytes_per_point bytes (pinned for the real queue)
   const float* ext = nullptr;   // urf_queue_submit_ref: the caller's buffer is used in place (no copy)
@@ -50,6 +58,7 @@ struct urf_queue {
   urf_queue_process_fn enq = nullptr;      // stand-in: with fin the asynchronous pair (urf_queue_create_with_async), alone
   urf_queue_finish_fn fin = nullptr;       // the synchronous batch function (urf_queue_create_with), which does it all
   void* user = nullptr;
+  urf_queue_params_fn params_fn = nullptr;   // stand-in: called where a real queue's worker calls urf_set_params_next
   bool pinned = false;
   int max_points = 0, max_batch = 1, policy = URF_QUEUE_BLOCK;
   int depth = 2;               // batches the worker keeps in flight: 2, or 1 around a synchronous stand-in
@@ -62,6 +71,8 @@ struct urf_queue {
   std::mutex mu;
   std::condition_variable cv_free, cv_pending, cv_done;
   uint64_t next_seq = 1;       // sequence number of the next accepted scan
+  int32_t gen = 0;             // generation stamped on the next accepted scan
+  std::map<int32_t, urf_params> sets;   // generation -> set, from the oldest one a PENDING scan carries up to `gen`
   // Consumer side. The header allows one consumer at a time, so only that thread changes `lent`, and it may read it
   // outside the lock: after a delivery call `lent` is exactly the run that call took, in submission order.
   std::vector<int> lent;       // slots lent out by the last delivery call, given back on the consumer's next call
@@ -78,6 +89,10 @@ using urf_internal::wait_for;
 // One batch of the worker: the slots it took and the arguments of its batch call (which must outlive an asynchronous
 // batch until its finish).
 struct Run {
+  int32_t gen = 0;             // the generation of every scan of the run
+  bool apply = false;          // gen differs from the last one the worker applied: `set` goes to the ctx (or hook) first
+  urf_params set{};
+  urf_queue_params_fn params_fn = nullptr;
   std::vector<int> idx;
   std::vector<const float*> ptrs;
   std::vector<int> ns;
@@ -86,10 +101,19 @@ struct Run {
   int rc = URF_OK;             // synchronous stand-in: what the batch function returned, reported by finish_run
 };
 
-// Takes every pending scan, oldest first, up to max_batch, into r (the slots become RUNNING: from here on they count as
-// started and DROP_OLDEST no longer drops them). wait: first block until a scan is pending or the queue is closed.
+// Drops the sets no PENDING scan carries, except the current generation's (mu held). A RUNNING scan's set, if its run
+// still has to apply it, was copied into the run.
+void prune_sets(urf_queue* q) {
+  int32_t keep = q->gen;
+  for (const Slot& s : q->slots) if (s.state == PENDING) keep = std::min(keep, s.gen);
+  q->sets.erase(q->sets.begin(), q->sets.lower_bound(keep));
+}
+
+// Takes every pending scan of the oldest pending scan's generation, oldest first, up to max_batch, into r (the slots become
+// RUNNING: from here on they count as started and DROP_OLDEST no longer drops them). `applied`: the generation the worker
+// last applied; a run of another one carries its set. wait: first block until a scan is pending or the queue is closed.
 // Returns the number taken; *closed tells whether the queue was closed.
-int take_run(urf_queue* q, Run& r, bool wait, bool* closed) {
+int take_run(urf_queue* q, Run& r, int32_t applied, bool wait, bool* closed) {
   r.idx.clear();
   {
     std::unique_lock<std::mutex> lk(q->mu);
@@ -106,11 +130,19 @@ int take_run(urf_queue* q, Run& r, bool wait, bool* closed) {
         if (s.state == PENDING && (best < 0 || s.seq < q->slots[best].seq)) best = i;
       }
       if (best < 0 || (int)r.idx.size() >= q->max_batch) break;
+      if (r.idx.empty()) r.gen = q->slots[best].gen;
+      else if (q->slots[best].gen != r.gen) break;        // a batch never mixes generations
       q->slots[best].state = RUNNING;
       r.idx.push_back(best);
     }
     *closed = q->closed;
     if (r.idx.empty()) return 0;
+    // generation 0 has no stored set (it is what the ctx had): generations only grow, so a run of it never follows another
+    const auto it = q->sets.find(r.gen);
+    r.apply = r.gen != applied && it != q->sets.end();
+    if (r.apply) r.set = it->second;
+    r.params_fn = q->params_fn;
+    prune_sets(q);
     q->st.batches++;
     if ((int)r.idx.size() > q->st.largest_batch) q->st.largest_batch = (int)r.idx.size();
   }
@@ -136,11 +168,27 @@ void complete_run(urf_queue* q, const Run& r, int rc) {
     std::lock_guard<std::mutex> lk(q->mu);
     for (size_t j = 0; j < r.idx.size(); j++) {
       Slot& s = q->slots[r.idx[j]];
-      s.res = r.outs[j]; s.rc = rc; s.state = DONE;
+      s.res = r.outs[j]; s.res.params_gen = r.gen;        // the queue's numbering, not the context's
+      s.rc = rc; s.state = DONE;
       q->st.processed++;
     }
   }
   q->cv_done.notify_all();
+}
+
+// Applies run r's set, if it carries one, to the context (its batches already enqueued keep theirs) or the stand-in's hook,
+// and records the generation in *applied. A failure fails the run like a refused enqueue.
+int apply_run(urf_queue* q, const Run& r, int32_t* applied) {
+  if (!r.apply) return URF_OK;
+  int rc = URF_OK;
+  if (q->ctx) {
+    rc = urf_set_params_next(q->ctx, &r.set);
+    if (rc > 0) rc = URF_OK;                              // the context's own generation number
+  } else if (r.params_fn) {
+    rc = r.params_fn(q->user, &r.set, r.gen);
+  }
+  if (rc == URF_OK) *applied = r.gen;
+  return rc;
 }
 
 // Starts run r. A synchronous stand-in does all its work here, and that counts as accepted: finish_run reports how it went.
@@ -168,15 +216,17 @@ int finish_run(urf_queue* q, const Run& r) { return q->ctx ? urf_finish_batch(q-
 // before a close before the worker returns.
 void worker_loop(urf_queue* q) {
   std::deque<Run> flight;                                 // enqueued, oldest first (at most q->depth)
+  int32_t applied = 0;                                    // generation of the parameters the last enqueued run used
   for (;;) {
     while ((int)flight.size() < q->depth) {
       Run r;
       bool closed = false;
-      if (!take_run(q, r, flight.empty(), &closed)) {
+      if (!take_run(q, r, applied, flight.empty(), &closed)) {
         if (flight.empty() && closed) return;
         break;
       }
-      const int rc = enqueue_run(q, r);
+      int rc = apply_run(q, r, &applied);
+      if (rc == URF_OK) rc = enqueue_run(q, r);
       if (rc != URF_OK) { complete_run(q, r, rc); continue; }   // nothing of a refused batch is in flight
       flight.push_back(std::move(r));                     // the vectors' storage, which the batch points at, moves along
       std::lock_guard<std::mutex> lk(q->mu);
@@ -294,7 +344,7 @@ int submit_common(urf_queue* q, const void* data, int n, uint64_t tag, int timeo
       closed_late = true;
     } else {
       s.n = n; s.tag = tag; s.rc = URF_OK;
-      s.seq = q->next_seq++;
+      s.seq = q->next_seq++; s.gen = q->gen;
       s.state = PENDING;
       q->st.submitted++;
     }
@@ -325,6 +375,18 @@ int urf_queue_submit_ref(urf_queue* q, const float* xyzi, int n, uint64_t tag, i
 int urf_queue_submit_cloud2(urf_queue* q, const void* data, int n_points, uint64_t tag, int timeout_ms) {
   if (q && q->step == 0) return URF_ERR_INVALID;
   return submit_common(q, data, n_points, tag, timeout_ms, false);
+}
+
+int urf_queue_update_params(urf_queue* q, const urf_params* p) {
+  if (!q || !p || urf::validate_params(p) != URF_OK) return URF_ERR_INVALID;
+  return urf_internal::queue_update_params(q, p, 0);
+}
+
+int urf_queue_set_params_hook(urf_queue* q, urf_queue_params_fn fn) {
+  if (!q || q->ctx) return URF_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(q->mu);
+  q->params_fn = fn;
+  return URF_OK;
 }
 
 namespace {
@@ -485,6 +547,15 @@ int queue_lend_run(urf_queue* q, int count, const int* dst, uint64_t* tags, int3
   }
   hand_out(q, dst, tags, rcs, outs, label_views);
   return (int)q->lent.size();
+}
+
+int queue_update_params(urf_queue* q, const urf_params* p, int32_t gen) {
+  std::lock_guard<std::mutex> lk(q->mu);
+  if (q->closed) return URF_ERR_CLOSED;
+  q->gen = gen > 0 ? gen : q->gen + 1;
+  q->sets[q->gen] = *p;
+  prune_sets(q);
+  return q->gen;
 }
 
 void queue_copy_lent_labels(const urf_queue* q, int32_t* dst) {

@@ -34,6 +34,11 @@ int queue_lend_run(urf_queue* q, int count, const int* dst, uint64_t* tags, int3
 // from an int8 slot. Nothing is copied for a failed scan or with dst == NULL.
 void queue_copy_lent_labels(const urf_queue* q, int32_t* dst);
 
+// Makes p (already validated) the set of the queue's next parameter generation: `gen`, or with gen == 0 the queue's last
+// plus one. Every scan accepted from now on carries it. Returns the generation, or URF_ERR_CLOSED after urf_queue_close.
+// urf_mq passes its own numbers, so that a device queue's results report the mq's generations.
+int queue_update_params(urf_queue* q, const urf_params* p, int32_t gen);
+
 // Runs fn(ctx, arg) on the context of every device of the mq, in device order, while nothing is in flight (everything
 // submitted has been collected): URF_ERR_INVALID otherwise. Stops at the first error and returns it. Stand-in devices
 // (urf_mq_create_with) have no context and are skipped.

@@ -50,11 +50,17 @@ class UrfParams(C.Structure):
     ]
 
 
+class _ResultGen(C.Union):
+    """urf_result's anonymous union: `reserved` under its old name, `params_gen` the parameter generation."""
+    _fields_ = [("reserved", C.c_int32), ("params_gen", C.c_int32)]
+
+
 class UrfResult(C.Structure):
+    _anonymous_ = ("_gen",)
     _fields_ = [
         ("status", C.c_int32), ("n_in", C.c_int32), ("n_roi", C.c_int32), ("n_rings", C.c_int32),
         ("n_order", C.c_int32), ("n_road", C.c_int32), ("n_curb", C.c_int32), ("n_vert", C.c_int32),
-        ("flags", C.c_int32), ("reserved", C.c_int32),
+        ("flags", C.c_int32), ("_gen", _ResultGen),
         ("label", C.POINTER(C.c_int32)),
         ("ring", C.POINTER(C.c_int32)),
         ("order", C.POINTER(C.c_int32)),
@@ -100,6 +106,8 @@ URF_ERR_TIMEOUT, URF_ERR_CLOSED = -6, -7
 QUEUE_PROCESS_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.c_int, C.POINTER(UrfResult))
 # int (*)(void* user): finishes the oldest batch of an asynchronous stand-in (urf_queue_create_with_async)
 QUEUE_FINISH_FN = C.CFUNCTYPE(C.c_int, C.c_void_p)
+# int (*)(void* user, const urf_params* p, int32_t gen): a stand-in queue's parameter hook (urf_queue_set_params_hook)
+QUEUE_PARAMS_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(UrfParams), C.c_int32)
 
 
 # cfg/LidarFilters.cfg:10-84 defaults
