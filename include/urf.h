@@ -302,11 +302,22 @@ void urf_pinned_free(void* p);
  * anyone else until urf_queue_destroy returns; parameters of a running queue change through urf_queue_update_params.
  */
 typedef struct urf_queue urf_queue;
-/* policy of urf_queue_create*: BLOCK or DROP_OLDEST, optionally OR-ed with URF_QUEUE_LABEL8 — int8 label slots (max_points
- * bytes per slot instead of 4 * max_points; the worker fetches one-byte labels from the device, the int32 label copy is not
- * issued). On such a queue urf_queue_next widens the labels into the caller's int32 buffer, urf_queue_next_view returns
- * URF_ERR_INVALID (there is no int32 array to point at) and urf_queue_next_batch lends int8_t views. */
-enum { URF_QUEUE_BLOCK = 0, URF_QUEUE_DROP_OLDEST = 1, URF_QUEUE_LABEL8 = 2 };
+/* policy of urf_queue_create*: BLOCK or DROP_OLDEST, optionally OR-ed with URF_QUEUE_LABEL8 and/or URF_QUEUE_ORDER (any
+ * other bit: URF_ERR_INVALID).
+ *   URF_QUEUE_LABEL8 — int8 label slots (max_points bytes per slot instead of 4 * max_points; the worker fetches one-byte
+ *   labels from the device, the int32 label copy is not issued). On such a queue urf_queue_next widens the labels into the
+ *   caller's int32 buffer, urf_queue_next_view returns URF_ERR_INVALID (there is no int32 array to point at) and
+ *   urf_queue_next_batch lends int8_t views.
+ *   URF_QUEUE_ORDER — every scan also delivers its emission order and ring offsets (urf_result.order / ring_start), from
+ *   which a consumer rebuilds the road, curb and road_probably clouds in the reference's order. Each slot holds
+ *   int32 order[max_points] and int32 ring_start[URF_MAX_CHANNELS + 1] besides its labels: 4 bytes per point plus 1,028
+ *   bytes (pinned on a real queue, malloc'ed for a stand-in). The worker passes both to the batch call, so every batch runs
+ *   the per-ring azimuth sort and copies 4 bytes per input point more to the host. order and ring_start are bit for bit
+ *   what urf_process_batch (float4 queues) or urf_process_cloud2_batch (record queues) give for the same scan, under the
+ *   ctx's tie order and the parameter generation the scan ran with (channels may differ between generations: n_rings + 1
+ *   entries of ring_start are meaningful). For URF_TOO_FEW_POINTS, n_order == 0 and ring_start is all zeros.
+ *   Without the bit the worker passes NULL for both and every delivered order / ring_start pointer is NULL. */
+enum { URF_QUEUE_BLOCK = 0, URF_QUEUE_DROP_OLDEST = 1, URF_QUEUE_LABEL8 = 2, URF_QUEUE_ORDER = 4 };
 enum { URF_ERR_TIMEOUT = -6, URF_ERR_CLOSED = -7 };
 typedef struct urf_queue_stats {
   uint64_t submitted, processed, dropped, delivered, batches;
@@ -322,23 +333,30 @@ int urf_queue_create(urf_queue** out, urf_ctx* ctx, int max_points, int slots, i
  * slot is already being processed or waiting to be collected it waits like BLOCK. Results are ordered by the moment a
  * submit call finished copying (with one producer: submission order). */
 int urf_queue_submit(urf_queue* q, const float* xyzi, int n, uint64_t tag, int timeout_ms);
-/* Next result in submission order (dropped scans are skipped). out->label (n ints) may be NULL; ring / order /
- * ring_start are not produced by the queue. URF_ERR_TIMEOUT when nothing finished within timeout_ms (< 0: wait),
- * URF_ERR_CLOSED once the queue is closed and drained. A scan whose processing failed returns that error code. */
+/* Next result in submission order (dropped scans are skipped). out->label (n ints) may be NULL. With URF_QUEUE_ORDER,
+ * out->order (room for n ints) and out->ring_start (room for URF_MAX_CHANNELS + 1 ints) may be non-NULL on entry: they
+ * receive n_order and n_rings + 1 entries. The caller's label / order / ring_start pointers stay in *out. Without the bit
+ * order and ring_start are set to NULL; ring is never produced by the queue. URF_ERR_TIMEOUT when nothing finished within
+ * timeout_ms (< 0: wait), URF_ERR_CLOSED once the queue is closed and drained. A scan whose processing failed returns that
+ * error code. */
 int urf_queue_next(urf_queue* q, uint64_t* tag, urf_result* out, int timeout_ms);
 /* urf_queue_next without the copy of the labels: *label_view points at the n_in labels inside the queue's staging slot
  * (NULL for a failed scan); the slot stays reserved until the consumer's next urf_queue_next / _next_view call on this queue
- * or urf_queue_release_view. out->label is ignored. One consumer thread at a time may hold a view. */
+ * or urf_queue_release_view. out->label is ignored. With URF_QUEUE_ORDER out->order and out->ring_start point into the
+ * same slot, read-only and valid as long as the label view (NULL for a failed scan). One consumer thread at a time may
+ * hold a view. */
 int urf_queue_next_view(urf_queue* q, uint64_t* tag, urf_result* out, const int32_t** label_view, int timeout_ms);
 /* Batched delivery: one wake-up and one lock round for every scan that is ready, instead of one per scan. Waits up to
  * timeout_ms (< 0: forever) until the oldest live scan is done, then lends out the run of consecutive finished scans that
  * starts with it, in submission order, at most max_results of them (it never skips a scan that is not done yet; dropped
  * scans are skipped as by urf_queue_next). Returns how many it lent (>= 1), or URF_ERR_TIMEOUT / URF_ERR_CLOSED as
  * urf_queue_next. For scan j: tags[j], rcs[j] (URF_OK, or the error code of the batch the scan failed in), outs[j] (counts,
- * flags and the n_vert vertices; pointer members set to NULL) and label_views[j], which points at the n_in labels inside
- * the queue's slot — int8_t with URF_QUEUE_LABEL8, int32_t otherwise — or is NULL for a failed scan. tags, rcs and
- * label_views may be NULL. Every lent slot stays reserved until the consumer's next urf_queue_next* call on this queue or
- * urf_queue_release_view, so the views stay valid until then. */
+ * flags and the n_vert vertices; label and ring set to NULL; order and ring_start as below) and label_views[j], which
+ * points at the n_in labels inside the queue's slot — int8_t with URF_QUEUE_LABEL8, int32_t otherwise — or is NULL for a
+ * failed scan. With URF_QUEUE_ORDER outs[j].order (n_order entries) and outs[j].ring_start (n_rings + 1 entries) point
+ * into the same slot, read-only, NULL for a failed scan; without it they are NULL. tags, rcs and label_views may be NULL.
+ * Every lent slot stays reserved until the consumer's next urf_queue_next* call on this queue or urf_queue_release_view,
+ * so the views stay valid until then. */
 int urf_queue_next_batch(urf_queue* q, int max_results, uint64_t* tags, int32_t* rcs, urf_result* outs, const void** label_views,
                          int timeout_ms);
 /* Gives back every slot lent by urf_queue_next_view / urf_queue_next_batch. */
@@ -379,7 +397,8 @@ int urf_queue_update_params(urf_queue* q, const urf_params* p);
 
 /* Test hook: the same queue around a caller-supplied batch function with urf_process_batch's signature (`user` is passed
  * as its ctx argument) and malloc'ed instead of pinned staging — the queue mechanics can then be exercised without a GPU.
- * With URF_QUEUE_LABEL8 the function still writes int32 labels (outs[b].label); the queue narrows them into its int8 slots. */
+ * With URF_QUEUE_LABEL8 the function still writes int32 labels (outs[b].label); the queue narrows them into its int8 slots.
+ * With URF_QUEUE_ORDER outs[b].order / ring_start point into the slot, for the function to fill (and NULL without it). */
 typedef int (*urf_queue_process_fn)(void* user, const float* const* xyzi, const int* n, int batch, urf_result* outs);
 int urf_queue_create_with(urf_queue** out, urf_queue_process_fn fn, void* user, int max_points, int slots, int max_batch,
                           int policy);
@@ -428,6 +447,11 @@ int urf_mq_next_batch(urf_mq* mq, int max_results, uint64_t* tags, int32_t* rcs,
 /* urf_mq_create with int8 label slots on every device (URF_QUEUE_LABEL8; urf_mq_next_view then returns URF_ERR_INVALID). */
 int urf_mq_create_label8(urf_mq** out, const int* devices, int n_devices, int max_points, int slots_per_device, int max_batch,
                          const urf_params* params /* or NULL: cfg defaults */);
+/* urf_mq_create with the device queues' slot options: policy = URF_QUEUE_BLOCK, optionally OR-ed with URF_QUEUE_LABEL8
+ * and/or URF_QUEUE_ORDER (urf_mq_next / _next_view / _next_batch then deliver order and ring_start as urf_queue_next* do).
+ * URF_QUEUE_DROP_OLDEST and unknown bits return URF_ERR_INVALID: the mq has no drop policy. */
+int urf_mq_create_policy(urf_mq** out, const int* devices, int n_devices, int max_points, int slots_per_device, int max_batch,
+                         const urf_params* params /* or NULL: cfg defaults */, int policy);
 /* urf_queue_update_params over all devices, at one point of the global order: every scan before it in the delivery order
  * runs with the earlier sets, every scan after it with p. Returns the mq's generation (1, 2, ...), which the results of every
  * device report in params_gen. Waits while a producer is inside a submit call (the update takes every device's submit lock). */
@@ -440,6 +464,8 @@ int urf_mq_create_with(urf_mq** out, urf_queue_process_fn fn, void* const* users
                        int slots_per_device, int max_batch);
 int urf_mq_create_with_label8(urf_mq** out, urf_queue_process_fn fn, void* const* users, int n_devices, int max_points,
                               int slots_per_device, int max_batch);
+int urf_mq_create_with_policy(urf_mq** out, urf_queue_process_fn fn, void* const* users, int n_devices, int max_points,
+                              int slots_per_device, int max_batch, int policy);   /* policy as urf_mq_create_policy */
 /* Test hook: urf_queue_set_params_hook on every stand-in device (fn gets users[j] for device j). URF_ERR_INVALID on real devices. */
 int urf_mq_set_params_hook(urf_mq* mq, urf_queue_params_fn fn);
 

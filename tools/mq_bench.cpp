@@ -4,10 +4,11 @@
 // reference (scans already in pinned memory, no host copy). Prints one JSON line per mode: scans/s and the host-side
 // limiter it points at. Host tool: links liburf_b200.so, no CUDA code of its own.
 //   usage: mq_bench <scans.bin> <points per scan> <n_scans_in_file> <n_devices> <producers> <total scans> <slots> <max_batch>
-//          [full_roi channels interval [modes max_results]]
+//          [full_roi channels interval [modes max_results [order]]]
 // modes: comma-separated subset of 0 (copying submit), 1 (by reference), 2 (by reference, labels viewed in place with
 // urf_mq_next_view), 3 (by reference, int8 label slots, results taken with urf_mq_next_batch, up to max_results per call);
-// default 0,1,2.
+// default 0,1,2. order: 1 creates the device queues with URF_QUEUE_ORDER (every batch runs the ring sort and copies the
+// emission order back; mode 3 reads n_order of every view); default 0.
 #include <algorithm>
 #include <atomic>
 #include <chrono>
@@ -28,6 +29,7 @@ int main(int argc, char** argv) {
   std::vector<int> modes = {0, 1, 2};
   if (argc > 12) { modes.clear(); for (const char* c = argv[12]; *c; c++) if (*c >= '0' && *c <= '3') modes.push_back(*c - '0'); }
   const int max_results = argc > 13 ? atoi(argv[13]) : 64;
+  const bool order = argc > 14 && atoi(argv[14]) != 0;
   const size_t bytes = (size_t)n * 16;
   std::vector<float*> pinned(K);
   FILE* f = fopen(path, "rb");
@@ -48,10 +50,11 @@ int main(int argc, char** argv) {
   for (int mode : modes) {                                        // 0: copying submit, 1: by reference (pinned), 2: 1 + labels viewed in place,
                                                                   // 3: 1 + int8 slots delivered in runs (urf_mq_next_batch)
     urf_mq* mq = nullptr;
-    int rc = mode == 3 ? urf_mq_create_label8(&mq, devs.data(), D, n, slots, mb, &prm) : urf_mq_create(&mq, devs.data(), D, n, slots, mb, &prm);
+    const int policy = URF_QUEUE_BLOCK | (mode == 3 ? URF_QUEUE_LABEL8 : 0) | (order ? URF_QUEUE_ORDER : 0);
+    int rc = urf_mq_create_policy(&mq, devs.data(), D, n, slots, mb, &prm, policy);
     if (rc != URF_OK) { fprintf(stderr, "urf_mq_create: %s (%s)\n", urf_strerror(rc), urf_last_cuda_error(nullptr)); return 1; }
     std::vector<int32_t> lab(n);
-    std::atomic<long> road{0};
+    std::atomic<long> road{0}, ordered{0};
     auto run = [&](int count, bool timed) {
       std::vector<std::thread> prod;
       const auto t0 = std::chrono::steady_clock::now();
@@ -74,6 +77,8 @@ int main(int argc, char** argv) {
             for (int j = 0; j < k; j++) {
               if (rcs[j] != URF_OK) { fprintf(stderr, "next_batch: %s\n", urf_strerror(rcs[j])); exit(1); }
               if (timed) road += outs[j].n_road;
+              if (timed && outs[j].order && outs[j].ring_start && outs[j].n_order > 0)
+                ordered += outs[j].order[outs[j].n_order - 1] >= 0 ? outs[j].n_order : 0;
             }
             i += k;
           }
@@ -99,9 +104,10 @@ int main(int argc, char** argv) {
     int largest = 0; unsigned long long mn = ~0ull, mx = 0;
     for (int d = 0; d < D; d++) { largest = st.largest_batch[d] > largest ? st.largest_batch[d] : largest; mn = st.submitted[d] < mn ? st.submitted[d] : mn; mx = st.submitted[d] > mx ? st.submitted[d] : mx; }
     printf("{\"mq_bench\": \"%s\", \"devices\": %d, \"producers\": %d, \"points_per_scan\": %d, \"scans\": %d, \"seconds\": %.4f, \"scans_per_sec\": %.1f, "
-           "\"mpoints_per_sec\": %.1f, \"h2d_gb_per_sec\": %.2f, \"largest_batch\": %d, \"per_device_min_max\": [%llu, %llu], \"road_points\": %ld}\n",
+           "\"mpoints_per_sec\": %.1f, \"h2d_gb_per_sec\": %.2f, \"largest_batch\": %d, \"per_device_min_max\": [%llu, %llu], \"road_points\": %ld, "
+           "\"order\": %d, \"ordered_points\": %ld}\n",
            mode == 3 ? "by_reference_pinned_label8_next_batch" : mode == 2 ? "by_reference_pinned_labels_viewed_in_place" : mode ? "by_reference_pinned" : "copying_submit", D, P, n, total, s, total / s, total / s * n / 1e6, total / s * bytes / 1e9, largest, mn, mx,
-           road.load());
+           road.load(), (int)order, ordered.load());
     fflush(stdout);
     urf_mq_destroy(mq);
   }

@@ -11,7 +11,7 @@ import os
 import numpy as np
 
 from .ctypes_abi import (UrfMqStats, QUEUE_FINISH_FN, QUEUE_PARAMS_FN, QUEUE_PROCESS_FN, URF_ERR_CLOSED, URF_ERR_TIMEOUT, URF_MAX_CHANNELS, URF_MAX_VERTS, URF_OK, URF_QUEUE_BLOCK,
-                         URF_QUEUE_DROP_OLDEST, URF_QUEUE_LABEL8, URF_TOO_FEW_POINTS, UrfClouds, UrfParams, UrfQueueStats, UrfResult,
+                         URF_QUEUE_DROP_OLDEST, URF_QUEUE_LABEL8, URF_QUEUE_ORDER, URF_TOO_FEW_POINTS, UrfClouds, UrfParams, UrfQueueStats, UrfResult,
                          UrfStrip, make_params)
 
 LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "liburf_b200.so")
@@ -26,7 +26,7 @@ EXPORTS = ["urf_queue_next_batch", "urf_mq_next_batch", "urf_mq_create_label8", 
            "urf_last_launch_count", "urf_build_markers", "urf_set_tie_order", "urf_get_tie_order", "urf_mq_set_tie_order",
            "urf_enqueue_batch", "urf_enqueue_cloud2_batch", "urf_finish_batch", "urf_queue_create_with_async",
            "urf_set_params_next", "urf_queue_update_params", "urf_mq_update_params", "urf_queue_set_params_hook",
-           "urf_mq_set_params_hook"]
+           "urf_mq_set_params_hook", "urf_mq_create_policy", "urf_mq_create_with_policy"]
 
 # urf_set_tie_order modes (include/urf.h): equal azimuths inside a ring in input order, or in the reference's Lomuto order
 TIE_ORDERS = {"input": 0, "reference": 1}
@@ -115,6 +115,8 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
     lib.urf_mq_get_stats.argtypes = [vp, C.POINTER(UrfMqStats)]
     lib.urf_mq_create_label8.argtypes = [C.POINTER(vp), C.POINTER(ip), ip, ip, ip, ip, C.POINTER(UrfParams)]
     lib.urf_mq_create_with_label8.argtypes = [C.POINTER(vp), QUEUE_PROCESS_FN, C.POINTER(vp), ip, ip, ip, ip]
+    lib.urf_mq_create_policy.argtypes = [C.POINTER(vp), C.POINTER(ip), ip, ip, ip, ip, C.POINTER(UrfParams), ip]
+    lib.urf_mq_create_with_policy.argtypes = [C.POINTER(vp), QUEUE_PROCESS_FN, C.POINTER(vp), ip, ip, ip, ip, ip]
     batch_args = [vp, ip, C.POINTER(C.c_uint64), C.POINTER(C.c_int32), C.POINTER(UrfResult), C.POINTER(vp), ip]
     lib.urf_queue_next_batch.argtypes = batch_args
     lib.urf_queue_next_view.argtypes = [vp, C.POINTER(C.c_uint64), C.POINTER(UrfResult), C.POINTER(vp), ip]
@@ -461,6 +463,14 @@ class Detector:
         return a[:count]
 
 
+def _slot_ints(ptr, n: int, copy: bool) -> np.ndarray:
+    """The first n int32 of a lent slot's array: a view, or with `copy` a copy."""
+    if n <= 0:
+        return np.zeros(0, np.int32)
+    a = np.ctypeslib.as_array(ptr, shape=(n,))
+    return a.copy() if copy else a
+
+
 class _BatchBuffers:
     """Output arrays of urf_queue_next_batch / urf_mq_next_batch for up to `cap` scans, reused between calls."""
 
@@ -472,8 +482,9 @@ class _BatchBuffers:
         self.views = (C.c_void_p * cap)()
 
     def results(self, k: int, label8: bool, copy: bool) -> list:
-        """(tag, ScanResult) of the k scans handed out. Labels are numpy views of the lent slots (int8 or int32) unless
-        `copy`; a scan whose batch failed has status = its (negative) error code and label None."""
+        """(tag, ScanResult) of the k scans handed out. Labels, and the emission order and ring offsets of a queue that
+        delivers them, are numpy views of the lent slots (labels int8 or int32) unless `copy`; a scan whose batch failed has
+        status = its (negative) error code and label / order / ring_start None."""
         ct = C.c_int8 if label8 else C.c_int32
         out = []
         for j in range(k):
@@ -486,6 +497,9 @@ class _BatchBuffers:
                 if copy:
                     lab = lab.copy()
             r = _scan_result(res, lab)
+            if res.order:                                # URF_QUEUE_ORDER, and the scan did not fail
+                r.order = _slot_ints(res.order, r.n_order, copy)
+                r.ring_start = _slot_ints(res.ring_start, r.n_rings + 1, copy)
             if rc != URF_OK:
                 r.status = rc
             out.append((int(self.tags[j]), r))
@@ -498,11 +512,12 @@ class _StreamQueue:
     `_PREFIX` + name (urf_queue_* or urf_mq_*), which have the same arguments in both families."""
     _PREFIX = ""
 
-    def __init__(self, max_points: int, label8: bool, params: UrfParams | None = None):
+    def __init__(self, max_points: int, label8: bool, params: UrfParams | None = None, order: bool = False):
         self.lib = load_library()
         self._h = C.c_void_p()
         self.max_points = max_points
         self.label8 = label8
+        self.order = order                # URF_QUEUE_ORDER: results carry order and ring_start
         self._cb = None                   # ctypes callbacks of a stand-in, kept alive with the queue
         self._params_cb = None            # the parameter hook of a stand-in
         self._bufs = None
@@ -547,10 +562,16 @@ class _StreamQueue:
         return rc
 
     def next(self, timeout_ms: int = -1):
-        """(tag, ScanResult) of the oldest finished scan, or None on timeout / when the closed queue is drained."""
+        """(tag, ScanResult) of the oldest finished scan, or None on timeout / when the closed queue is drained. With
+        `order` the result's order and ring_start are copies of the scan's n_order / n_rings + 1 entries."""
         lab = np.full(self.max_points, -1, np.int32)
         res = UrfResult()
         res.label = lab.ctypes.data_as(C.POINTER(C.c_int32))
+        order = rs = None
+        if self.order:
+            order, rs = np.zeros(self.max_points, np.int32), np.zeros(URF_MAX_CHANNELS + 1, np.int32)
+            res.order = order.ctypes.data_as(C.POINTER(C.c_int32))
+            res.ring_start = rs.ctypes.data_as(C.POINTER(C.c_int32))
         tag = C.c_uint64()
         rc = self._call("next", C.byref(tag), C.byref(res), timeout_ms)
         if rc in (URF_ERR_TIMEOUT, URF_ERR_CLOSED):
@@ -558,13 +579,13 @@ class _StreamQueue:
         if rc != URF_OK:
             raise UrfError(rc, self._PREFIX + "next")
         self._keep.pop(tag.value, None)
-        return tag.value, _scan_result(res, lab[: res.n_in].copy())
+        return tag.value, _scan_result(res, lab[: res.n_in].copy(), order=order, ring_start=rs)
 
     def next_batch(self, max_results: int, timeout_ms: int = -1, copy: bool = False) -> list:
         """[(tag, ScanResult)] of the run of finished scans that starts with the oldest one (urf_queue_next_batch /
-        urf_mq_next_batch), at most max_results; [] on timeout / when the closed queue is drained. Labels are views of the
-        lent slots (int8 with label8), valid until the next next* call, unless `copy`. A scan whose batch failed has
-        status < 0 and label None."""
+        urf_mq_next_batch), at most max_results; [] on timeout / when the closed queue is drained. Labels (int8 with
+        label8), and with `order` the emission order and ring_start, are views of the lent slots, valid until the next
+        next* call, unless `copy`. A scan whose batch failed has status < 0 and label / order / ring_start None."""
         if max_results < 1:
             raise ValueError("max_results must be >= 1")
         if self._bufs is None or self._bufs.cap < max_results:
@@ -594,22 +615,23 @@ class MultiGpuQueue(_StreamQueue):
     """One ingest stream over several GPUs (include/urf.h urf_mq, BASELINE config 4): a context + streaming queue per device,
     every scan goes to the device with the fewest scans in flight, results come back in submission order. Any number of
     producer threads, one consumer. `by_reference` submits hand the array to the library without a copy: keep it alive and
-    unchanged until its result has come back. label8: int8 label slots on every device (see ScanQueue)."""
+    unchanged until its result has come back. label8: int8 label slots on every device, order: the emission order and ring
+    offsets with every result (see ScanQueue)."""
     _PREFIX = "urf_mq_"
     _m = property(lambda self: self._h)      # the library handle, under the name this class has always had for it
 
     def __init__(self, devices, max_points: int, slots_per_device: int = 8, max_batch: int = 4, params: UrfParams | None = None,
-                 process_fn=None, label8: bool = False):
-        super().__init__(max_points, label8, None if process_fn is not None else params if params is not None else make_params())
+                 process_fn=None, label8: bool = False, order: bool = False):
+        super().__init__(max_points, label8, None if process_fn is not None else params if params is not None else make_params(), order)
+        policy = URF_QUEUE_BLOCK | (URF_QUEUE_LABEL8 if label8 else 0) | (URF_QUEUE_ORDER if order else 0)
         if process_fn is not None:                      # tests: stand-in devices, no GPU
             self._cb = QUEUE_PROCESS_FN(process_fn)
-            create = self.lib.urf_mq_create_with_label8 if label8 else self.lib.urf_mq_create_with
-            rc = create(C.byref(self._h), self._cb, None, len(devices), max_points, slots_per_device, max_batch)
+            rc = self.lib.urf_mq_create_with_policy(C.byref(self._h), self._cb, None, len(devices), max_points, slots_per_device,
+                                                    max_batch, policy)
         else:
             dv = (C.c_int * len(devices))(*devices)
-            create = self.lib.urf_mq_create_label8 if label8 else self.lib.urf_mq_create
-            rc = create(C.byref(self._h), dv, len(devices), max_points, slots_per_device, max_batch,
-                        C.byref(params) if params is not None else None)
+            rc = self.lib.urf_mq_create_policy(C.byref(self._h), dv, len(devices), max_points, slots_per_device, max_batch,
+                                               C.byref(params) if params is not None else None, policy)
         if rc != URF_OK:
             raise UrfError(rc, "urf_mq_create", self.lib.urf_last_cuda_error(None).decode())
 
@@ -640,15 +662,21 @@ class ScanQueue(_StreamQueue):
     every result that is ready at once. With `process_fn` (a Python callable with urf_process_batch's arguments) the queue
     runs without a GPU — tests only; with `enqueue_fn` and `finish_fn` instead (urf_enqueue_batch's arguments / none) it
     runs the real queue's two-batches-in-flight schedule around them. label8: int8 label slots (URF_QUEUE_LABEL8) — a
-    quarter of the label traffic and memory; `next` still returns int32 labels, `next_batch` int8 ones."""
+    quarter of the label traffic and memory; `next` still returns int32 labels, `next_batch` int8 ones. order
+    (URF_QUEUE_ORDER): every result also carries its emission order and ring_start, so that cloud_indices("road" | "curb" |
+    "road_probably") works on it; the batches then run the ring sort and copy 4 bytes per point more."""
     _PREFIX = "urf_queue_"
     _q = property(lambda self: self._h)      # the library handle, under the name this class has always had for it
 
     def __init__(self, detector: "Detector | None", max_points: int, slots: int = 8, max_batch: int = 4,
-                 policy: int = URF_QUEUE_BLOCK, process_fn=None, label8: bool = False, enqueue_fn=None, finish_fn=None):
-        super().__init__(max_points, label8, detector.params if detector is not None else None)
+                 policy: int = URF_QUEUE_BLOCK, process_fn=None, label8: bool = False, enqueue_fn=None, finish_fn=None,
+                 order: bool = False):
+        order = order or bool(policy & URF_QUEUE_ORDER)
+        super().__init__(max_points, label8, detector.params if detector is not None else None, order)
         if label8:
             policy |= URF_QUEUE_LABEL8
+        if order:
+            policy |= URF_QUEUE_ORDER
         if enqueue_fn is not None:
             self._cb = (QUEUE_PROCESS_FN(enqueue_fn), QUEUE_FINISH_FN(lambda user: finish_fn()))
             rc = self.lib.urf_queue_create_with_async(C.byref(self._h), *self._cb, None, max_points, slots, max_batch, policy)

@@ -94,10 +94,14 @@ int submit_common(urf_mq* m, const float* xyzi, int n, uint64_t tag, int timeout
 }
 
 // fn == NULL: a context (with `params`, if given) and a pinned queue on each of `devices`; otherwise stand-in devices
-// around fn, which gets users[j] for device j. The first device that cannot be made ends the attempt.
+// around fn, which gets users[j] for device j. Every device queue gets `policy`. The first device that cannot be made ends
+// the attempt.
 int create(urf_mq** out, const int* devices, urf_queue_process_fn fn, void* const* users, int n_devices, int max_points,
            int slots_per_device, int max_batch, const urf_params* params, int policy) {
-  if (!out || (!devices && !fn) || n_devices < 1 || max_points < 1 || slots_per_device < 1 || max_batch < 1) return URF_ERR_INVALID;
+  // BLOCK with the slot options only: the mq has no drop policy
+  if (!out || (!devices && !fn) || n_devices < 1 || max_points < 1 || slots_per_device < 1 || max_batch < 1 ||
+      (policy & ~(URF_QUEUE_LABEL8 | URF_QUEUE_ORDER)) != URF_QUEUE_BLOCK)
+    return URF_ERR_INVALID;
   *out = nullptr;
   urf_mq* m = new urf_mq;
   m->label8 = (policy & URF_QUEUE_LABEL8) != 0;
@@ -200,6 +204,16 @@ int urf_mq_create_with_label8(urf_mq** out, urf_queue_process_fn fn, void* const
   return create(out, nullptr, fn, users, n_devices, max_points, slots_per_device, max_batch, nullptr, URF_QUEUE_BLOCK | URF_QUEUE_LABEL8);
 }
 
+int urf_mq_create_policy(urf_mq** out, const int* devices, int n_devices, int max_points, int slots_per_device, int max_batch,
+                         const urf_params* params, int policy) {
+  return create(out, devices, nullptr, nullptr, n_devices, max_points, slots_per_device, max_batch, params, policy);
+}
+
+int urf_mq_create_with_policy(urf_mq** out, urf_queue_process_fn fn, void* const* users, int n_devices, int max_points,
+                              int slots_per_device, int max_batch, int policy) {
+  return create(out, nullptr, fn, users, n_devices, max_points, slots_per_device, max_batch, nullptr, policy);
+}
+
 int urf_mq_set_params(urf_mq* m, const urf_params* p) {
   if (!m || !p) return URF_ERR_INVALID;
   return urf_internal::mq_apply_idle(m, [](urf_ctx* c, const void* q) { return urf_set_params(c, static_cast<const urf_params*>(q)); }, p);
@@ -250,13 +264,12 @@ int urf_mq_next_view(urf_mq* m, uint64_t* tag, urf_result* out, const int32_t** 
 
 int urf_mq_next(urf_mq* m, uint64_t* tag, urf_result* out, int timeout_ms) {
   if (!m || !out) return URF_ERR_INVALID;
-  int32_t* user_label = out->label;
+  int32_t* const label = out->label, * const order = out->order, * const ring_start = out->ring_start;   // the caller's
   int32_t rc = URF_OK;
   const int k = take_front_run(m, 1, tag, &rc, out, nullptr, timeout_ms);
   if (k < 0) return k;
-  out->label = user_label;
   const int d = m->ds[0];
-  urf_internal::queue_copy_lent_labels(m->dev[d].q, user_label);
+  urf_internal::queue_copy_lent(m->dev[d].q, label, order, ring_start, out);
   urf_queue_release_view(m->dev[d].q);                    // nothing stays lent: the slot goes back to the producers at once
   m->used[d] = 0;
   return rc;

@@ -13,7 +13,9 @@
 //
 // Label slots are int32, or int8 with URF_QUEUE_LABEL8: the worker then asks the batch body for one-byte labels (float4
 // queues go through urf_enqueue_cloud2_batch with 16-byte records, as the synchronous path went through
-// urf_process_cloud2_batch).
+// urf_process_cloud2_batch). With URF_QUEUE_ORDER a slot also holds the scan's emission order and ring_start: the worker
+// points the batch call's outs at them, the batch body fills them as it does for any caller, and delivery lends them with
+// the labels.
 //
 // The worker is one loop with a depth. On a real context it keeps two batches in flight (urf_enqueue_batch /
 // urf_finish_batch): it enqueues what is pending, enqueues the next pending run too if there is one, and only then waits
@@ -49,6 +51,8 @@ struct Slot {
   const float* ext = nullptr;   // urf_queue_submit_ref: the caller's buffer is used in place (no copy)
   int32_t* label = nullptr;  // max_points; NULL in a real URF_QUEUE_LABEL8 queue
   int8_t* label8 = nullptr;  // max_points, URF_QUEUE_LABEL8 only
+  int32_t* order = nullptr;       // max_points, URF_QUEUE_ORDER only: the emission order
+  int32_t* ring_start = nullptr;  // URF_MAX_CHANNELS + 1, URF_QUEUE_ORDER only
   urf_result res{};
 };
 }  // namespace
@@ -63,6 +67,7 @@ struct urf_queue {
   int max_points = 0, max_batch = 1, policy = URF_QUEUE_BLOCK;
   int depth = 2;               // batches the worker keeps in flight: 2, or 1 around a synchronous stand-in
   bool label8 = false;         // URF_QUEUE_LABEL8: int8 label slots
+  bool order = false;          // URF_QUEUE_ORDER: every slot also holds the scan's emission order and ring offsets
   // record format of the scans: step == 0: (x, y, z, intensity) float4 points; step > 0: raw PointCloud2 records of `step`
   // bytes (urf_queue_create_cloud2), handed to urf_process_cloud2_batch and unpacked on the device
   int step = 0, ox = 0, oy = 4, oz = 8, oi = -1;
@@ -152,6 +157,7 @@ int take_run(urf_queue* q, Run& r, int32_t applied, bool wait, bool* closed) {
     const Slot& s = q->slots[r.idx[j]];
     r.ptrs[j] = s.ext ? s.ext : s.in; r.ns[j] = s.n;
     r.outs[j].label = s.label;                            // NULL in a real int8 queue: no int32 label copy is issued
+    r.outs[j].order = s.order; r.outs[j].ring_start = s.ring_start;   // NULL without URF_QUEUE_ORDER: no ring sort, no copy
     r.l8[j] = s.label8;
   }
   return B;
@@ -239,17 +245,17 @@ void worker_loop(urf_queue* q) {
 }
 
 void free_slot(const urf_queue* q, Slot& s) {
-  for (void* p : {(void*)s.in, (void*)s.label, (void*)s.label8}) {
+  for (void* p : {(void*)s.in, (void*)s.label, (void*)s.label8, (void*)s.order, (void*)s.ring_start}) {
     if (q->pinned) urf_pinned_free(p); else std::free(p);
   }
-  s.in = nullptr; s.label = nullptr; s.label8 = nullptr;
+  s.in = nullptr; s.label = nullptr; s.label8 = nullptr; s.order = nullptr; s.ring_start = nullptr;
 }
 
 // Either ctx (real queue, pinned slots) or enq (stand-in; synchronous, and the worker's depth 1, without fin) is set.
 int create_common(urf_queue** out, urf_ctx* ctx, urf_queue_process_fn enq, urf_queue_finish_fn fin, void* user,
                   int max_points, int slots, int max_batch, int policy, int step = 0, int ox = 0, int oy = 4, int oz = 8, int oi = -1) {
-  const bool label8 = (policy & URF_QUEUE_LABEL8) != 0;
-  policy &= ~URF_QUEUE_LABEL8;
+  const bool label8 = (policy & URF_QUEUE_LABEL8) != 0, order = (policy & URF_QUEUE_ORDER) != 0;
+  policy &= ~(URF_QUEUE_LABEL8 | URF_QUEUE_ORDER);
   if (!out || (!ctx && !enq) || max_points < 1 || slots < 1 || max_batch < 1 ||
       (policy != URF_QUEUE_BLOCK && policy != URF_QUEUE_DROP_OLDEST))
     return URF_ERR_INVALID;
@@ -257,7 +263,7 @@ int create_common(urf_queue** out, urf_ctx* ctx, urf_queue_process_fn enq, urf_q
   urf_queue* q = new urf_queue;
   q->ctx = ctx; q->enq = enq; q->fin = fin; q->user = user;
   q->pinned = pinned; q->max_points = max_points; q->max_batch = max_batch; q->policy = policy;
-  q->label8 = label8; q->depth = ctx || fin ? 2 : 1;
+  q->label8 = label8; q->order = order; q->depth = ctx || fin ? 2 : 1;
   q->step = step; q->ox = ox; q->oy = oy; q->oz = oz; q->oi = oi;
   q->bytes_per_point = step > 0 ? (size_t)step : 16;
   q->slots.resize(slots); q->lent.reserve(slots); q->live.reserve(slots);
@@ -269,7 +275,11 @@ int create_common(urf_queue** out, urf_ctx* ctx, urf_queue_process_fn enq, urf_q
     s.in = static_cast<float*>(alloc(in_bytes));
     if (want32) s.label = static_cast<int32_t*>(alloc(sizeof(int32_t) * (size_t)max_points));
     if (want8) s.label8 = static_cast<int8_t*>(alloc((size_t)max_points));
-    if (!s.in || (want32 && !s.label) || (want8 && !s.label8)) {
+    if (order) {
+      s.order = static_cast<int32_t*>(alloc(sizeof(int32_t) * (size_t)max_points));
+      s.ring_start = static_cast<int32_t*>(alloc(sizeof(int32_t) * (URF_MAX_CHANNELS + 1)));
+    }
+    if (!s.in || (want32 && !s.label) || (want8 && !s.label8) || (order && (!s.order || !s.ring_start))) {
       for (Slot& t : q->slots) free_slot(q, t);
       delete q;
       return URF_ERR_NOMEM;
@@ -450,7 +460,8 @@ void copy_result(urf_result* dst, const urf_result& src) {
   std::memcpy(dst->vert, src.vert, sizeof(src.vert[0]) * (size_t)nv);
 }
 
-// Hands out the slots of q->lent: the j-th goes to index dst ? dst[j] : j. Runs outside the lock (the slots are ours).
+// Hands out the slots of q->lent: the j-th goes to index dst ? dst[j] : j; with URF_QUEUE_ORDER the order and ring_start
+// of a scan that did not fail point into its slot. Runs outside the lock (the slots are ours).
 void hand_out(const urf_queue* q, const int* dst, uint64_t* tags, int32_t* rcs, urf_result* outs, const void** label_views) {
   for (int j = 0; j < (int)q->lent.size(); j++) {
     const Slot& s = q->slots[q->lent[j]];
@@ -458,6 +469,7 @@ void hand_out(const urf_queue* q, const int* dst, uint64_t* tags, int32_t* rcs, 
     if (tags) tags[o] = s.tag;
     if (rcs) rcs[o] = s.rc;
     copy_result(&outs[o], s.res);
+    if (q->order && s.rc == URF_OK) { outs[o].order = s.order; outs[o].ring_start = s.ring_start; }
     if (label_views) label_views[o] = s.rc != URF_OK ? nullptr : q->label8 ? (const void*)s.label8 : (const void*)s.label;
   }
 }
@@ -485,12 +497,11 @@ int urf_queue_next_view(urf_queue* q, uint64_t* tag, urf_result* out, const int3
 
 int urf_queue_next(urf_queue* q, uint64_t* tag, urf_result* out, int timeout_ms) {
   if (!q || !out) return URF_ERR_INVALID;
-  int32_t* user_label = out->label;
+  int32_t* const label = out->label, * const order = out->order, * const ring_start = out->ring_start;   // the caller's
   int32_t rc = URF_OK;
   const int k = urf_queue_next_batch(q, 1, tag, &rc, out, nullptr, timeout_ms);
   if (k < 0) return k;
-  out->label = user_label;
-  urf_internal::queue_copy_lent_labels(q, user_label);    // outside the lock
+  urf_internal::queue_copy_lent(q, label, order, ring_start, out);   // outside the lock
   urf_queue_release_view(q);                              // nothing stays lent: the slot goes back to the producers at once
   return rc;
 }
@@ -558,11 +569,18 @@ int queue_update_params(urf_queue* q, const urf_params* p, int32_t gen) {
   return q->gen;
 }
 
-void queue_copy_lent_labels(const urf_queue* q, int32_t* dst) {
+void queue_copy_lent(const urf_queue* q, int32_t* label, int32_t* order, int32_t* ring_start, urf_result* out) {
   const Slot& s = q->slots[q->lent.front()];
-  if (!dst || s.rc != URF_OK || s.n < 1) return;
-  if (q->label8) for (int i = 0; i < s.n; i++) dst[i] = s.label8[i];   // int8 slot: widened for the caller
-  else std::memcpy(dst, s.label, sizeof(int32_t) * (size_t)s.n);
+  out->label = label;
+  if (q->order) { out->order = order; out->ring_start = ring_start; }
+  if (s.rc != URF_OK) return;
+  if (label && s.n > 0) {
+    if (q->label8) for (int i = 0; i < s.n; i++) label[i] = s.label8[i];   // int8 slot: widened for the caller
+    else std::memcpy(label, s.label, sizeof(int32_t) * (size_t)s.n);
+  }
+  if (!q->order) return;
+  if (order && s.res.n_order > 0) std::memcpy(order, s.order, sizeof(int32_t) * (size_t)std::min(s.res.n_order, s.n));
+  if (ring_start) std::memcpy(ring_start, s.ring_start, sizeof(int32_t) * (size_t)(std::min(std::max(s.res.n_rings, 0), URF_MAX_CHANNELS) + 1));
 }
 
 }  // namespace urf_internal

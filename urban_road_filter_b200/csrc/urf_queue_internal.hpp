@@ -1,5 +1,5 @@
 // urf_queue_internal.hpp — what urf_queue.cpp and urf_mq.cpp share (host code, C++ linkage, not part of include/urf.h):
-// the timed wait, the two halves of a delivery call, which urf_mq needs separately, the copy of a lent scan's labels, and
+// the timed wait, the two halves of a delivery call, which urf_mq needs separately, the copy of a lent scan's labels and order, and
 // the idle rule of the mq's settings. urf_mq first asks every device queue how far its run of finished scans reaches, cuts
 // the global order at the first scan that is not done, and only then has each queue lend exactly its share.
 #pragma once
@@ -30,9 +30,11 @@ int queue_done_run(urf_queue* q, int max_results, int timeout_ms);
 // of tags / rcs / outs / label_views (each may be NULL except outs). Returns the number lent.
 int queue_lend_run(urf_queue* q, int count, const int* dst, uint64_t* tags, int32_t* rcs, urf_result* outs, const void** label_views);
 
-// Copies the labels of the oldest scan the last delivery call lent into the caller's n_in int32 labels, widening them
-// from an int8 slot. Nothing is copied for a failed scan or with dst == NULL.
-void queue_copy_lent_labels(const urf_queue* q, int32_t* dst);
+// The copy-out of urf_queue_next / urf_mq_next for the oldest scan the last delivery call lent: puts the caller's buffers
+// (out's members on entry; order and ring_start only with URF_QUEUE_ORDER) back into *out and copies the n_in labels into
+// `label` (int32, widened from an int8 slot), and with URF_QUEUE_ORDER the n_order entries of the emission order into
+// `order` and n_rings + 1 entries into `ring_start`. NULL buffers are skipped; nothing is copied for a failed scan.
+void queue_copy_lent(const urf_queue* q, int32_t* label, int32_t* order, int32_t* ring_start, urf_result* out);
 
 // Makes p (already validated) the set of the queue's next parameter generation: `gen`, or with gen == 0 the queue's last
 // plus one. Every scan accepted from now on carries it. Returns the generation, or URF_ERR_CLOSED after urf_queue_close.

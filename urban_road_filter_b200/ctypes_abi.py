@@ -101,6 +101,7 @@ class UrfMqStats(C.Structure):
 
 URF_QUEUE_BLOCK, URF_QUEUE_DROP_OLDEST = 0, 1
 URF_QUEUE_LABEL8 = 2          # OR-ed into the policy: int8 label slots
+URF_QUEUE_ORDER = 4           # OR-ed into the policy: every result also carries its emission order and ring offsets
 URF_ERR_TIMEOUT, URF_ERR_CLOSED = -6, -7
 # int (*)(void* user, const float* const* xyzi, const int* n, int batch, urf_result* outs)
 QUEUE_PROCESS_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.c_int, C.POINTER(UrfResult))
