@@ -380,6 +380,11 @@ int urf_queue_submit_ref(urf_queue* q, const float* xyzi, int n, uint64_t tag, i
 int urf_queue_create_cloud2(urf_queue** out, urf_ctx* ctx, int max_points, int slots, int max_batch, int policy, int point_step,
                             int off_x, int off_y, int off_z, int off_intensity);
 int urf_queue_submit_cloud2(urf_queue* q, const void* data, int n_points, uint64_t tag, int timeout_ms);
+/* As urf_queue_submit_cloud2, but the records are NOT copied: `data` (n_points * point_step bytes) is used in place by the
+ * worker's host-to-device copy and must stay valid and unchanged until the scan's result has been delivered, as for
+ * urf_queue_submit_ref. A float4 queue refuses record submits (URF_ERR_INVALID), and a record queue refuses
+ * urf_queue_submit / urf_queue_submit_ref. */
+int urf_queue_submit_cloud2_ref(urf_queue* q, const void* data, int n_points, uint64_t tag, int timeout_ms);
 
 /*
  * Parameter update on a running queue, with no drain (the reference's paramsCallback, which runs between two scan
@@ -414,6 +419,17 @@ int urf_queue_create_with_async(urf_queue** out, urf_queue_process_fn enqueue, u
  * batch with the code, as a refused enqueue does. URF_ERR_INVALID on a queue around a ctx. */
 typedef int (*urf_queue_params_fn)(void* user, const urf_params* p, int32_t gen);
 int urf_queue_set_params_hook(urf_queue* q, urf_queue_params_fn fn);
+/* Test hook: a record queue (urf_queue_create_cloud2: same format checks, same submits) around a synchronous stand-in, as
+ * urf_queue_create_with. The batch function gets the raw record pointers in its `xyzi` argument: xyzi[b] points at
+ * n[b] * point_step bytes (the queue's slot, or with urf_queue_submit_cloud2_ref the caller's own buffer), never 4-byte
+ * aligned float4 points. Its `user` argument, and the parameter hook's, is a urf_cloud2_user the queue owns: the record
+ * format and the caller's `user`, valid until urf_queue_destroy. */
+typedef struct urf_cloud2_user {
+  void*   user;                  /* the creator's `user` (urf_mq_create_cloud2_with: users[j] for device j, or NULL) */
+  int32_t point_step, off_x, off_y, off_z, off_intensity;
+} urf_cloud2_user;
+int urf_queue_create_cloud2_with(urf_queue** out, urf_queue_process_fn fn, void* user, int max_points, int slots, int max_batch,
+                                 int policy, int point_step, int off_x, int off_y, int off_z, int off_intensity);
 
 /*
  * Multi-GPU ingest (BASELINE config 4: one continuous scan stream sharded across the GPUs of a box). The reference is one
@@ -456,6 +472,21 @@ int urf_mq_create_policy(urf_mq** out, const int* devices, int n_devices, int ma
  * runs with the earlier sets, every scan after it with p. Returns the mq's generation (1, 2, ...), which the results of every
  * device report in params_gen. Waits while a producer is inside a submit call (the update takes every device's submit lock). */
 int urf_mq_update_params(urf_mq* mq, const urf_params* p);
+/* urf_mq_create_policy whose scans are raw sensor_msgs/PointCloud2 records of ONE sensor format: every device gets a context
+ * and a urf_queue_create_cloud2 queue, and the records cross PCIe as they are and are unpacked on the device
+ * (urf_process_cloud2_batch), so a producer hands in a message's `data` without repacking it. Format checks as
+ * urf_queue_create_cloud2, policy as urf_mq_create_policy; both are checked before any device is set up. Producers call
+ * urf_mq_submit_cloud2 (copy into the device queue's pinned slot) or urf_mq_submit_cloud2_ref (no copy: `data` must stay
+ * valid and unchanged until the scan's result has been delivered). A record mq refuses urf_mq_submit / urf_mq_submit_ref
+ * and a float4 mq refuses the record submits (URF_ERR_INVALID); n_points > max_points is URF_ERR_CAPACITY. Device choice,
+ * delivery order, urf_mq_next / _next_view / _next_batch, urf_mq_update_params generations, urf_mq_set_tie_order,
+ * urf_mq_get_stats, close and destroy are those of a float4 mq, and every result is bit for bit what
+ * urf_process_cloud2_batch gives for the same records under the device context's tie order and the scan's generation. */
+int urf_mq_create_cloud2(urf_mq** out, const int* devices, int n_devices, int max_points, int slots_per_device, int max_batch,
+                         const urf_params* params /* or NULL: cfg defaults */, int policy, int point_step, int off_x, int off_y,
+                         int off_z, int off_intensity);
+int urf_mq_submit_cloud2(urf_mq* mq, const void* data, int n_points, uint64_t tag, int timeout_ms);
+int urf_mq_submit_cloud2_ref(urf_mq* mq, const void* data, int n_points, uint64_t tag, int timeout_ms);
 int urf_mq_get_stats(urf_mq* mq, urf_mq_stats* st);
 void urf_mq_close(urf_mq* mq);
 void urf_mq_destroy(urf_mq* mq);
@@ -466,6 +497,11 @@ int urf_mq_create_with_label8(urf_mq** out, urf_queue_process_fn fn, void* const
                               int slots_per_device, int max_batch);
 int urf_mq_create_with_policy(urf_mq** out, urf_queue_process_fn fn, void* const* users, int n_devices, int max_points,
                               int slots_per_device, int max_batch, int policy);   /* policy as urf_mq_create_policy */
+/* Test hook: urf_mq_create_cloud2 over N stand-in devices, each a urf_queue_create_cloud2_with queue around fn (its
+ * urf_cloud2_user carries users[j] for device j). */
+int urf_mq_create_cloud2_with(urf_mq** out, urf_queue_process_fn fn, void* const* users, int n_devices, int max_points,
+                              int slots_per_device, int max_batch, int policy, int point_step, int off_x, int off_y, int off_z,
+                              int off_intensity);
 /* Test hook: urf_queue_set_params_hook on every stand-in device (fn gets users[j] for device j). URF_ERR_INVALID on real devices. */
 int urf_mq_set_params_hook(urf_mq* mq, urf_queue_params_fn fn);
 

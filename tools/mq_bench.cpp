@@ -4,11 +4,18 @@
 // reference (scans already in pinned memory, no host copy). Prints one JSON line per mode: scans/s and the host-side
 // limiter it points at. Host tool: links liburf_b200.so, no CUDA code of its own.
 //   usage: mq_bench <scans.bin> <points per scan> <n_scans_in_file> <n_devices> <producers> <total scans> <slots> <max_batch>
-//          [full_roi channels interval [modes max_results [order]]]
+//          [full_roi channels interval [modes max_results [order [point_step off_x off_y off_z off_intensity]]]]
 // modes: comma-separated subset of 0 (copying submit), 1 (by reference), 2 (by reference, labels viewed in place with
 // urf_mq_next_view), 3 (by reference, int8 label slots, results taken with urf_mq_next_batch, up to max_results per call);
 // default 0,1,2. order: 1 creates the device queues with URF_QUEUE_ORDER (every batch runs the ring sort and copies the
 // emission order back; mode 3 reads n_order of every view); default 0.
+// point_step > 0: the file holds PointCloud2 records of that many bytes per point (x / y / z / intensity FLOAT32 at the
+// offsets given, off_intensity -1: none) instead of float4 points, and only the record modes run, both delivered as mode 3:
+//   4: a record mq (urf_mq_create_cloud2), scans submitted as they are with urf_mq_submit_cloud2_ref;
+//   5: a float4 mq; each producer first repacks the scan's records into (x, y, z, intensity) points, inside the timed
+//      region, into the next of its own D * slots + 1 pinned buffers, and submits that with urf_mq_submit_ref. A scan of a
+//      producer cannot be undelivered D * slots + 1 submits later (the mq holds D * slots scans), so a buffer is never
+//      rewritten before its scan's copy has run.
 #include <algorithm>
 #include <atomic>
 #include <chrono>
@@ -27,10 +34,14 @@ int main(int argc, char** argv) {
   const int full_roi = argc > 9 ? atoi(argv[9]) : 1, channels = argc > 10 ? atoi(argv[10]) : 64;
   const double interval = argc > 11 ? atof(argv[11]) : 0.18;
   std::vector<int> modes = {0, 1, 2};
-  if (argc > 12) { modes.clear(); for (const char* c = argv[12]; *c; c++) if (*c >= '0' && *c <= '3') modes.push_back(*c - '0'); }
+  if (argc > 12) { modes.clear(); for (const char* c = argv[12]; *c; c++) if (*c >= '0' && *c <= '5') modes.push_back(*c - '0'); }
   const int max_results = argc > 13 ? atoi(argv[13]) : 64;
   const bool order = argc > 14 && atoi(argv[14]) != 0;
-  const size_t bytes = (size_t)n * 16;
+  const int step = argc > 15 ? atoi(argv[15]) : 0, ox = argc > 16 ? atoi(argv[16]) : 0, oy = argc > 17 ? atoi(argv[17]) : 4,
+            oz = argc > 18 ? atoi(argv[18]) : 8, oi = argc > 19 ? atoi(argv[19]) : -1;
+  for (int m : modes)
+    if ((m >= 4) != (step > 0)) { fprintf(stderr, "modes 4 and 5 need a record file (point_step > 0), modes 0-3 a float4 file\n"); return 2; }
+  const size_t bytes = (size_t)n * (step > 0 ? step : 16);       // one scan in the file
   std::vector<float*> pinned(K);
   FILE* f = fopen(path, "rb");
   if (!f) { perror(path); return 2; }
@@ -40,7 +51,21 @@ int main(int argc, char** argv) {
   }
   fclose(f);
   std::vector<std::vector<float>> pageable(K);                    // the copying mode reads from ordinary (pageable) memory, like a driver
-  for (int k = 0; k < K; k++) pageable[k].assign(pinned[k], pinned[k] + (size_t)n * 4);
+  if (step == 0) for (int k = 0; k < K; k++) pageable[k].assign(pinned[k], pinned[k] + (size_t)n * 4);
+  const int ring = D * slots + 1;                                 // mode 5: repack buffers per producer
+  std::vector<std::vector<float*>> repacked(P);
+  if (std::find(modes.begin(), modes.end(), 5) != modes.end())
+    for (auto& bufs : repacked)
+      for (int r = 0; r < ring; r++) {
+        bufs.push_back(static_cast<float*>(urf_pinned_alloc((size_t)n * 16)));
+        if (!bufs.back()) { fprintf(stderr, "cannot allocate repack buffers\n"); return 2; }
+      }
+  auto repack = [&](const unsigned char* rec, float* dst) {       // what a producer without record submits does per scan
+    for (int i = 0; i < n; i++, rec += step, dst += 4) {
+      std::memcpy(dst, rec + ox, 4); std::memcpy(dst + 1, rec + oy, 4); std::memcpy(dst + 2, rec + oz, 4);
+      if (oi >= 0) std::memcpy(dst + 3, rec + oi, 4); else dst[3] = 0.f;
+    }
+  };
   urf_params prm;
   urf_default_params(&prm);
   prm.channels = channels; prm.interval = interval;
@@ -48,10 +73,12 @@ int main(int argc, char** argv) {
   std::vector<int> devs(D);
   for (int d = 0; d < D; d++) devs[d] = d;
   for (int mode : modes) {                                        // 0: copying submit, 1: by reference (pinned), 2: 1 + labels viewed in place,
-                                                                  // 3: 1 + int8 slots delivered in runs (urf_mq_next_batch)
+                                                                  // 3: 1 + int8 slots delivered in runs (urf_mq_next_batch),
+                                                                  // 4: records by reference, 5: records repacked, both as 3
     urf_mq* mq = nullptr;
-    const int policy = URF_QUEUE_BLOCK | (mode == 3 ? URF_QUEUE_LABEL8 : 0) | (order ? URF_QUEUE_ORDER : 0);
-    int rc = urf_mq_create_policy(&mq, devs.data(), D, n, slots, mb, &prm, policy);
+    const int policy = URF_QUEUE_BLOCK | (mode >= 3 ? URF_QUEUE_LABEL8 : 0) | (order ? URF_QUEUE_ORDER : 0);
+    int rc = mode == 4 ? urf_mq_create_cloud2(&mq, devs.data(), D, n, slots, mb, &prm, policy, step, ox, oy, oz, oi)
+                       : urf_mq_create_policy(&mq, devs.data(), D, n, slots, mb, &prm, policy);
     if (rc != URF_OK) { fprintf(stderr, "urf_mq_create: %s (%s)\n", urf_strerror(rc), urf_last_cuda_error(nullptr)); return 1; }
     std::vector<int32_t> lab(n);
     std::atomic<long> road{0}, ordered{0};
@@ -59,14 +86,22 @@ int main(int argc, char** argv) {
       std::vector<std::thread> prod;
       const auto t0 = std::chrono::steady_clock::now();
       for (int p = 0; p < P; p++) prod.emplace_back([&, p] {
+        int next_buf = 0;
         for (int i = p; i < count; i += P) {
           const int k = i % K;
-          const int r = mode ? urf_mq_submit_ref(mq, pinned[k], n, (uint64_t)i, -1) : urf_mq_submit(mq, pageable[k].data(), n, (uint64_t)i, -1);
+          int r;
+          if (mode == 4) r = urf_mq_submit_cloud2_ref(mq, pinned[k], n, (uint64_t)i, -1);
+          else if (mode == 5) {
+            float* buf = repacked[p][next_buf];
+            next_buf = (next_buf + 1) % ring;
+            repack(reinterpret_cast<const unsigned char*>(pinned[k]), buf);
+            r = urf_mq_submit_ref(mq, buf, n, (uint64_t)i, -1);
+          } else r = mode ? urf_mq_submit_ref(mq, pinned[k], n, (uint64_t)i, -1) : urf_mq_submit(mq, pageable[k].data(), n, (uint64_t)i, -1);
           if (r != URF_OK) { fprintf(stderr, "submit: %s\n", urf_strerror(r)); exit(1); }
         }
       });
       std::thread cons([&] {
-        if (mode == 3) {
+        if (mode >= 3) {
           std::vector<uint64_t> tags(max_results);
           std::vector<int32_t> rcs(max_results);
           std::vector<urf_result> outs(max_results);
@@ -103,14 +138,19 @@ int main(int argc, char** argv) {
     urf_mq_get_stats(mq, &st);
     int largest = 0; unsigned long long mn = ~0ull, mx = 0;
     for (int d = 0; d < D; d++) { largest = st.largest_batch[d] > largest ? st.largest_batch[d] : largest; mn = st.submitted[d] < mn ? st.submitted[d] : mn; mx = st.submitted[d] > mx ? st.submitted[d] : mx; }
+    const int h2d_bytes = mode == 4 ? step : 16;                  // input bytes per point that cross PCIe
+    static const char* const names[] = {"copying_submit", "by_reference_pinned", "by_reference_pinned_labels_viewed_in_place",
+                                        "by_reference_pinned_label8_next_batch", "records_by_reference_label8_next_batch",
+                                        "records_repacked_to_float4_by_reference_label8_next_batch"};
     printf("{\"mq_bench\": \"%s\", \"devices\": %d, \"producers\": %d, \"points_per_scan\": %d, \"scans\": %d, \"seconds\": %.4f, \"scans_per_sec\": %.1f, "
            "\"mpoints_per_sec\": %.1f, \"h2d_gb_per_sec\": %.2f, \"largest_batch\": %d, \"per_device_min_max\": [%llu, %llu], \"road_points\": %ld, "
-           "\"order\": %d, \"ordered_points\": %ld}\n",
-           mode == 3 ? "by_reference_pinned_label8_next_batch" : mode == 2 ? "by_reference_pinned_labels_viewed_in_place" : mode ? "by_reference_pinned" : "copying_submit", D, P, n, total, s, total / s, total / s * n / 1e6, total / s * bytes / 1e9, largest, mn, mx,
-           road.load(), (int)order, ordered.load());
+           "\"order\": %d, \"ordered_points\": %ld, \"h2d_bytes_per_point\": %d}\n",
+           names[mode], D, P, n, total, s, total / s, total / s * n / 1e6, total / s * n * h2d_bytes / 1e9, largest, mn, mx,
+           road.load(), (int)order, ordered.load(), h2d_bytes);
     fflush(stdout);
     urf_mq_destroy(mq);
   }
   for (float* p : pinned) urf_pinned_free(p);
+  for (auto& bufs : repacked) for (float* p : bufs) urf_pinned_free(p);
   return 0;
 }

@@ -26,7 +26,9 @@ EXPORTS = ["urf_queue_next_batch", "urf_mq_next_batch", "urf_mq_create_label8", 
            "urf_last_launch_count", "urf_build_markers", "urf_set_tie_order", "urf_get_tie_order", "urf_mq_set_tie_order",
            "urf_enqueue_batch", "urf_enqueue_cloud2_batch", "urf_finish_batch", "urf_queue_create_with_async",
            "urf_set_params_next", "urf_queue_update_params", "urf_mq_update_params", "urf_queue_set_params_hook",
-           "urf_mq_set_params_hook", "urf_mq_create_policy", "urf_mq_create_with_policy"]
+           "urf_mq_set_params_hook", "urf_mq_create_policy", "urf_mq_create_with_policy", "urf_queue_submit_cloud2_ref",
+           "urf_queue_create_cloud2_with", "urf_mq_create_cloud2", "urf_mq_create_cloud2_with", "urf_mq_submit_cloud2",
+           "urf_mq_submit_cloud2_ref"]
 
 # urf_set_tie_order modes (include/urf.h): equal azimuths inside a ring in input order, or in the reference's Lomuto order
 TIE_ORDERS = {"input": 0, "reference": 1}
@@ -102,6 +104,8 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
     lib.urf_queue_submit_ref.argtypes = [vp, vp, ip, C.c_uint64, ip]
     lib.urf_queue_create_cloud2.argtypes = [C.POINTER(vp), vp, ip, ip, ip, ip, ip, ip, ip, ip, ip]
     lib.urf_queue_submit_cloud2.argtypes = [vp, vp, ip, C.c_uint64, ip]
+    lib.urf_queue_submit_cloud2_ref.argtypes = [vp, vp, ip, C.c_uint64, ip]
+    lib.urf_queue_create_cloud2_with.argtypes = [C.POINTER(vp), QUEUE_PROCESS_FN, vp, ip, ip, ip, ip, ip, ip, ip, ip, ip]
     lib.urf_mq_create.argtypes = [C.POINTER(vp), C.POINTER(ip), ip, ip, ip, ip, C.POINTER(UrfParams)]
     lib.urf_mq_create_with.argtypes = [C.POINTER(vp), QUEUE_PROCESS_FN, C.POINTER(vp), ip, ip, ip, ip]
     lib.urf_mq_set_params.argtypes = [vp, C.POINTER(UrfParams)]
@@ -117,6 +121,10 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
     lib.urf_mq_create_with_label8.argtypes = [C.POINTER(vp), QUEUE_PROCESS_FN, C.POINTER(vp), ip, ip, ip, ip]
     lib.urf_mq_create_policy.argtypes = [C.POINTER(vp), C.POINTER(ip), ip, ip, ip, ip, C.POINTER(UrfParams), ip]
     lib.urf_mq_create_with_policy.argtypes = [C.POINTER(vp), QUEUE_PROCESS_FN, C.POINTER(vp), ip, ip, ip, ip, ip]
+    lib.urf_mq_create_cloud2.argtypes = [C.POINTER(vp), C.POINTER(ip), ip, ip, ip, ip, C.POINTER(UrfParams), ip, ip, ip, ip, ip, ip]
+    lib.urf_mq_create_cloud2_with.argtypes = [C.POINTER(vp), QUEUE_PROCESS_FN, C.POINTER(vp), ip, ip, ip, ip, ip, ip, ip, ip, ip, ip]
+    lib.urf_mq_submit_cloud2.argtypes = [vp, vp, ip, C.c_uint64, ip]
+    lib.urf_mq_submit_cloud2_ref.argtypes = [vp, vp, ip, C.c_uint64, ip]
     batch_args = [vp, ip, C.POINTER(C.c_uint64), C.POINTER(C.c_int32), C.POINTER(UrfResult), C.POINTER(vp), ip]
     lib.urf_queue_next_batch.argtypes = batch_args
     lib.urf_queue_next_view.argtypes = [vp, C.POINTER(C.c_uint64), C.POINTER(UrfResult), C.POINTER(vp), ip]
@@ -508,16 +516,18 @@ class _BatchBuffers:
 
 class _StreamQueue:
     """What ScanQueue and MultiGpuQueue share: the library handle `_h`, the arrays of by-reference submits, the reused
-    batch buffers, and submit / next / next_batch / close / destroy, written against the library functions
+    batch buffers, and submit / submit_records / next / next_batch / close / destroy, written against the library functions
     `_PREFIX` + name (urf_queue_* or urf_mq_*), which have the same arguments in both families."""
     _PREFIX = ""
 
-    def __init__(self, max_points: int, label8: bool, params: UrfParams | None = None, order: bool = False):
+    def __init__(self, max_points: int, label8: bool, params: UrfParams | None = None, order: bool = False, records=None):
         self.lib = load_library()
         self._h = C.c_void_p()
         self.max_points = max_points
         self.label8 = label8
         self.order = order                # URF_QUEUE_ORDER: results carry order and ring_start
+        # record queue: (point_step, off_x, off_y, off_z, off_intensity) of its PointCloud2 records; None: float4 scans
+        self.records = None if records is None else tuple(int(v) for v in records)
         self._cb = None                   # ctypes callbacks of a stand-in, kept alive with the queue
         self._params_cb = None            # the parameter hook of a stand-in
         self._bufs = None
@@ -559,6 +569,22 @@ class _StreamQueue:
         rc = self._call("submit_ref" if by_reference else "submit", pts.ctypes.data, pts.shape[0], tag, timeout_ms)
         if rc not in (URF_OK, URF_ERR_TIMEOUT, URF_ERR_CLOSED):
             raise UrfError(rc, self._PREFIX + "submit")
+        return rc
+
+    def submit_records(self, data, n_points: int, tag: int = 0, timeout_ms: int = -1, by_reference: bool = False) -> int:
+        """A scan of a record queue: the raw `data` bytes of a sensor_msgs/PointCloud2 (bytes, bytearray or an array), of
+        which the first n_points records count (urf_queue_submit_cloud2 / urf_mq_submit_cloud2). Returns as submit, and
+        raises UrfError(URF_ERR_INVALID) on a float4 queue. by_reference: no copy (urf_*_submit_cloud2_ref): keep `data`
+        alive and unchanged until its result has come back."""
+        raw = np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray)) else np.ascontiguousarray(data).view(np.uint8).reshape(-1)
+        if self.records is not None and raw.size < n_points * self.records[0]:
+            raise ValueError(f"{raw.size} bytes hold fewer than {n_points} records of {self.records[0]} bytes")
+        if by_reference:
+            self._keep[tag] = raw
+        name = "submit_cloud2_ref" if by_reference else "submit_cloud2"
+        rc = self._call(name, raw.ctypes.data, n_points, tag, timeout_ms)
+        if rc not in (URF_OK, URF_ERR_TIMEOUT, URF_ERR_CLOSED):
+            raise UrfError(rc, self._PREFIX + name)
         return rc
 
     def next(self, timeout_ms: int = -1):
@@ -616,22 +642,25 @@ class MultiGpuQueue(_StreamQueue):
     every scan goes to the device with the fewest scans in flight, results come back in submission order. Any number of
     producer threads, one consumer. `by_reference` submits hand the array to the library without a copy: keep it alive and
     unchanged until its result has come back. label8: int8 label slots on every device, order: the emission order and ring
-    offsets with every result (see ScanQueue)."""
+    offsets with every result, records: a record mq (urf_mq_create_cloud2) fed with submit_records (see ScanQueue)."""
     _PREFIX = "urf_mq_"
     _m = property(lambda self: self._h)      # the library handle, under the name this class has always had for it
 
     def __init__(self, devices, max_points: int, slots_per_device: int = 8, max_batch: int = 4, params: UrfParams | None = None,
-                 process_fn=None, label8: bool = False, order: bool = False):
-        super().__init__(max_points, label8, None if process_fn is not None else params if params is not None else make_params(), order)
+                 process_fn=None, label8: bool = False, order: bool = False, records=None):
+        super().__init__(max_points, label8, None if process_fn is not None else params if params is not None else make_params(), order,
+                         records)
         policy = URF_QUEUE_BLOCK | (URF_QUEUE_LABEL8 if label8 else 0) | (URF_QUEUE_ORDER if order else 0)
+        fmt = self.records or ()
         if process_fn is not None:                      # tests: stand-in devices, no GPU
             self._cb = QUEUE_PROCESS_FN(process_fn)
-            rc = self.lib.urf_mq_create_with_policy(C.byref(self._h), self._cb, None, len(devices), max_points, slots_per_device,
-                                                    max_batch, policy)
+            create = self.lib.urf_mq_create_cloud2_with if fmt else self.lib.urf_mq_create_with_policy
+            rc = create(C.byref(self._h), self._cb, None, len(devices), max_points, slots_per_device, max_batch, policy, *fmt)
         else:
             dv = (C.c_int * len(devices))(*devices)
-            rc = self.lib.urf_mq_create_policy(C.byref(self._h), dv, len(devices), max_points, slots_per_device, max_batch,
-                                               C.byref(params) if params is not None else None, policy)
+            create = self.lib.urf_mq_create_cloud2 if fmt else self.lib.urf_mq_create_policy
+            rc = create(C.byref(self._h), dv, len(devices), max_points, slots_per_device, max_batch,
+                        C.byref(params) if params is not None else None, policy, *fmt)
         if rc != URF_OK:
             raise UrfError(rc, "urf_mq_create", self.lib.urf_last_cuda_error(None).decode())
 
@@ -664,29 +693,37 @@ class ScanQueue(_StreamQueue):
     runs the real queue's two-batches-in-flight schedule around them. label8: int8 label slots (URF_QUEUE_LABEL8) — a
     quarter of the label traffic and memory; `next` still returns int32 labels, `next_batch` int8 ones. order
     (URF_QUEUE_ORDER): every result also carries its emission order and ring_start, so that cloud_indices("road" | "curb" |
-    "road_probably") works on it; the batches then run the ring sort and copy 4 bytes per point more."""
+    "road_probably") works on it; the batches then run the ring sort and copy 4 bytes per point more. records
+    (point_step, off_x, off_y, off_z, off_intensity): a queue of raw PointCloud2 records of that one format
+    (urf_queue_create_cloud2, or urf_queue_create_cloud2_with around process_fn), fed with submit_records and unpacked on
+    the device; `submit` then raises, as submit_records does on a float4 queue."""
     _PREFIX = "urf_queue_"
     _q = property(lambda self: self._h)      # the library handle, under the name this class has always had for it
 
     def __init__(self, detector: "Detector | None", max_points: int, slots: int = 8, max_batch: int = 4,
                  policy: int = URF_QUEUE_BLOCK, process_fn=None, label8: bool = False, enqueue_fn=None, finish_fn=None,
-                 order: bool = False):
+                 order: bool = False, records=None):
         order = order or bool(policy & URF_QUEUE_ORDER)
-        super().__init__(max_points, label8, detector.params if detector is not None else None, order)
+        super().__init__(max_points, label8, detector.params if detector is not None else None, order, records)
+        fmt = self.records or ()
         if label8:
             policy |= URF_QUEUE_LABEL8
         if order:
             policy |= URF_QUEUE_ORDER
         if enqueue_fn is not None:
+            if fmt:
+                raise ValueError("records: a record queue has no asynchronous stand-in")
             self._cb = (QUEUE_PROCESS_FN(enqueue_fn), QUEUE_FINISH_FN(lambda user: finish_fn()))
             rc = self.lib.urf_queue_create_with_async(C.byref(self._h), *self._cb, None, max_points, slots, max_batch, policy)
         elif process_fn is not None:
             self._cb = QUEUE_PROCESS_FN(process_fn)
-            rc = self.lib.urf_queue_create_with(C.byref(self._h), self._cb, None, max_points, slots, max_batch, policy)
+            create = self.lib.urf_queue_create_cloud2_with if fmt else self.lib.urf_queue_create_with
+            rc = create(C.byref(self._h), self._cb, None, max_points, slots, max_batch, policy, *fmt)
         else:
             assert detector is not None and detector.max_batch >= max_batch and detector.max_points >= max_points
             self._det = detector          # keeps the ctx alive; nobody else may use it while the queue exists
-            rc = self.lib.urf_queue_create(C.byref(self._h), detector._ctx, max_points, slots, max_batch, policy)
+            create = self.lib.urf_queue_create_cloud2 if fmt else self.lib.urf_queue_create
+            rc = create(C.byref(self._h), detector._ctx, max_points, slots, max_batch, policy, *fmt)
         if rc != URF_OK:
             raise UrfError(rc, "urf_queue_create")
 

@@ -100,8 +100,8 @@ def build_kat() -> None:
         subprocess.run(["g++", "-std=c++17", "-O1", "-g", "-fsanitize=thread", "-pthread", "-o", tgt, *qsrc], check=True)
     # the same for batched delivery (urf_queue_next_batch / urf_mq_next_batch) and int8 label slots, for the worker's
     # two-batches-in-flight schedule around an asynchronous stand-in, for parameter updates on a running queue, and for
-    # the emission order delivered with URF_QUEUE_ORDER
-    for name in ("queue_batch_stress", "queue_async_stress", "queue_params_stress", "queue_order_stress"):
+    # the emission order delivered with URF_QUEUE_ORDER, and for PointCloud2 records through the multi-GPU queue
+    for name in ("queue_batch_stress", "queue_async_stress", "queue_params_stress", "queue_order_stress", "mq_records_stress"):
         tgt = os.path.join(bdir, name)
         src = [os.path.join(kat, name + ".cpp")] + qsrc[1:]
         if _stale(tgt, src + qdeps):

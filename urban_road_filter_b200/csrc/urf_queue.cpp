@@ -48,7 +48,7 @@ struct Slot {
   int32_t gen = 0;           // parameter generation in force when the scan became PENDING
   int n = 0, rc = URF_OK;
   float* in = nullptr;       // max_points * bytes_per_point bytes (pinned for the real queue)
-  const float* ext = nullptr;   // urf_queue_submit_ref: the caller's buffer is used in place (no copy)
+  const float* ext = nullptr;   // urf_queue_submit_ref / _cloud2_ref: the caller's buffer is used in place (no copy)
   int32_t* label = nullptr;  // max_points; NULL in a real URF_QUEUE_LABEL8 queue
   int8_t* label8 = nullptr;  // max_points, URF_QUEUE_LABEL8 only
   int32_t* order = nullptr;       // max_points, URF_QUEUE_ORDER only: the emission order
@@ -72,6 +72,7 @@ struct urf_queue {
   // bytes (urf_queue_create_cloud2), handed to urf_process_cloud2_batch and unpacked on the device
   int step = 0, ox = 0, oy = 4, oz = 8, oi = -1;
   size_t bytes_per_point = 16;
+  urf_cloud2_user rec{};       // record stand-in (urf_queue_create_cloud2_with): `user` points here, rec.user is the creator's
   std::vector<Slot> slots;
   std::mutex mu;
   std::condition_variable cv_free, cv_pending, cv_done;
@@ -266,6 +267,7 @@ int create_common(urf_queue** out, urf_ctx* ctx, urf_queue_process_fn enq, urf_q
   q->label8 = label8; q->order = order; q->depth = ctx || fin ? 2 : 1;
   q->step = step; q->ox = ox; q->oy = oy; q->oz = oz; q->oi = oi;
   q->bytes_per_point = step > 0 ? (size_t)step : 16;
+  if (!ctx && step > 0) { q->rec = urf_cloud2_user{user, step, ox, oy, oz, oi}; q->user = &q->rec; }
   q->slots.resize(slots); q->lent.reserve(slots); q->live.reserve(slots);
   // int8 slots hold max_points bytes of labels; a stand-in batch function still writes int32 labels, which need a buffer
   const bool want32 = !label8 || !ctx, want8 = label8;
@@ -301,10 +303,15 @@ int urf_queue_create(urf_queue** out, urf_ctx* ctx, int max_points, int slots, i
 
 int urf_queue_create_cloud2(urf_queue** out, urf_ctx* ctx, int max_points, int slots, int max_batch, int policy, int point_step, int off_x,
                             int off_y, int off_z, int off_intensity) {
-  if (!ctx || point_step < 12 || point_step > URF_MAX_POINT_STEP) return URF_ERR_INVALID;
-  for (int o : {off_x, off_y, off_z}) if (o < 0 || o + 4 > point_step) return URF_ERR_INVALID;
-  if (off_intensity >= 0 && off_intensity + 4 > point_step) return URF_ERR_INVALID;
+  if (!ctx || urf_internal::check_cloud2_format(point_step, off_x, off_y, off_z, off_intensity) != URF_OK) return URF_ERR_INVALID;
   return create_common(out, ctx, nullptr, nullptr, nullptr, max_points, slots, max_batch, policy, point_step, off_x, off_y, off_z,
+                       off_intensity);
+}
+
+int urf_queue_create_cloud2_with(urf_queue** out, urf_queue_process_fn fn, void* user, int max_points, int slots, int max_batch,
+                                 int policy, int point_step, int off_x, int off_y, int off_z, int off_intensity) {
+  if (!fn || urf_internal::check_cloud2_format(point_step, off_x, off_y, off_z, off_intensity) != URF_OK) return URF_ERR_INVALID;
+  return create_common(out, nullptr, fn, nullptr, user, max_points, slots, max_batch, policy, point_step, off_x, off_y, off_z,
                        off_intensity);
 }
 
@@ -319,72 +326,25 @@ int urf_queue_create_with_async(urf_queue** out, urf_queue_process_fn enqueue, u
   return create_common(out, nullptr, enqueue, finish, user, max_points, slots, max_batch, policy);
 }
 
-namespace {
-int submit_common(urf_queue* q, const void* data, int n, uint64_t tag, int timeout_ms, bool by_reference) {
-  if (!q || n < 0 || (n > 0 && !data)) return URF_ERR_INVALID;
-  if (n > q->max_points) return URF_ERR_CAPACITY;
-  int slot = -1;
-  {
-    std::unique_lock<std::mutex> lk(q->mu);
-    auto find = [&] {
-      if (q->closed) return true;
-      for (int i = 0; i < (int)q->slots.size(); i++) if (q->slots[i].state == FREE) { slot = i; return true; }
-      if (q->policy == URF_QUEUE_DROP_OLDEST) {           // lidar_segmentation.cpp:53: the subscriber keeps only the newest scan
-        int best = -1;
-        for (int i = 0; i < (int)q->slots.size(); i++) {
-          const Slot& s = q->slots[i];
-          if (s.state == PENDING && (best < 0 || s.seq < q->slots[best].seq)) best = i;
-        }
-        if (best >= 0) { q->st.dropped++; slot = best; return true; }
-      }
-      return false;
-    };
-    if (!wait_for(q->cv_free, lk, timeout_ms, find)) return URF_ERR_TIMEOUT;
-    if (q->closed) return URF_ERR_CLOSED;
-    q->slots[slot].state = FILLING;                       // a dropped scan's sequence number simply never reaches DONE
-  }
-  Slot& s = q->slots[slot];
-  bool closed_late = false;
-  if (by_reference) s.ext = static_cast<const float*>(data);
-  else { s.ext = nullptr; if (n > 0) std::memcpy(s.in, data, q->bytes_per_point * (size_t)n); }
-  {
-    std::lock_guard<std::mutex> lk(q->mu);
-    if (q->closed) {                                      // closed while copying: the worker may already be gone
-      s.state = FREE;
-      closed_late = true;
-    } else {
-      s.n = n; s.tag = tag; s.rc = URF_OK;
-      s.seq = q->next_seq++; s.gen = q->gen;
-      s.state = PENDING;
-      q->st.submitted++;
-    }
-  }
-  if (closed_late) {
-    // a consumer whose last look at the slots still saw this one FILLING must get to see the drained state: close()'s
-    // own notify may have come before that look
-    q->cv_done.notify_all();
-    q->cv_free.notify_one();
-    return URF_ERR_CLOSED;
-  }
-  q->cv_pending.notify_one();
-  q->cv_done.notify_all();                                // a consumer waiting on a dropped sequence number re-evaluates
-  return URF_OK;
-}
-}  // namespace
 
 int urf_queue_submit(urf_queue* q, const float* xyzi, int n, uint64_t tag, int timeout_ms) {
   if (q && q->step != 0) return URF_ERR_INVALID;           // a record queue takes urf_queue_submit_cloud2
-  return submit_common(q, xyzi, n, tag, timeout_ms, false);
+  return urf_internal::queue_submit(q, xyzi, n, tag, timeout_ms, false);
 }
 
 int urf_queue_submit_ref(urf_queue* q, const float* xyzi, int n, uint64_t tag, int timeout_ms) {
   if (q && q->step != 0) return URF_ERR_INVALID;
-  return submit_common(q, xyzi, n, tag, timeout_ms, true);
+  return urf_internal::queue_submit(q, xyzi, n, tag, timeout_ms, true);
 }
 
 int urf_queue_submit_cloud2(urf_queue* q, const void* data, int n_points, uint64_t tag, int timeout_ms) {
+  if (q && q->step == 0) return URF_ERR_INVALID;           // a float4 queue takes urf_queue_submit
+  return urf_internal::queue_submit(q, data, n_points, tag, timeout_ms, false);
+}
+
+int urf_queue_submit_cloud2_ref(urf_queue* q, const void* data, int n_points, uint64_t tag, int timeout_ms) {
   if (q && q->step == 0) return URF_ERR_INVALID;
-  return submit_common(q, data, n_points, tag, timeout_ms, false);
+  return urf_internal::queue_submit(q, data, n_points, tag, timeout_ms, true);
 }
 
 int urf_queue_update_params(urf_queue* q, const urf_params* p) {
@@ -544,6 +504,13 @@ void urf_queue_destroy(urf_queue* q) {
 
 namespace urf_internal {
 
+int check_cloud2_format(int point_step, int off_x, int off_y, int off_z, int off_intensity) {
+  if (point_step < 12 || point_step > URF_MAX_POINT_STEP) return URF_ERR_INVALID;
+  for (int o : {off_x, off_y, off_z}) if (o < 0 || o + 4 > point_step) return URF_ERR_INVALID;
+  if (off_intensity >= 0 && off_intensity + 4 > point_step) return URF_ERR_INVALID;
+  return URF_OK;
+}
+
 int queue_done_run(urf_queue* q, int max_results, int timeout_ms) {
   std::unique_lock<std::mutex> lk(q->mu);
   const int k = wait_done_run(q, lk, max_results, timeout_ms);
@@ -558,6 +525,57 @@ int queue_lend_run(urf_queue* q, int count, const int* dst, uint64_t* tags, int3
   }
   hand_out(q, dst, tags, rcs, outs, label_views);
   return (int)q->lent.size();
+}
+
+int queue_submit(urf_queue* q, const void* data, int n, uint64_t tag, int timeout_ms, bool by_reference) {
+  if (!q || n < 0 || (n > 0 && !data)) return URF_ERR_INVALID;
+  if (n > q->max_points) return URF_ERR_CAPACITY;
+  int slot = -1;
+  {
+    std::unique_lock<std::mutex> lk(q->mu);
+    auto find = [&] {
+      if (q->closed) return true;
+      for (int i = 0; i < (int)q->slots.size(); i++) if (q->slots[i].state == FREE) { slot = i; return true; }
+      if (q->policy == URF_QUEUE_DROP_OLDEST) {           // lidar_segmentation.cpp:53: the subscriber keeps only the newest scan
+        int best = -1;
+        for (int i = 0; i < (int)q->slots.size(); i++) {
+          const Slot& s = q->slots[i];
+          if (s.state == PENDING && (best < 0 || s.seq < q->slots[best].seq)) best = i;
+        }
+        if (best >= 0) { q->st.dropped++; slot = best; return true; }
+      }
+      return false;
+    };
+    if (!wait_for(q->cv_free, lk, timeout_ms, find)) return URF_ERR_TIMEOUT;
+    if (q->closed) return URF_ERR_CLOSED;
+    q->slots[slot].state = FILLING;                       // a dropped scan's sequence number simply never reaches DONE
+  }
+  Slot& s = q->slots[slot];
+  bool closed_late = false;
+  if (by_reference) s.ext = static_cast<const float*>(data);
+  else { s.ext = nullptr; if (n > 0) std::memcpy(s.in, data, q->bytes_per_point * (size_t)n); }
+  {
+    std::lock_guard<std::mutex> lk(q->mu);
+    if (q->closed) {                                      // closed while copying: the worker may already be gone
+      s.state = FREE;
+      closed_late = true;
+    } else {
+      s.n = n; s.tag = tag; s.rc = URF_OK;
+      s.seq = q->next_seq++; s.gen = q->gen;
+      s.state = PENDING;
+      q->st.submitted++;
+    }
+  }
+  if (closed_late) {
+    // a consumer whose last look at the slots still saw this one FILLING must get to see the drained state: close()'s
+    // own notify may have come before that look
+    q->cv_done.notify_all();
+    q->cv_free.notify_one();
+    return URF_ERR_CLOSED;
+  }
+  q->cv_pending.notify_one();
+  q->cv_done.notify_all();                                // a consumer waiting on a dropped sequence number re-evaluates
+  return URF_OK;
 }
 
 int queue_update_params(urf_queue* q, const urf_params* p, int32_t gen) {

@@ -111,6 +111,13 @@ QUEUE_FINISH_FN = C.CFUNCTYPE(C.c_int, C.c_void_p)
 QUEUE_PARAMS_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(UrfParams), C.c_int32)
 
 
+class UrfCloud2User(C.Structure):
+    """urf_cloud2_user: what a record stand-in's batch function and parameter hook get as `user` (the record format and the
+    creator's user)."""
+    _fields_ = [("user", C.c_void_p), ("point_step", C.c_int32), ("off_x", C.c_int32), ("off_y", C.c_int32),
+                ("off_z", C.c_int32), ("off_intensity", C.c_int32)]
+
+
 # cfg/LidarFilters.cfg:10-84 defaults
 DEFAULTS = dict(
     fixed_frame=b"left_os1/os1_lidar", topic_name=b"/left_os1/os1_cloud_node/points",
