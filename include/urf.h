@@ -226,6 +226,25 @@ int urf_process_cloud2_batch(urf_ctx* ctx, const void* const* data, const int* n
                              int off_y, int off_z, int off_intensity, urf_result* outs, int8_t* const* label8);
 
 /*
+ * Several sensor formats in one batch (a vehicle with Ouster and Velodyne LiDARs): only the unpack on the device reads the
+ * record format, so one batch can carry scans of different formats. A format is what a PointCloud2's `fields` and
+ * `point_step` give: FLOAT32 x / y / z at off_x / off_y / off_z and intensity at off_intensity (or -1: none) inside a record
+ * of point_step bytes. A float4 scan is the format {16, 0, 4, 8, 12}.
+ */
+typedef struct urf_cloud2_format {
+  int32_t point_step, off_x, off_y, off_z, off_intensity;
+} urf_cloud2_format;
+#define URF_MAX_FORMATS 8        /* formats of one urf_queue_create_formats / urf_mq_create_formats table */
+/* urf_process_cloud2_batch where scan b's records have the format fmt[b]. Every fmt[b] passes the checks of
+ * urf_process_cloud2 (URF_ERR_INVALID otherwise); outs and label8 as urf_process_cloud2_batch, and every output of scan b is
+ * bit for bit what urf_process_cloud2_batch gives for that scan alone in its own format, in both tie orders. The records of
+ * scan b are staged on the device at b * stride * step_max bytes, step_max being the batch's largest point_step (the staging
+ * buffer grows as for urf_process_cloud2_batch); the formats cross PCIe with the point counts, 20 bytes per scan. A batch
+ * whose scans all have one format runs exactly as urf_process_cloud2_batch. */
+int urf_process_cloud2_batch_mixed(urf_ctx* ctx, const void* const* data, const int* n_points, const urf_cloud2_format* fmt,
+                                   int batch, urf_result* outs, int8_t* const* label8);
+
+/*
  * Asynchronous host-buffer batches: urf_enqueue_batch (float4 scans, as urf_process_batch) and urf_enqueue_cloud2_batch
  * (PointCloud2 records, as urf_process_cloud2_batch) queue the copies and kernels of a batch and return at once;
  * urf_finish_batch waits for the OLDEST batch in flight and fills its outs[] (and label8[] buffers). While batch N runs,
@@ -253,6 +272,10 @@ int urf_process_cloud2_batch(urf_ctx* ctx, const void* const* data, const int* n
 int urf_enqueue_batch(urf_ctx* ctx, const float* const* xyzi, const int* n, int batch, urf_result* outs, int8_t* const* label8);
 int urf_enqueue_cloud2_batch(urf_ctx* ctx, const void* const* data, const int* n_points, int batch, int point_step, int off_x,
                              int off_y, int off_z, int off_intensity, urf_result* outs, int8_t* const* label8);
+/* urf_process_cloud2_batch_mixed without waiting: finished by urf_finish_batch, two batches in flight as above. The fmt
+ * array is read during the call only. */
+int urf_enqueue_cloud2_batch_mixed(urf_ctx* ctx, const void* const* data, const int* n_points, const urf_cloud2_format* fmt,
+                                   int batch, urf_result* outs, int8_t* const* label8);
 int urf_finish_batch(urf_ctx* ctx);
 
 /* Device-resident variant used to time the kernels without PCIe: d_xyzi is a DEVICE pointer to the scans stored back to
@@ -432,6 +455,39 @@ int urf_queue_create_cloud2_with(urf_queue** out, urf_queue_process_fn fn, void*
                                  int policy, int point_step, int off_x, int off_y, int off_z, int off_intensity);
 
 /*
+ * A queue for the PointCloud2 records of SEVERAL sensor formats (one queue for every LiDAR of a vehicle): a table of
+ * 1..URF_MAX_FORMATS formats at creation (each passes urf_queue_create_cloud2's checks, URF_ERR_INVALID otherwise), and each
+ * submit names its scan's format by its index in the table. The worker runs what is pending through
+ * urf_enqueue_cloud2_batch_mixed, so a batch mixes formats freely (never parameter generations), and every result is bit for
+ * bit what urf_process_cloud2_batch gives for that scan alone in its own format. A float4 producer shares the queue by
+ * registering {16, 0, 4, 8, 12}.
+ *   - Slots hold max_points * (the table's largest point_step) bytes each.
+ *   - urf_queue_submit_format copies n_points records of format `fmt` into a slot; urf_queue_submit_format_ref uses them in
+ *     place, with urf_queue_submit_cloud2_ref's lifetime contract. fmt outside the table: URF_ERR_INVALID; n_points >
+ *     max_points: URF_ERR_CAPACITY.
+ *   - A formats queue refuses urf_queue_submit, urf_queue_submit_ref and urf_queue_submit_cloud2* (URF_ERR_INVALID), and every
+ *     other queue refuses the _format submits.
+ *   - Policy, delivery (urf_queue_next / _next_view / _next_batch, URF_QUEUE_LABEL8, URF_QUEUE_ORDER), DROP_OLDEST,
+ *     urf_queue_update_params generations, the ctx's tie order, stats, close and destroy are those of a record queue.
+ */
+int urf_queue_create_formats(urf_queue** out, urf_ctx* ctx, int max_points, int slots, int max_batch, int policy,
+                             const urf_cloud2_format* formats, int n_formats);
+int urf_queue_submit_format(urf_queue* q, int fmt, const void* data, int n_points, uint64_t tag, int timeout_ms);
+int urf_queue_submit_format_ref(urf_queue* q, int fmt, const void* data, int n_points, uint64_t tag, int timeout_ms);
+/* Test hook: a formats queue around a synchronous stand-in, as urf_queue_create_cloud2_with. xyzi[b] points at scan b's raw
+ * bytes (the queue's slot, or the caller's buffer after urf_queue_submit_format_ref). The batch function's `user`, and the
+ * parameter hook's, is a urf_formats_user the queue owns, valid until urf_queue_destroy: the creator's `user`, the format
+ * table (the queue's copy) and `fmt`, which during a batch call points at the format index of each of its scans. */
+typedef struct urf_formats_user {
+  void*                    user;           /* the creator's `user` (urf_mq_create_formats_with: users[j] for device j, or NULL) */
+  const urf_cloud2_format* formats;        /* [n_formats] */
+  int32_t                  n_formats;
+  const int32_t*           fmt;            /* [batch]: fmt[b] is scan b's index into formats; valid during the call only */
+} urf_formats_user;
+int urf_queue_create_formats_with(urf_queue** out, urf_queue_process_fn fn, void* user, int max_points, int slots, int max_batch,
+                                  int policy, const urf_cloud2_format* formats, int n_formats);
+
+/*
  * Multi-GPU ingest (BASELINE config 4: one continuous scan stream sharded across the GPUs of a box). The reference is one
  * subscriber in one process (lidar_segmentation.cpp:53); urf_mq is one submit / next interface over N devices: it creates
  * a context and a urf_queue (above) per device, hands every scan to the device with the fewest scans in flight, and
@@ -502,6 +558,22 @@ int urf_mq_create_with_policy(urf_mq** out, urf_queue_process_fn fn, void* const
 int urf_mq_create_cloud2_with(urf_mq** out, urf_queue_process_fn fn, void* const* users, int n_devices, int max_points,
                               int slots_per_device, int max_batch, int policy, int point_step, int off_x, int off_y, int off_z,
                               int off_intensity);
+/* urf_mq_create_policy whose device queues are urf_queue_create_formats queues of one format table: one context, one worker
+ * and one set of pinned slots per device carry every sensor format, and the scans of all of them share one device choice
+ * and one delivery order. Table and policy checks as urf_queue_create_formats and urf_mq_create_policy, made before any
+ * device is set up. urf_mq_submit_format / _format_ref name the scan's format as urf_queue_submit_format does (same
+ * refusals); a formats mq refuses urf_mq_submit, urf_mq_submit_ref and urf_mq_submit_cloud2*, and every other mq the _format
+ * submits. Device choice, delivery, generations, urf_mq_set_tie_order, stats, close and destroy are those of a record mq, and
+ * every result is bit for bit what urf_process_cloud2_batch gives for that scan alone in its own format. */
+int urf_mq_create_formats(urf_mq** out, const int* devices, int n_devices, int max_points, int slots_per_device, int max_batch,
+                          const urf_params* params /* or NULL: cfg defaults */, int policy, const urf_cloud2_format* formats,
+                          int n_formats);
+int urf_mq_submit_format(urf_mq* mq, int fmt, const void* data, int n_points, uint64_t tag, int timeout_ms);
+int urf_mq_submit_format_ref(urf_mq* mq, int fmt, const void* data, int n_points, uint64_t tag, int timeout_ms);
+/* Test hook: urf_mq_create_formats over N stand-in devices, each a urf_queue_create_formats_with queue around fn (its
+ * urf_formats_user carries users[j] for device j). */
+int urf_mq_create_formats_with(urf_mq** out, urf_queue_process_fn fn, void* const* users, int n_devices, int max_points,
+                               int slots_per_device, int max_batch, int policy, const urf_cloud2_format* formats, int n_formats);
 /* Test hook: urf_queue_set_params_hook on every stand-in device (fn gets users[j] for device j). URF_ERR_INVALID on real devices. */
 int urf_mq_set_params_hook(urf_mq* mq, urf_queue_params_fn fn);
 

@@ -11,8 +11,8 @@ import os
 import numpy as np
 
 from .ctypes_abi import (UrfMqStats, QUEUE_FINISH_FN, QUEUE_PARAMS_FN, QUEUE_PROCESS_FN, URF_ERR_CLOSED, URF_ERR_TIMEOUT, URF_MAX_CHANNELS, URF_MAX_VERTS, URF_OK, URF_QUEUE_BLOCK,
-                         URF_QUEUE_DROP_OLDEST, URF_QUEUE_LABEL8, URF_QUEUE_ORDER, URF_TOO_FEW_POINTS, UrfClouds, UrfParams, UrfQueueStats, UrfResult,
-                         UrfStrip, make_params)
+                         URF_QUEUE_DROP_OLDEST, URF_QUEUE_LABEL8, URF_QUEUE_ORDER, URF_TOO_FEW_POINTS, UrfClouds, UrfCloud2Format, UrfParams,
+                         UrfQueueStats, UrfResult, UrfStrip, make_params)
 
 LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "liburf_b200.so")
 
@@ -28,7 +28,19 @@ EXPORTS = ["urf_queue_next_batch", "urf_mq_next_batch", "urf_mq_create_label8", 
            "urf_set_params_next", "urf_queue_update_params", "urf_mq_update_params", "urf_queue_set_params_hook",
            "urf_mq_set_params_hook", "urf_mq_create_policy", "urf_mq_create_with_policy", "urf_queue_submit_cloud2_ref",
            "urf_queue_create_cloud2_with", "urf_mq_create_cloud2", "urf_mq_create_cloud2_with", "urf_mq_submit_cloud2",
-           "urf_mq_submit_cloud2_ref"]
+           "urf_mq_submit_cloud2_ref", "urf_process_cloud2_batch_mixed", "urf_enqueue_cloud2_batch_mixed", "urf_queue_create_formats",
+           "urf_queue_create_formats_with", "urf_queue_submit_format", "urf_queue_submit_format_ref", "urf_mq_create_formats",
+           "urf_mq_create_formats_with", "urf_mq_submit_format", "urf_mq_submit_format_ref"]
+
+# One PointCloud2 record format (include/urf.h urf_cloud2_format): what a message's point_step and `fields` give. A float4 scan
+# is CloudFormat(16, 0, 4, 8, 12).
+CloudFormat = collections.namedtuple("CloudFormat", "point_step off_x off_y off_z off_intensity")
+FLOAT4_FORMAT = CloudFormat(16, 0, 4, 8, 12)
+
+
+def _format_array(formats):
+    """A ctypes urf_cloud2_format array of `formats` (CloudFormat or 5-tuples)."""
+    return (UrfCloud2Format * len(formats))(*[UrfCloud2Format(*(int(v) for v in f)) for f in formats])
 
 # urf_set_tie_order modes (include/urf.h): equal azimuths inside a ring in input order, or in the reference's Lomuto order
 TIE_ORDERS = {"input": 0, "reference": 1}
@@ -125,6 +137,15 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
     lib.urf_mq_create_cloud2_with.argtypes = [C.POINTER(vp), QUEUE_PROCESS_FN, C.POINTER(vp), ip, ip, ip, ip, ip, ip, ip, ip, ip, ip]
     lib.urf_mq_submit_cloud2.argtypes = [vp, vp, ip, C.c_uint64, ip]
     lib.urf_mq_submit_cloud2_ref.argtypes = [vp, vp, ip, C.c_uint64, ip]
+    fp = C.POINTER(UrfCloud2Format)
+    lib.urf_process_cloud2_batch_mixed.argtypes = [vp, C.POINTER(vp), C.POINTER(ip), fp, ip, C.POINTER(UrfResult), C.POINTER(vp)]
+    lib.urf_enqueue_cloud2_batch_mixed.argtypes = [vp, C.POINTER(vp), C.POINTER(ip), fp, ip, C.POINTER(UrfResult), C.POINTER(vp)]
+    lib.urf_queue_create_formats.argtypes = [C.POINTER(vp), vp, ip, ip, ip, ip, fp, ip]
+    lib.urf_queue_create_formats_with.argtypes = [C.POINTER(vp), QUEUE_PROCESS_FN, vp, ip, ip, ip, ip, fp, ip]
+    lib.urf_mq_create_formats.argtypes = [C.POINTER(vp), C.POINTER(ip), ip, ip, ip, ip, C.POINTER(UrfParams), ip, fp, ip]
+    lib.urf_mq_create_formats_with.argtypes = [C.POINTER(vp), QUEUE_PROCESS_FN, C.POINTER(vp), ip, ip, ip, ip, ip, fp, ip]
+    for name in ("urf_queue_submit_format", "urf_queue_submit_format_ref", "urf_mq_submit_format", "urf_mq_submit_format_ref"):
+        getattr(lib, name).argtypes = [vp, ip, vp, ip, C.c_uint64, ip]
     batch_args = [vp, ip, C.POINTER(C.c_uint64), C.POINTER(C.c_int32), C.POINTER(UrfResult), C.POINTER(vp), ip]
     lib.urf_queue_next_batch.argtypes = batch_args
     lib.urf_queue_next_view.argtypes = [vp, C.POINTER(C.c_uint64), C.POINTER(UrfResult), C.POINTER(vp), ip]
@@ -208,13 +229,15 @@ class BatchHandle:
     batch's copies run asynchronously; a copy from or to pageable memory makes the enqueue wait for it. Allocating
     page-locked memory can wait for the device: build handles before enqueueing if batches are to overlap. A handle can be
     enqueued again once it is finished (collect copies the results out); its page-locked memory is freed by free() or when
-    the handle is dropped. want_label=False: no label buffers (a call whose caller does not read the labels)."""
+    the handle is dropped. want_label=False: no label buffers (a call whose caller does not read the labels). formats (one
+    CloudFormat per scan, or None): a batch of mixed record formats (urf_*_cloud2_batch_mixed); step and offs are then unused."""
 
     def __init__(self, inputs, ns, want_ring: bool, want_order: bool, label8: bool, step: int = 0, offs=(0, 4, 8, -1),
-                 pinned: bool = False, want_label: bool = True):
+                 pinned: bool = False, want_label: bool = True, formats=None):
         B = len(inputs)
         self.lib = load_library()
         self.step, self.offs, self.pinned = step, tuple(offs), pinned
+        self.fmts = None if formats is None else _format_array(formats)
         self._pins = []
         self.inputs = [self._array(a) for a in inputs] if pinned else inputs
         self.ptrs = (C.c_void_p * B)(*[a.ctypes.data for a in self.inputs])
@@ -265,6 +288,15 @@ class BatchHandle:
         raws = [np.ascontiguousarray(r).view(np.uint8).reshape(-1) for r in records]
         return cls(raws, [r.size // point_step for r in raws], want_ring, want_order, label8, point_step,
                    (off_x, off_y, off_z, off_intensity), pinned)
+
+    @classmethod
+    def of_mixed(cls, records, formats, want_ring: bool, want_order: bool, label8: bool, pinned: bool = False) -> "BatchHandle":
+        """A batch of raw PointCloud2 record arrays where records[b] has the format formats[b] (CloudFormat or 5-tuple)."""
+        if len(records) != len(formats):
+            raise ValueError(f"{len(records)} scans but {len(formats)} formats")
+        raws = [np.ascontiguousarray(r).view(np.uint8).reshape(-1) for r in records]
+        return cls(raws, [r.size // int(f[0]) for r, f in zip(raws, formats)], want_ring, want_order, label8, pinned=pinned,
+                   formats=[CloudFormat(*(int(v) for v in f)) for f in formats])
 
     def collect(self) -> list[ScanResult]:
         """ScanResults of the finished call: labels as int32 (int8 ones widened), ring cut to n_in; copies of page-locked
@@ -378,14 +410,28 @@ class Detector:
                                                           hb.l8), "urf_process_cloud2_batch")
         return hb.collect()
 
+    def filtered_batch_mixed(self, records, formats, want_order: bool = False, label8: bool = True,
+                             want_ring: bool = False) -> list[ScanResult]:
+        """filtered_batch_records for a batch of several sensor formats: records[b] (uint8 record bytes) has the format
+        formats[b] (CloudFormat or (point_step, off_x, off_y, off_z, off_intensity)); one unpack launch for the whole batch
+        (urf_process_cloud2_batch_mixed). Every result is what filtered_batch_records gives for that scan alone."""
+        hb = BatchHandle.of_mixed(records, formats, want_ring, want_order, label8)
+        self._check(self.lib.urf_process_cloud2_batch_mixed(self._ctx, hb.ptrs, hb.ns, hb.fmts, len(hb.ns), hb.res, hb.l8),
+                    "urf_process_cloud2_batch_mixed")
+        return hb.collect()
+
     def enqueue(self, hb: "BatchHandle") -> "BatchHandle":
-        """Enqueues a prepared batch (BatchHandle.of_clouds / of_records; urf_enqueue_batch / urf_enqueue_cloud2_batch) and
+        """Enqueues a prepared batch (BatchHandle.of_clouds / of_records / of_mixed; urf_enqueue_batch /
+        urf_enqueue_cloud2_batch / urf_enqueue_cloud2_batch_mixed) and
         returns at once when its buffers are pinned. finish_batch fills its `results`. At most two batches are in flight;
         the detector keeps the handle alive until then. While batches are in flight every other compute call and
         set_params / set_tie_order / set_option raise (URF_ERR_INVALID); set_params_next changes the set of the next
         enqueue."""
         B = len(hb.ns)
-        if hb.step == 0:
+        if hb.fmts is not None:
+            rc, where = (self.lib.urf_enqueue_cloud2_batch_mixed(self._ctx, hb.ptrs, hb.ns, hb.fmts, B, hb.res, hb.l8),
+                         "urf_enqueue_cloud2_batch_mixed")
+        elif hb.step == 0:
             rc, where = self.lib.urf_enqueue_batch(self._ctx, hb.ptrs, hb.ns, B, hb.res, hb.l8), "urf_enqueue_batch"
         else:
             rc, where = self.lib.urf_enqueue_cloud2_batch(self._ctx, hb.ptrs, hb.ns, B, hb.step, *hb.offs, hb.res, hb.l8), "urf_enqueue_cloud2_batch"
@@ -520,7 +566,10 @@ class _StreamQueue:
     `_PREFIX` + name (urf_queue_* or urf_mq_*), which have the same arguments in both families."""
     _PREFIX = ""
 
-    def __init__(self, max_points: int, label8: bool, params: UrfParams | None = None, order: bool = False, records=None):
+    def __init__(self, max_points: int, label8: bool, params: UrfParams | None = None, order: bool = False, records=None,
+                 formats=None):
+        if records is not None and formats is not None:
+            raise ValueError("records and formats: a queue takes one record format or a table of them")
         self.lib = load_library()
         self._h = C.c_void_p()
         self.max_points = max_points
@@ -528,6 +577,9 @@ class _StreamQueue:
         self.order = order                # URF_QUEUE_ORDER: results carry order and ring_start
         # record queue: (point_step, off_x, off_y, off_z, off_intensity) of its PointCloud2 records; None: float4 scans
         self.records = None if records is None else tuple(int(v) for v in records)
+        # formats queue: its table of CloudFormats (urf_*_create_formats), each submit_records naming one by index
+        self.formats = None if formats is None else [CloudFormat(*(int(v) for v in f)) for f in formats]
+        self._fmt_table = None if formats is None else _format_array(self.formats)
         self._cb = None                   # ctypes callbacks of a stand-in, kept alive with the queue
         self._params_cb = None            # the parameter hook of a stand-in
         self._bufs = None
@@ -571,18 +623,26 @@ class _StreamQueue:
             raise UrfError(rc, self._PREFIX + "submit")
         return rc
 
-    def submit_records(self, data, n_points: int, tag: int = 0, timeout_ms: int = -1, by_reference: bool = False) -> int:
+    def submit_records(self, data, n_points: int, tag: int = 0, timeout_ms: int = -1, by_reference: bool = False,
+                       fmt: int | None = None) -> int:
         """A scan of a record queue: the raw `data` bytes of a sensor_msgs/PointCloud2 (bytes, bytearray or an array), of
         which the first n_points records count (urf_queue_submit_cloud2 / urf_mq_submit_cloud2). Returns as submit, and
         raises UrfError(URF_ERR_INVALID) on a float4 queue. by_reference: no copy (urf_*_submit_cloud2_ref): keep `data`
-        alive and unchanged until its result has come back."""
+        alive and unchanged until its result has come back. fmt: the scan's index into the table of a formats queue
+        (urf_*_submit_format[_ref]); the library refuses it on any other queue, and a formats queue refuses fmt=None."""
         raw = np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray)) else np.ascontiguousarray(data).view(np.uint8).reshape(-1)
-        if self.records is not None and raw.size < n_points * self.records[0]:
-            raise ValueError(f"{raw.size} bytes hold fewer than {n_points} records of {self.records[0]} bytes")
+        step = (self.records[0] if self.records is not None and fmt is None else
+                self.formats[fmt].point_step if self.formats is not None and fmt is not None and 0 <= fmt < len(self.formats) else 0)
+        if raw.size < n_points * step:
+            raise ValueError(f"{raw.size} bytes hold fewer than {n_points} records of {step} bytes")
         if by_reference:
             self._keep[tag] = raw
-        name = "submit_cloud2_ref" if by_reference else "submit_cloud2"
-        rc = self._call(name, raw.ctypes.data, n_points, tag, timeout_ms)
+        if fmt is None:
+            name = "submit_cloud2_ref" if by_reference else "submit_cloud2"
+            rc = self._call(name, raw.ctypes.data, n_points, tag, timeout_ms)
+        else:
+            name = "submit_format_ref" if by_reference else "submit_format"
+            rc = self._call(name, fmt, raw.ctypes.data, n_points, tag, timeout_ms)
         if rc not in (URF_OK, URF_ERR_TIMEOUT, URF_ERR_CLOSED):
             raise UrfError(rc, self._PREFIX + name)
         return rc
@@ -642,23 +702,25 @@ class MultiGpuQueue(_StreamQueue):
     every scan goes to the device with the fewest scans in flight, results come back in submission order. Any number of
     producer threads, one consumer. `by_reference` submits hand the array to the library without a copy: keep it alive and
     unchanged until its result has come back. label8: int8 label slots on every device, order: the emission order and ring
-    offsets with every result, records: a record mq (urf_mq_create_cloud2) fed with submit_records (see ScanQueue)."""
+    offsets with every result, records: a record mq (urf_mq_create_cloud2) fed with submit_records (see ScanQueue), formats:
+    a formats mq (urf_mq_create_formats) whose submit_records name each scan's format (see ScanQueue)."""
     _PREFIX = "urf_mq_"
     _m = property(lambda self: self._h)      # the library handle, under the name this class has always had for it
 
     def __init__(self, devices, max_points: int, slots_per_device: int = 8, max_batch: int = 4, params: UrfParams | None = None,
-                 process_fn=None, label8: bool = False, order: bool = False, records=None):
+                 process_fn=None, label8: bool = False, order: bool = False, records=None, formats=None):
         super().__init__(max_points, label8, None if process_fn is not None else params if params is not None else make_params(), order,
-                         records)
+                         records, formats)
         policy = URF_QUEUE_BLOCK | (URF_QUEUE_LABEL8 if label8 else 0) | (URF_QUEUE_ORDER if order else 0)
-        fmt = self.records or ()
+        fmt = self.records or (() if formats is None else (self._fmt_table, len(self.formats)))
+        kind = "cloud2" if self.records else "formats" if formats is not None else "policy"
         if process_fn is not None:                      # tests: stand-in devices, no GPU
             self._cb = QUEUE_PROCESS_FN(process_fn)
-            create = self.lib.urf_mq_create_cloud2_with if fmt else self.lib.urf_mq_create_with_policy
+            create = getattr(self.lib, "urf_mq_create_with_policy" if kind == "policy" else f"urf_mq_create_{kind}_with")
             rc = create(C.byref(self._h), self._cb, None, len(devices), max_points, slots_per_device, max_batch, policy, *fmt)
         else:
             dv = (C.c_int * len(devices))(*devices)
-            create = self.lib.urf_mq_create_cloud2 if fmt else self.lib.urf_mq_create_policy
+            create = getattr(self.lib, f"urf_mq_create_{kind}")
             rc = create(C.byref(self._h), dv, len(devices), max_points, slots_per_device, max_batch,
                         C.byref(params) if params is not None else None, policy, *fmt)
         if rc != URF_OK:
@@ -696,33 +758,36 @@ class ScanQueue(_StreamQueue):
     "road_probably") works on it; the batches then run the ring sort and copy 4 bytes per point more. records
     (point_step, off_x, off_y, off_z, off_intensity): a queue of raw PointCloud2 records of that one format
     (urf_queue_create_cloud2, or urf_queue_create_cloud2_with around process_fn), fed with submit_records and unpacked on
-    the device; `submit` then raises, as submit_records does on a float4 queue."""
+    the device; `submit` then raises, as submit_records does on a float4 queue. formats (a list of CloudFormat or 5-tuples,
+    1..URF_MAX_FORMATS): a queue of several record formats (urf_queue_create_formats[_with]); submit_records(..., fmt=k)
+    names each scan's format, and batches mix formats."""
     _PREFIX = "urf_queue_"
     _q = property(lambda self: self._h)      # the library handle, under the name this class has always had for it
 
     def __init__(self, detector: "Detector | None", max_points: int, slots: int = 8, max_batch: int = 4,
                  policy: int = URF_QUEUE_BLOCK, process_fn=None, label8: bool = False, enqueue_fn=None, finish_fn=None,
-                 order: bool = False, records=None):
+                 order: bool = False, records=None, formats=None):
         order = order or bool(policy & URF_QUEUE_ORDER)
-        super().__init__(max_points, label8, detector.params if detector is not None else None, order, records)
-        fmt = self.records or ()
+        super().__init__(max_points, label8, detector.params if detector is not None else None, order, records, formats)
+        fmt = self.records or (() if formats is None else (self._fmt_table, len(self.formats)))
+        kind = "_cloud2" if self.records else "_formats" if formats is not None else ""
         if label8:
             policy |= URF_QUEUE_LABEL8
         if order:
             policy |= URF_QUEUE_ORDER
         if enqueue_fn is not None:
             if fmt:
-                raise ValueError("records: a record queue has no asynchronous stand-in")
+                raise ValueError("records / formats: a record queue has no asynchronous stand-in")
             self._cb = (QUEUE_PROCESS_FN(enqueue_fn), QUEUE_FINISH_FN(lambda user: finish_fn()))
             rc = self.lib.urf_queue_create_with_async(C.byref(self._h), *self._cb, None, max_points, slots, max_batch, policy)
         elif process_fn is not None:
             self._cb = QUEUE_PROCESS_FN(process_fn)
-            create = self.lib.urf_queue_create_cloud2_with if fmt else self.lib.urf_queue_create_with
+            create = getattr(self.lib, f"urf_queue_create{kind}_with")
             rc = create(C.byref(self._h), self._cb, None, max_points, slots, max_batch, policy, *fmt)
         else:
             assert detector is not None and detector.max_batch >= max_batch and detector.max_points >= max_points
             self._det = detector          # keeps the ctx alive; nobody else may use it while the queue exists
-            create = self.lib.urf_queue_create_cloud2 if fmt else self.lib.urf_queue_create
+            create = getattr(self.lib, f"urf_queue_create{kind}")
             rc = create(C.byref(self._h), detector._ctx, max_points, slots, max_batch, policy, *fmt)
         if rc != URF_OK:
             raise UrfError(rc, "urf_queue_create")

@@ -94,14 +94,16 @@ def build_kat() -> None:
     # ThreadSanitizer build of the streaming queue around a stand-in batch function (no CUDA involved)
     tgt = os.path.join(bdir, "queue_stress")
     qsrc = [os.path.join(kat, "queue_stress.cpp"), os.path.join(CSRC, "urf_queue.cpp"), os.path.join(CSRC, "urf_mq.cpp"),
-            os.path.join(kat, "queue_async_stubs.cpp"), os.path.join(kat, "queue_params_stubs.cpp")]
+            os.path.join(kat, "queue_async_stubs.cpp"), os.path.join(kat, "queue_params_stubs.cpp"), os.path.join(kat, "queue_formats_stubs.cpp")]
     qdeps = [os.path.join(ROOT, "include", "urf.h"), os.path.join(CSRC, "urf_queue_internal.hpp"), os.path.join(CSRC, "urf_params.hpp")]
     if _stale(tgt, qsrc + qdeps):
         subprocess.run(["g++", "-std=c++17", "-O1", "-g", "-fsanitize=thread", "-pthread", "-o", tgt, *qsrc], check=True)
     # the same for batched delivery (urf_queue_next_batch / urf_mq_next_batch) and int8 label slots, for the worker's
     # two-batches-in-flight schedule around an asynchronous stand-in, for parameter updates on a running queue, and for
-    # the emission order delivered with URF_QUEUE_ORDER, and for PointCloud2 records through the multi-GPU queue
-    for name in ("queue_batch_stress", "queue_async_stress", "queue_params_stress", "queue_order_stress", "mq_records_stress"):
+    # the emission order delivered with URF_QUEUE_ORDER, for PointCloud2 records through the multi-GPU queue, and for records
+    # of several formats in one stream
+    for name in ("queue_batch_stress", "queue_async_stress", "queue_params_stress", "queue_order_stress", "mq_records_stress",
+                 "queue_formats_stress"):
         tgt = os.path.join(bdir, name)
         src = [os.path.join(kat, name + ".cpp")] + qsrc[1:]
         if _stale(tgt, src + qdeps):

@@ -70,7 +70,11 @@ struct urf_ctx {
     // urf_create, so single scans never allocate; re-allocated at P * step bytes by the first batch that needs more
     DevMem<unsigned char> rawb;
     size_t rawb_bytes = 0;
-    DevMem<int> ring;                  // ring ids for the caller; none in slot 0 before the first asynchronous call: the sort
+    // per-scan record formats of a mixed batch (urf_*_cloud2_batch_mixed), max_batch entries each, allocated by the slot's
+    // first mixed batch; the chunks copy their slices on s_in with their point counts
+    DevMem<urf_cloud2_format> fmt;
+    HostMem<urf_cloud2_format> h_fmt;
+    DevMem<int> ring;                 // ring ids for the caller; none in slot 0 before the first asynchronous call: the sort
                                        // scratch (buf.sortbuf) takes them, see ring_chunk
     HostMem<int> h_n; HostMem<ScanOut> h_out;   // pinned copies of n and out
     Event ev0, ev1, ev_done;           // bracket the batch's kernels; after its last copy to the host
@@ -635,21 +639,40 @@ namespace {
 // Shared body of the host-buffer batch entry points. step == 0: data[b] holds n[b] (x, y, z, intensity) float4 records that
 // are copied straight into the input buffer; step > 0: data[b] holds n[b] records of `step` bytes with FLOAT32 x / y / z /
 // intensity at the given byte offsets (oi < 0: none) — the raw bytes cross PCIe and are unpacked on the device.
+// fmt (or NULL): scan b's records have the format fmt[b] instead (step and the offsets are then ignored); a batch whose
+// formats are all equal runs as the one-format call.
 // label8 (or NULL): per scan an int8 HOST buffer for the labels (one byte per point instead of four).
 // clouds (or NULL, batch == 1 only): the four published clouds of the scan, packed on the device.
 // Enqueues the batch into the next free host slot and returns; finish_batch waits for it and fills outs.
 int enqueue_batch(urf_ctx* ctx, const void* const* data, const int* n, int batch, int step, int ox, int oy, int oz, int oi,
-                  urf_result* outs, int8_t* const* label8, urf_clouds* clouds) {
+                  const urf_cloud2_format* fmt, urf_result* outs, int8_t* const* label8, urf_clouds* clouds) {
   if (!ctx || !data || !n || !outs || batch < 1) return URF_ERR_INVALID;
   if (batch > ctx->max_batch || ctx->hs_count == 2) return URF_ERR_CAPACITY;
-  if (step != 0) {
-    if (step < 12 || step > URF_MAX_POINT_STEP) return URF_ERR_INVALID;
-    for (int o : {ox, oy, oz}) if (o < 0 || o + 4 > step) return URF_ERR_INVALID;
-    if (oi >= 0 && oi + 4 > step) return URF_ERR_INVALID;
+  if (fmt) {                                                  // step becomes the batch's largest point_step
+    bool mixed = false;
+    step = 0;
+    for (int b = 0; b < batch; b++) {
+      if (urf::check_cloud2_format(fmt[b]) != URF_OK) return URF_ERR_INVALID;
+      step = std::max(step, (int)fmt[b].point_step);
+      mixed |= std::memcmp(&fmt[b], &fmt[0], sizeof(urf_cloud2_format)) != 0;
+    }
+    ox = fmt[0].off_x; oy = fmt[0].off_y; oz = fmt[0].off_z; oi = fmt[0].off_intensity;
+    if (!mixed) fmt = nullptr;
+  } else if (step != 0 && urf::check_cloud2_format(step, ox, oy, oz, oi) != URF_OK) {
+    return URF_ERR_INVALID;
   }
   CK(cudaSetDevice(ctx->device));
   const int slot = (ctx->hs_head + ctx->hs_count) % 2;
   urf_ctx::HostSlot& h = ctx->hs[slot];                       // free: its last batch was finished, its copies are done
+  if (fmt && !h.fmt) {                                        // the slot's first mixed batch: its format tables
+    DevMem<urf_cloud2_format> d;
+    HostMem<urf_cloud2_format> hf;
+    int rc = dalloc(ctx, d, (size_t)ctx->max_batch);
+    if (rc == URF_OK) rc = cuda_rc(ctx, new_pinned(hf, (size_t)ctx->max_batch), "cudaMallocHost");
+    if (rc != URF_OK) return rc;
+    h.fmt = std::move(d); h.h_fmt = std::move(hf);
+  }
+  if (fmt) std::memcpy(h.h_fmt.get(), fmt, sizeof(urf_cloud2_format) * (size_t)batch);
   int nmax = 1;
   bool want_order = clouds != nullptr, want_ring = false, want_l8 = false;
   for (int b = 0; b < batch; b++) {
@@ -716,10 +739,12 @@ int enqueue_batch(urf_ctx* ctx, const void* const* data, const int* n, int batch
   for (int c = 0; c < nchunks; c++) {
     const int b0 = cb[c], nb = cb[c + 1] - b0;
     CK(cudaMemcpyAsync(scan_view(bufv, b0, e).n, h.h_n.get() + b0, sizeof(int) * nb, cudaMemcpyHostToDevice, ctx->s_in.get()));
+    if (fmt) CK(cudaMemcpyAsync(h.fmt.get() + b0, h.h_fmt.get() + b0, sizeof(urf_cloud2_format) * nb, cudaMemcpyHostToDevice, ctx->s_in.get()));
     for (int b = b0; b < b0 + nb; b++) {
       if (n[b] <= 0) continue;
+      const size_t bytes = (size_t)(fmt ? fmt[b].point_step : step) * (size_t)n[b];
       if (step == 0) CK(cudaMemcpyAsync(scan_view(bufv, b, e).in, data[b], sizeof(float) * 4 * (size_t)n[b], cudaMemcpyHostToDevice, ctx->s_in.get()));
-      else CK(cudaMemcpyAsync(h.rawb.get() + b * pts * step, data[b], (size_t)step * (size_t)n[b], cudaMemcpyHostToDevice, ctx->s_in.get()));
+      else CK(cudaMemcpyAsync(h.rawb.get() + b * pts * step, data[b], bytes, cudaMemcpyHostToDevice, ctx->s_in.get()));
     }
     CK(cudaEventRecord(ctx->ev_in[c].get(), ctx->s_in.get()));
   }
@@ -729,7 +754,8 @@ int enqueue_batch(urf_ctx* ctx, const void* const* data, const int* n, int batch
     CK(cudaStreamWaitEvent(st, ctx->ev_in[c].get(), 0));
     const DevBuffers view = scan_view(bufv, b0, e);
     if (step != 0)
-      k_unpack_cloud2_batch<<<dim3((S + 255) / 256, nb), 256, 0, st>>>(h.rawb.get() + b0 * pts * step, view.in, view.n, S, step, ox, oy, oz, oi);
+      k_unpack_cloud2_batch<<<dim3((S + 255) / 256, nb), 256, 0, st>>>(h.rawb.get() + b0 * pts * step, view.in, view.n, S, step,
+                                                                        urf_cloud2_format{step, ox, oy, oz, oi}, fmt ? h.fmt.get() + b0 : nullptr);
     // ev0 / ev1 bracket the kernels of the whole call: before the first chunk's pipeline, after the last one's
     int L = graphed ? ctx->g_launches : 0;
     int rc = c == 0 ? cuda_rc(ctx, cudaEventRecord(h.ev0.get(), st), "cudaEventRecord(ev0)") : URF_OK;
@@ -831,56 +857,69 @@ int alloc_second_slot(urf_ctx* ctx) {
 
 // The synchronous entry points: one enqueue and one finish, refused while asynchronous batches are in flight.
 int process_batch_impl(urf_ctx* ctx, const void* const* data, const int* n, int batch, int step, int ox, int oy, int oz, int oi,
-                       urf_result* outs, int8_t* const* label8, urf_clouds* clouds) {
+                       const urf_cloud2_format* fmt, urf_result* outs, int8_t* const* label8, urf_clouds* clouds) {
   if (ctx && ctx->hs_count) return URF_ERR_INVALID;
-  const int rc = enqueue_batch(ctx, data, n, batch, step, ox, oy, oz, oi, outs, label8, clouds);
+  const int rc = enqueue_batch(ctx, data, n, batch, step, ox, oy, oz, oi, fmt, outs, label8, clouds);
   return rc != URF_OK ? rc : finish_batch(ctx);
 }
 
 int enqueue_async(urf_ctx* ctx, const void* const* data, const int* n, int batch, int step, int ox, int oy, int oz, int oi,
-                  urf_result* outs, int8_t* const* label8) {
+                  const urf_cloud2_format* fmt, urf_result* outs, int8_t* const* label8) {
   if (!ctx) return URF_ERR_INVALID;
   const int rc = alloc_second_slot(ctx);
-  return rc != URF_OK ? rc : enqueue_batch(ctx, data, n, batch, step, ox, oy, oz, oi, outs, label8, nullptr);
+  return rc != URF_OK ? rc : enqueue_batch(ctx, data, n, batch, step, ox, oy, oz, oi, fmt, outs, label8, nullptr);
 }
 }  // namespace
 
 int urf_enqueue_batch(urf_ctx* ctx, const float* const* xyzi, const int* n, int batch, urf_result* outs, int8_t* const* label8) {
-  return enqueue_async(ctx, reinterpret_cast<const void* const*>(xyzi), n, batch, 0, 0, 0, 0, -1, outs, label8);
+  return enqueue_async(ctx, reinterpret_cast<const void* const*>(xyzi), n, batch, 0, 0, 0, 0, -1, nullptr, outs, label8);
 }
 
 int urf_enqueue_cloud2_batch(urf_ctx* ctx, const void* const* data, const int* n_points, int batch, int point_step, int off_x, int off_y,
                              int off_z, int off_intensity, urf_result* outs, int8_t* const* label8) {
   if (point_step == 0) return URF_ERR_INVALID;
-  return enqueue_async(ctx, data, n_points, batch, point_step, off_x, off_y, off_z, off_intensity, outs, label8);
+  return enqueue_async(ctx, data, n_points, batch, point_step, off_x, off_y, off_z, off_intensity, nullptr, outs, label8);
+}
+
+// the mixed entry points take their step and offsets from fmt; a batch of one format runs as the one-format call
+int urf_enqueue_cloud2_batch_mixed(urf_ctx* ctx, const void* const* data, const int* n_points, const urf_cloud2_format* fmt, int batch,
+                                   urf_result* outs, int8_t* const* label8) {
+  if (!fmt) return URF_ERR_INVALID;
+  return enqueue_async(ctx, data, n_points, batch, 0, 0, 0, 0, -1, fmt, outs, label8);
+}
+
+int urf_process_cloud2_batch_mixed(urf_ctx* ctx, const void* const* data, const int* n_points, const urf_cloud2_format* fmt, int batch,
+                                   urf_result* outs, int8_t* const* label8) {
+  if (!fmt) return URF_ERR_INVALID;
+  return process_batch_impl(ctx, data, n_points, batch, 0, 0, 0, 0, -1, fmt, outs, label8, nullptr);
 }
 
 int urf_finish_batch(urf_ctx* ctx) { return finish_batch(ctx); }
 
 int urf_process_batch(urf_ctx* ctx, const float* const* xyzi, const int* n, int batch, urf_result* outs) {
-  return process_batch_impl(ctx, reinterpret_cast<const void* const*>(xyzi), n, batch, 0, 0, 0, 0, -1, outs, nullptr, nullptr);
+  return process_batch_impl(ctx, reinterpret_cast<const void* const*>(xyzi), n, batch, 0, 0, 0, 0, -1, nullptr, outs, nullptr, nullptr);
 }
 
 int urf_process_batch_xyz(urf_ctx* ctx, const float* const* xyz, const int* n, int batch, urf_result* outs, int8_t* const* label8) {
-  return process_batch_impl(ctx, reinterpret_cast<const void* const*>(xyz), n, batch, 12, 0, 4, 8, -1, outs, label8, nullptr);
+  return process_batch_impl(ctx, reinterpret_cast<const void* const*>(xyz), n, batch, 12, 0, 4, 8, -1, nullptr, outs, label8, nullptr);
 }
 
 // the record entry points reject point_step 0 themselves: the body reads step 0 as float4 input
 int urf_process_cloud2_batch(urf_ctx* ctx, const void* const* data, const int* n_points, int batch, int point_step, int off_x, int off_y,
                              int off_z, int off_intensity, urf_result* outs, int8_t* const* label8) {
   if (point_step == 0) return URF_ERR_INVALID;
-  return process_batch_impl(ctx, data, n_points, batch, point_step, off_x, off_y, off_z, off_intensity, outs, label8, nullptr);
+  return process_batch_impl(ctx, data, n_points, batch, point_step, off_x, off_y, off_z, off_intensity, nullptr, outs, label8, nullptr);
 }
 
 int urf_process_cloud2(urf_ctx* ctx, const void* data, int n, int point_step, int off_x, int off_y, int off_z, urf_result* out) {
   if (point_step == 0) return URF_ERR_INVALID;
-  return process_batch_impl(ctx, &data, &n, 1, point_step, off_x, off_y, off_z, -1, out, nullptr, nullptr);
+  return process_batch_impl(ctx, &data, &n, 1, point_step, off_x, off_y, off_z, -1, nullptr, out, nullptr, nullptr);
 }
 
 int urf_process_cloud2_packed(urf_ctx* ctx, const void* data, int n, int point_step, int off_x, int off_y, int off_z,
                               int off_intensity, urf_result* out, urf_clouds* clouds) {
   if (!clouds || point_step == 0) return URF_ERR_INVALID;
-  return process_batch_impl(ctx, &data, &n, 1, point_step, off_x, off_y, off_z, off_intensity, out, nullptr, clouds);
+  return process_batch_impl(ctx, &data, &n, 1, point_step, off_x, off_y, off_z, off_intensity, nullptr, out, nullptr, clouds);
 }
 
 int urf_process(urf_ctx* ctx, const float* xyzi, int n, urf_result* out) {

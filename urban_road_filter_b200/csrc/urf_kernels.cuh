@@ -2141,21 +2141,25 @@ __global__ void __launch_bounds__(kLomutoThreads) k_lomuto_rings(DevBuffers buf,
 }
 
 // k_unpack_cloud2_batch: PointCloud2 record -> (x, y, z, intensity) float4 (SURVEY.md §8 f1) for a batch: scan
-// b = blockIdx.y, its records at raw + b * S * point_step, its points at dst + b * S. Byte-wise loads when a field is not
-// 4-byte aligned (Velodyne's 22-byte records). off_i < 0: no intensity field, 0 is stored.
+// b = blockIdx.y, its records at raw + b * S * step_max, its points at dst + b * S. Scan b's format is fmt[b] (a batch of
+// mixed formats, urf_process_cloud2_batch_mixed: the per-scan table in device memory), or with fmt == NULL `one` for every
+// scan (step_max == one.point_step). Byte-wise loads when a field is not 4-byte aligned (Velodyne's 22-byte records).
+// off_intensity < 0: no intensity field, 0 is stored.
 __device__ __forceinline__ float load_f32_unaligned(const unsigned char* p) {
   if ((reinterpret_cast<size_t>(p) & 3) == 0) return *reinterpret_cast<const float*>(p);
   const unsigned v = (unsigned)p[0] | ((unsigned)p[1] << 8) | ((unsigned)p[2] << 16) | ((unsigned)p[3] << 24);
   return __uint_as_float(v);
 }
 __global__ void __launch_bounds__(256) k_unpack_cloud2_batch(const unsigned char* __restrict__ raw, float4* __restrict__ dst,
-                                                              const int* __restrict__ n, int S, int point_step, int off_x, int off_y,
-                                                              int off_z, int off_i) {
+                                                              const int* __restrict__ n, int S, int step_max, urf_cloud2_format one,
+                                                              const urf_cloud2_format* __restrict__ fmt) {
   const int b = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n[b]) return;
-  const unsigned char* rec = raw + ((size_t)b * point_slice(S) + i) * point_step;
-  dst[(size_t)b * point_slice(S) + i] = make_float4(load_f32_unaligned(rec + off_x), load_f32_unaligned(rec + off_y), load_f32_unaligned(rec + off_z),
-                                       off_i >= 0 ? load_f32_unaligned(rec + off_i) : 0.f);
+  const urf_cloud2_format f = fmt ? fmt[b] : one;
+  const unsigned char* rec = raw + (size_t)b * point_slice(S) * step_max + (size_t)i * f.point_step;
+  dst[(size_t)b * point_slice(S) + i] = make_float4(load_f32_unaligned(rec + f.off_x), load_f32_unaligned(rec + f.off_y),
+                                                    load_f32_unaligned(rec + f.off_z),
+                                                    f.off_intensity >= 0 ? load_f32_unaligned(rec + f.off_intensity) : 0.f);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------

@@ -4,7 +4,8 @@
 // The reference is a single subscriber with queue depth 1 (`nh->subscribe(params::topicName, 1, &Detector::filtered, this)`,
 // lidar_segmentation.cpp:53); the demo graph feeds four LiDAR topics (config/demo1.rviz:91,121,151,181). urf_mq keeps one
 // submit/next interface in front of N devices: every device owns a context and a streaming queue (urf_queue: pinned
-// staging slots for float4 scans or, in a record mq, for the PointCloud2 records of one sensor format + one worker thread
+// staging slots for float4 scans or, in a record mq, for the PointCloud2 records of one sensor format (of the formats of a
+// table, each scan naming its own, in a formats mq) + one worker thread
 // that takes whatever is pending as one batch and keeps two batches in flight); a scan goes to the device with the fewest
 // scans in flight (ties: round-robin), and results come back in the order the submissions completed.
 // Scans are independent units, so there is nothing to exchange between devices (no collective on this path).
@@ -48,8 +49,6 @@ struct urf_mq {
   int submitting = 0;                // submit calls between device choice and order append
   bool closed = false;
   bool label8 = false;               // int8 label slots on every device (urf_mq_create_label8)
-  int step = 0;                      // 0: float4 scans (urf_mq_submit*); > 0: PointCloud2 records of `step` bytes, one format
-                                     // on every device queue (urf_mq_create_cloud2, urf_mq_submit_cloud2*)
   int32_t gen = 0;                   // last parameter generation; changed only with every device's submit_mu held
   // Scratch of take_front_run. The header allows ONE consumer thread, so it needs no lock.
   std::vector<int> ds;               // devices of the first scans in the global order (a snapshot of `order`'s front)
@@ -71,10 +70,10 @@ int pick_device(urf_mq* m) {         // fewest scans in flight; ties go round-ro
   return best;
 }
 
-// records: the scan is PointCloud2 records (urf_mq_submit_cloud2*), which only a record mq takes, as only a float4 mq takes
-// float4 scans.
-int submit_common(urf_mq* m, const void* data, int n, uint64_t tag, int timeout_ms, bool records, bool by_reference) {
-  if (!m || records != (m->step > 0)) return URF_ERR_INVALID;
+// kind: what the submit call hands in (float4 points, records, or records of table format fmt); every device queue has the
+// mq's kind and format table, so the first one answers whether the mq takes it, before a device is chosen.
+int submit_common(urf_mq* m, urf_internal::ScanKind kind, int fmt, const void* data, int n, uint64_t tag, int timeout_ms, bool by_reference) {
+  if (!m || urf_internal::queue_check_kind(m->dev[0].q, kind, fmt) != URF_OK) return URF_ERR_INVALID;
   int d;
   {
     std::lock_guard<std::mutex> lk(m->mu);
@@ -86,7 +85,7 @@ int submit_common(urf_mq* m, const void* data, int n, uint64_t tag, int timeout_
   // outside the mq lock: the copy into the device's pinned slot (or the wait for a free slot) runs in parallel for
   // producers that were dealt different devices
   std::lock_guard<std::mutex> dev_lk(m->dev[d].submit_mu);
-  const int rc = urf_internal::queue_submit(m->dev[d].q, data, n, tag, timeout_ms, by_reference);
+  const int rc = urf_internal::queue_submit(m->dev[d].q, kind, fmt, data, n, tag, timeout_ms, by_reference);
   {
     std::lock_guard<std::mutex> lk(m->mu);
     m->submitting--;
@@ -98,20 +97,20 @@ int submit_common(urf_mq* m, const void* data, int n, uint64_t tag, int timeout_
 }
 
 // fn == NULL: a context (with `params`, if given) and a pinned queue on each of `devices`; otherwise stand-in devices
-// around fn, which gets users[j] for device j. Every device queue gets `policy`, and with step > 0 the record format (step,
-// ox, oy, oz, oi). The first device that cannot be made ends the attempt.
+// around fn, which gets users[j] for device j. Every device queue gets `policy` and the scan kind: float4, the one record
+// format formats[0] (Records), or the format table (Formats). The first device that cannot be made ends the attempt.
 int create(urf_mq** out, const int* devices, urf_queue_process_fn fn, void* const* users, int n_devices, int max_points,
-           int slots_per_device, int max_batch, const urf_params* params, int policy, int step = 0, int ox = 0, int oy = 4,
-           int oz = 8, int oi = -1) {
+           int slots_per_device, int max_batch, const urf_params* params, int policy,
+           urf_internal::ScanKind kind = urf_internal::ScanKind::Float4, const urf_cloud2_format* formats = nullptr, int n_formats = 0) {
+  using urf_internal::ScanKind;
   // BLOCK with the slot options only: the mq has no drop policy
   if (!out || (!devices && !fn) || n_devices < 1 || max_points < 1 || slots_per_device < 1 || max_batch < 1 ||
       (policy & ~(URF_QUEUE_LABEL8 | URF_QUEUE_ORDER)) != URF_QUEUE_BLOCK ||
-      (step != 0 && urf_internal::check_cloud2_format(step, ox, oy, oz, oi) != URF_OK))
+      (kind != ScanKind::Float4 && urf::check_format_table(formats, n_formats) != URF_OK))
     return URF_ERR_INVALID;
   *out = nullptr;
   urf_mq* m = new urf_mq;
   m->label8 = (policy & URF_QUEUE_LABEL8) != 0;
-  m->step = step;
   for (int j = 0; j < n_devices; j++) m->dev.emplace_back();
   m->want.resize(n_devices); m->done.resize(n_devices); m->used.resize(n_devices); m->dst.resize(n_devices);
   for (int j = 0; j < n_devices; j++) {
@@ -119,12 +118,21 @@ int create(urf_mq** out, const int* devices, urf_queue_process_fn fn, void* cons
     d.device = fn ? j : devices[j];
     int rc = URF_OK;
     void* const user = users ? users[j] : nullptr;
-    if (fn && step) rc = urf_queue_create_cloud2_with(&d.q, fn, user, max_points, slots_per_device, max_batch, policy, step, ox, oy, oz, oi);
+    const urf_cloud2_format* f = formats;
+    if (fn && kind == ScanKind::Records)
+      rc = urf_queue_create_cloud2_with(&d.q, fn, user, max_points, slots_per_device, max_batch, policy, f->point_step, f->off_x,
+                                        f->off_y, f->off_z, f->off_intensity);
+    else if (fn && kind == ScanKind::Formats)
+      rc = urf_queue_create_formats_with(&d.q, fn, user, max_points, slots_per_device, max_batch, policy, formats, n_formats);
     else if (fn) rc = urf_queue_create_with(&d.q, fn, user, max_points, slots_per_device, max_batch, policy);
     else {
       rc = urf_create(&d.ctx, d.device, max_points, max_batch);
       if (rc == URF_OK && params) rc = urf_set_params(d.ctx, params);
-      if (rc == URF_OK && step) rc = urf_queue_create_cloud2(&d.q, d.ctx, max_points, slots_per_device, max_batch, policy, step, ox, oy, oz, oi);
+      if (rc == URF_OK && kind == ScanKind::Records)
+        rc = urf_queue_create_cloud2(&d.q, d.ctx, max_points, slots_per_device, max_batch, policy, f->point_step, f->off_x, f->off_y,
+                                     f->off_z, f->off_intensity);
+      else if (rc == URF_OK && kind == ScanKind::Formats)
+        rc = urf_queue_create_formats(&d.q, d.ctx, max_points, slots_per_device, max_batch, policy, formats, n_formats);
       else if (rc == URF_OK) rc = urf_queue_create(&d.q, d.ctx, max_points, slots_per_device, max_batch, policy);
     }
     if (rc != URF_OK) { urf_mq_destroy(m); return rc; }
@@ -226,15 +234,29 @@ int urf_mq_create_with_policy(urf_mq** out, urf_queue_process_fn fn, void* const
 
 int urf_mq_create_cloud2(urf_mq** out, const int* devices, int n_devices, int max_points, int slots_per_device, int max_batch,
                          const urf_params* params, int policy, int point_step, int off_x, int off_y, int off_z, int off_intensity) {
-  return create(out, devices, nullptr, nullptr, n_devices, max_points, slots_per_device, max_batch, params, policy, point_step, off_x,
-                off_y, off_z, off_intensity);
+  const urf_cloud2_format f{point_step, off_x, off_y, off_z, off_intensity};
+  return create(out, devices, nullptr, nullptr, n_devices, max_points, slots_per_device, max_batch, params, policy,
+                urf_internal::ScanKind::Records, &f, 1);
 }
 
 int urf_mq_create_cloud2_with(urf_mq** out, urf_queue_process_fn fn, void* const* users, int n_devices, int max_points,
                               int slots_per_device, int max_batch, int policy, int point_step, int off_x, int off_y, int off_z,
                               int off_intensity) {
-  return create(out, nullptr, fn, users, n_devices, max_points, slots_per_device, max_batch, nullptr, policy, point_step, off_x, off_y,
-                off_z, off_intensity);
+  const urf_cloud2_format f{point_step, off_x, off_y, off_z, off_intensity};
+  return create(out, nullptr, fn, users, n_devices, max_points, slots_per_device, max_batch, nullptr, policy,
+                urf_internal::ScanKind::Records, &f, 1);
+}
+
+int urf_mq_create_formats(urf_mq** out, const int* devices, int n_devices, int max_points, int slots_per_device, int max_batch,
+                          const urf_params* params, int policy, const urf_cloud2_format* formats, int n_formats) {
+  return create(out, devices, nullptr, nullptr, n_devices, max_points, slots_per_device, max_batch, params, policy,
+                urf_internal::ScanKind::Formats, formats, n_formats);
+}
+
+int urf_mq_create_formats_with(urf_mq** out, urf_queue_process_fn fn, void* const* users, int n_devices, int max_points,
+                               int slots_per_device, int max_batch, int policy, const urf_cloud2_format* formats, int n_formats) {
+  return create(out, nullptr, fn, users, n_devices, max_points, slots_per_device, max_batch, nullptr, policy,
+                urf_internal::ScanKind::Formats, formats, n_formats);
 }
 
 int urf_mq_set_params(urf_mq* m, const urf_params* p) {
@@ -266,13 +288,24 @@ int urf_mq_set_params_hook(urf_mq* m, urf_queue_params_fn fn) {
   return URF_OK;
 }
 
-int urf_mq_submit(urf_mq* m, const float* xyzi, int n, uint64_t tag, int timeout_ms) { return submit_common(m, xyzi, n, tag, timeout_ms, false, false); }
-int urf_mq_submit_ref(urf_mq* m, const float* xyzi, int n, uint64_t tag, int timeout_ms) { return submit_common(m, xyzi, n, tag, timeout_ms, false, true); }
+using urf_internal::ScanKind;
+int urf_mq_submit(urf_mq* m, const float* xyzi, int n, uint64_t tag, int timeout_ms) {
+  return submit_common(m, ScanKind::Float4, 0, xyzi, n, tag, timeout_ms, false);
+}
+int urf_mq_submit_ref(urf_mq* m, const float* xyzi, int n, uint64_t tag, int timeout_ms) {
+  return submit_common(m, ScanKind::Float4, 0, xyzi, n, tag, timeout_ms, true);
+}
 int urf_mq_submit_cloud2(urf_mq* m, const void* data, int n_points, uint64_t tag, int timeout_ms) {
-  return submit_common(m, data, n_points, tag, timeout_ms, true, false);
+  return submit_common(m, ScanKind::Records, 0, data, n_points, tag, timeout_ms, false);
 }
 int urf_mq_submit_cloud2_ref(urf_mq* m, const void* data, int n_points, uint64_t tag, int timeout_ms) {
-  return submit_common(m, data, n_points, tag, timeout_ms, true, true);
+  return submit_common(m, ScanKind::Records, 0, data, n_points, tag, timeout_ms, true);
+}
+int urf_mq_submit_format(urf_mq* m, int fmt, const void* data, int n_points, uint64_t tag, int timeout_ms) {
+  return submit_common(m, ScanKind::Formats, fmt, data, n_points, tag, timeout_ms, false);
+}
+int urf_mq_submit_format_ref(urf_mq* m, int fmt, const void* data, int n_points, uint64_t tag, int timeout_ms) {
+  return submit_common(m, ScanKind::Formats, fmt, data, n_points, tag, timeout_ms, true);
 }
 
 int urf_mq_next_batch(urf_mq* m, int max_results, uint64_t* tags, int32_t* rcs, urf_result* outs, const void** label_views,

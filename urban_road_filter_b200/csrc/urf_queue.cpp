@@ -17,6 +17,10 @@
 // points the batch call's outs at them, the batch body fills them as it does for any caller, and delivery lends them with
 // the labels.
 //
+// Scan kinds: float4 points, records of one format (urf_queue_create_cloud2), or records of the formats of a table, each
+// submit naming its scan's format (urf_queue_create_formats). A slot holds max_points records of the largest format, remembers
+// its scan's format, and a formats queue's run goes to urf_enqueue_cloud2_batch_mixed with each scan's format.
+//
 // The worker is one loop with a depth. On a real context it keeps two batches in flight (urf_enqueue_batch /
 // urf_finish_batch): it enqueues what is pending, enqueues the next pending run too if there is one, and only then waits
 // for the oldest batch, so the copies of one batch overlap the kernels of the other and the device does not wait for the
@@ -40,6 +44,8 @@
 #include "urf_params.hpp"
 #include "urf_queue_internal.hpp"
 
+using urf_internal::ScanKind;
+
 namespace {
 enum SlotState { FREE = 0, FILLING, PENDING, RUNNING, DONE, VIEWED };   // VIEWED: delivered, its labels lent to the consumer
 struct Slot {
@@ -47,6 +53,7 @@ struct Slot {
   uint64_t seq = 0, tag = 0;
   int32_t gen = 0;           // parameter generation in force when the scan became PENDING
   int n = 0, rc = URF_OK;
+  int fmt = 0;               // the scan's index into the queue's formats (0 but in a formats queue)
   float* in = nullptr;       // max_points * bytes_per_point bytes (pinned for the real queue)
   const float* ext = nullptr;   // urf_queue_submit_ref / _cloud2_ref: the caller's buffer is used in place (no copy)
   int32_t* label = nullptr;  // max_points; NULL in a real URF_QUEUE_LABEL8 queue
@@ -68,11 +75,14 @@ struct urf_queue {
   int depth = 2;               // batches the worker keeps in flight: 2, or 1 around a synchronous stand-in
   bool label8 = false;         // URF_QUEUE_LABEL8: int8 label slots
   bool order = false;          // URF_QUEUE_ORDER: every slot also holds the scan's emission order and ring offsets
-  // record format of the scans: step == 0: (x, y, z, intensity) float4 points; step > 0: raw PointCloud2 records of `step`
-  // bytes (urf_queue_create_cloud2), handed to urf_process_cloud2_batch and unpacked on the device
-  int step = 0, ox = 0, oy = 4, oz = 8, oi = -1;
-  size_t bytes_per_point = 16;
+  // what the scans are: (x, y, z, intensity) float4 points, raw PointCloud2 records of one format (urf_queue_create_cloud2),
+  // or records of the formats of a table, each submit naming its own (urf_queue_create_formats); records are handed to the
+  // batch body as they are and unpacked on the device
+  ScanKind kind = ScanKind::Float4;
+  std::vector<urf_cloud2_format> formats;   // float4: {16, 0, 4, 8, 12}; records: the one format; formats: the table
+  size_t bytes_per_point = 16;              // the largest point_step of `formats`
   urf_cloud2_user rec{};       // record stand-in (urf_queue_create_cloud2_with): `user` points here, rec.user is the creator's
+  urf_formats_user fu{};       // formats stand-in (urf_queue_create_formats_with): the same, with the table and the run's indices
   std::vector<Slot> slots;
   std::mutex mu;
   std::condition_variable cv_free, cv_pending, cv_done;
@@ -102,6 +112,8 @@ struct Run {
   std::vector<int> idx;
   std::vector<const float*> ptrs;
   std::vector<int> ns;
+  std::vector<int32_t> fidx;             // per scan: its index into the queue's formats
+  std::vector<urf_cloud2_format> fmts;   // per scan: its format (a formats queue's mixed batch)
   std::vector<urf_result> outs;
   std::vector<int8_t*> l8;
   int rc = URF_OK;             // synchronous stand-in: what the batch function returned, reported by finish_run
@@ -153,10 +165,11 @@ int take_run(urf_queue* q, Run& r, int32_t applied, bool wait, bool* closed) {
     if ((int)r.idx.size() > q->st.largest_batch) q->st.largest_batch = (int)r.idx.size();
   }
   const int B = (int)r.idx.size();
-  r.ptrs.resize(B); r.ns.resize(B); r.l8.resize(B); r.outs.assign(B, urf_result{});
+  r.ptrs.resize(B); r.ns.resize(B); r.fidx.resize(B); r.fmts.resize(B); r.l8.resize(B); r.outs.assign(B, urf_result{});
   for (int j = 0; j < B; j++) {                           // RUNNING slots belong to the worker: read outside the lock
     const Slot& s = q->slots[r.idx[j]];
     r.ptrs[j] = s.ext ? s.ext : s.in; r.ns[j] = s.n;
+    r.fidx[j] = s.fmt; r.fmts[j] = q->formats[s.fmt];
     r.outs[j].label = s.label;                            // NULL in a real int8 queue: no int32 label copy is issued
     r.outs[j].order = s.order; r.outs[j].ring_start = s.ring_start;   // NULL without URF_QUEUE_ORDER: no ring sort, no copy
     r.l8[j] = s.label8;
@@ -202,17 +215,20 @@ int apply_run(urf_queue* q, const Run& r, int32_t* applied) {
 int enqueue_run(urf_queue* q, Run& r) {
   const int B = (int)r.idx.size();
   if (q->enq) {
+    q->fu.fmt = r.fidx.data();                            // a formats stand-in's indices, for the call (it is synchronous)
     const int rc = q->enq(q->user, r.ptrs.data(), r.ns.data(), B, r.outs.data());
+    q->fu.fmt = nullptr;
     if (q->fin) return rc;
     r.rc = rc;
     return URF_OK;
   }
-  if (q->step == 0 && !q->label8) return urf_enqueue_batch(q->ctx, r.ptrs.data(), r.ns.data(), B, r.outs.data(), nullptr);
+  if (q->kind == ScanKind::Float4 && !q->label8) return urf_enqueue_batch(q->ctx, r.ptrs.data(), r.ns.data(), B, r.outs.data(), nullptr);
+  const auto data = reinterpret_cast<const void* const*>(r.ptrs.data());
+  int8_t* const* l8 = q->label8 ? r.l8.data() : nullptr;
+  if (q->kind == ScanKind::Formats) return urf_enqueue_cloud2_batch_mixed(q->ctx, data, r.ns.data(), r.fmts.data(), B, r.outs.data(), l8);
   // float4 scans with int8 labels are 16-byte records (x, y, z, intensity at 0, 4, 8, 12) to the record body
-  const bool f4 = q->step == 0;
-  return urf_enqueue_cloud2_batch(q->ctx, reinterpret_cast<const void* const*>(r.ptrs.data()), r.ns.data(), B, f4 ? 16 : q->step,
-                                  f4 ? 0 : q->ox, f4 ? 4 : q->oy, f4 ? 8 : q->oz, f4 ? 12 : q->oi, r.outs.data(),
-                                  q->label8 ? r.l8.data() : nullptr);
+  const urf_cloud2_format& f = q->formats[0];
+  return urf_enqueue_cloud2_batch(q->ctx, data, r.ns.data(), B, f.point_step, f.off_x, f.off_y, f.off_z, f.off_intensity, r.outs.data(), l8);
 }
 
 // Waits for the oldest run in flight, r.
@@ -253,8 +269,10 @@ void free_slot(const urf_queue* q, Slot& s) {
 }
 
 // Either ctx (real queue, pinned slots) or enq (stand-in; synchronous, and the worker's depth 1, without fin) is set.
+// kind Records / Formats: the record formats (one, or the table), which the caller has checked.
 int create_common(urf_queue** out, urf_ctx* ctx, urf_queue_process_fn enq, urf_queue_finish_fn fin, void* user,
-                  int max_points, int slots, int max_batch, int policy, int step = 0, int ox = 0, int oy = 4, int oz = 8, int oi = -1) {
+                  int max_points, int slots, int max_batch, int policy, ScanKind kind = ScanKind::Float4,
+                  const urf_cloud2_format* formats = nullptr, int n_formats = 0) {
   const bool label8 = (policy & URF_QUEUE_LABEL8) != 0, order = (policy & URF_QUEUE_ORDER) != 0;
   policy &= ~(URF_QUEUE_LABEL8 | URF_QUEUE_ORDER);
   if (!out || (!ctx && !enq) || max_points < 1 || slots < 1 || max_batch < 1 ||
@@ -265,9 +283,17 @@ int create_common(urf_queue** out, urf_ctx* ctx, urf_queue_process_fn enq, urf_q
   q->ctx = ctx; q->enq = enq; q->fin = fin; q->user = user;
   q->pinned = pinned; q->max_points = max_points; q->max_batch = max_batch; q->policy = policy;
   q->label8 = label8; q->order = order; q->depth = ctx || fin ? 2 : 1;
-  q->step = step; q->ox = ox; q->oy = oy; q->oz = oz; q->oi = oi;
-  q->bytes_per_point = step > 0 ? (size_t)step : 16;
-  if (!ctx && step > 0) { q->rec = urf_cloud2_user{user, step, ox, oy, oz, oi}; q->user = &q->rec; }
+  q->kind = kind;
+  if (kind == ScanKind::Float4) q->formats.assign(1, urf_cloud2_format{16, 0, 4, 8, 12});
+  else q->formats.assign(formats, formats + n_formats);
+  q->bytes_per_point = 0;
+  for (const urf_cloud2_format& f : q->formats) q->bytes_per_point = std::max(q->bytes_per_point, (size_t)f.point_step);
+  if (!ctx && kind == ScanKind::Records) {
+    const urf_cloud2_format& f = q->formats[0];
+    q->rec = urf_cloud2_user{user, f.point_step, f.off_x, f.off_y, f.off_z, f.off_intensity};
+    q->user = &q->rec;
+  }
+  if (!ctx && kind == ScanKind::Formats) { q->fu = urf_formats_user{user, q->formats.data(), (int32_t)q->formats.size(), nullptr}; q->user = &q->fu; }
   q->slots.resize(slots); q->lent.reserve(slots); q->live.reserve(slots);
   // int8 slots hold max_points bytes of labels; a stand-in batch function still writes int32 labels, which need a buffer
   const bool want32 = !label8 || !ctx, want8 = label8;
@@ -303,16 +329,28 @@ int urf_queue_create(urf_queue** out, urf_ctx* ctx, int max_points, int slots, i
 
 int urf_queue_create_cloud2(urf_queue** out, urf_ctx* ctx, int max_points, int slots, int max_batch, int policy, int point_step, int off_x,
                             int off_y, int off_z, int off_intensity) {
-  if (!ctx || urf_internal::check_cloud2_format(point_step, off_x, off_y, off_z, off_intensity) != URF_OK) return URF_ERR_INVALID;
-  return create_common(out, ctx, nullptr, nullptr, nullptr, max_points, slots, max_batch, policy, point_step, off_x, off_y, off_z,
-                       off_intensity);
+  const urf_cloud2_format f{point_step, off_x, off_y, off_z, off_intensity};
+  if (!ctx || urf::check_cloud2_format(f) != URF_OK) return URF_ERR_INVALID;
+  return create_common(out, ctx, nullptr, nullptr, nullptr, max_points, slots, max_batch, policy, ScanKind::Records, &f, 1);
 }
 
 int urf_queue_create_cloud2_with(urf_queue** out, urf_queue_process_fn fn, void* user, int max_points, int slots, int max_batch,
                                  int policy, int point_step, int off_x, int off_y, int off_z, int off_intensity) {
-  if (!fn || urf_internal::check_cloud2_format(point_step, off_x, off_y, off_z, off_intensity) != URF_OK) return URF_ERR_INVALID;
-  return create_common(out, nullptr, fn, nullptr, user, max_points, slots, max_batch, policy, point_step, off_x, off_y, off_z,
-                       off_intensity);
+  const urf_cloud2_format f{point_step, off_x, off_y, off_z, off_intensity};
+  if (!fn || urf::check_cloud2_format(f) != URF_OK) return URF_ERR_INVALID;
+  return create_common(out, nullptr, fn, nullptr, user, max_points, slots, max_batch, policy, ScanKind::Records, &f, 1);
+}
+
+int urf_queue_create_formats(urf_queue** out, urf_ctx* ctx, int max_points, int slots, int max_batch, int policy,
+                             const urf_cloud2_format* formats, int n_formats) {
+  if (!ctx || urf::check_format_table(formats, n_formats) != URF_OK) return URF_ERR_INVALID;
+  return create_common(out, ctx, nullptr, nullptr, nullptr, max_points, slots, max_batch, policy, ScanKind::Formats, formats, n_formats);
+}
+
+int urf_queue_create_formats_with(urf_queue** out, urf_queue_process_fn fn, void* user, int max_points, int slots, int max_batch,
+                                  int policy, const urf_cloud2_format* formats, int n_formats) {
+  if (!fn || urf::check_format_table(formats, n_formats) != URF_OK) return URF_ERR_INVALID;
+  return create_common(out, nullptr, fn, nullptr, user, max_points, slots, max_batch, policy, ScanKind::Formats, formats, n_formats);
 }
 
 int urf_queue_create_with(urf_queue** out, urf_queue_process_fn fn, void* user, int max_points, int slots, int max_batch, int policy) {
@@ -328,23 +366,27 @@ int urf_queue_create_with_async(urf_queue** out, urf_queue_process_fn enqueue, u
 
 
 int urf_queue_submit(urf_queue* q, const float* xyzi, int n, uint64_t tag, int timeout_ms) {
-  if (q && q->step != 0) return URF_ERR_INVALID;           // a record queue takes urf_queue_submit_cloud2
-  return urf_internal::queue_submit(q, xyzi, n, tag, timeout_ms, false);
+  return urf_internal::queue_submit(q, ScanKind::Float4, 0, xyzi, n, tag, timeout_ms, false);
 }
 
 int urf_queue_submit_ref(urf_queue* q, const float* xyzi, int n, uint64_t tag, int timeout_ms) {
-  if (q && q->step != 0) return URF_ERR_INVALID;
-  return urf_internal::queue_submit(q, xyzi, n, tag, timeout_ms, true);
+  return urf_internal::queue_submit(q, ScanKind::Float4, 0, xyzi, n, tag, timeout_ms, true);
 }
 
 int urf_queue_submit_cloud2(urf_queue* q, const void* data, int n_points, uint64_t tag, int timeout_ms) {
-  if (q && q->step == 0) return URF_ERR_INVALID;           // a float4 queue takes urf_queue_submit
-  return urf_internal::queue_submit(q, data, n_points, tag, timeout_ms, false);
+  return urf_internal::queue_submit(q, ScanKind::Records, 0, data, n_points, tag, timeout_ms, false);
 }
 
 int urf_queue_submit_cloud2_ref(urf_queue* q, const void* data, int n_points, uint64_t tag, int timeout_ms) {
-  if (q && q->step == 0) return URF_ERR_INVALID;
-  return urf_internal::queue_submit(q, data, n_points, tag, timeout_ms, true);
+  return urf_internal::queue_submit(q, ScanKind::Records, 0, data, n_points, tag, timeout_ms, true);
+}
+
+int urf_queue_submit_format(urf_queue* q, int fmt, const void* data, int n_points, uint64_t tag, int timeout_ms) {
+  return urf_internal::queue_submit(q, ScanKind::Formats, fmt, data, n_points, tag, timeout_ms, false);
+}
+
+int urf_queue_submit_format_ref(urf_queue* q, int fmt, const void* data, int n_points, uint64_t tag, int timeout_ms) {
+  return urf_internal::queue_submit(q, ScanKind::Formats, fmt, data, n_points, tag, timeout_ms, true);
 }
 
 int urf_queue_update_params(urf_queue* q, const urf_params* p) {
@@ -504,10 +546,8 @@ void urf_queue_destroy(urf_queue* q) {
 
 namespace urf_internal {
 
-int check_cloud2_format(int point_step, int off_x, int off_y, int off_z, int off_intensity) {
-  if (point_step < 12 || point_step > URF_MAX_POINT_STEP) return URF_ERR_INVALID;
-  for (int o : {off_x, off_y, off_z}) if (o < 0 || o + 4 > point_step) return URF_ERR_INVALID;
-  if (off_intensity >= 0 && off_intensity + 4 > point_step) return URF_ERR_INVALID;
+int queue_check_kind(const urf_queue* q, ScanKind kind, int fmt) {
+  if (!q || kind != q->kind || fmt < 0 || fmt >= (int)q->formats.size()) return URF_ERR_INVALID;
   return URF_OK;
 }
 
@@ -527,8 +567,8 @@ int queue_lend_run(urf_queue* q, int count, const int* dst, uint64_t* tags, int3
   return (int)q->lent.size();
 }
 
-int queue_submit(urf_queue* q, const void* data, int n, uint64_t tag, int timeout_ms, bool by_reference) {
-  if (!q || n < 0 || (n > 0 && !data)) return URF_ERR_INVALID;
+int queue_submit(urf_queue* q, ScanKind kind, int fmt, const void* data, int n, uint64_t tag, int timeout_ms, bool by_reference) {
+  if (queue_check_kind(q, kind, fmt) != URF_OK || n < 0 || (n > 0 && !data)) return URF_ERR_INVALID;
   if (n > q->max_points) return URF_ERR_CAPACITY;
   int slot = -1;
   {
@@ -553,14 +593,14 @@ int queue_submit(urf_queue* q, const void* data, int n, uint64_t tag, int timeou
   Slot& s = q->slots[slot];
   bool closed_late = false;
   if (by_reference) s.ext = static_cast<const float*>(data);
-  else { s.ext = nullptr; if (n > 0) std::memcpy(s.in, data, q->bytes_per_point * (size_t)n); }
+  else { s.ext = nullptr; if (n > 0) std::memcpy(s.in, data, (size_t)q->formats[fmt].point_step * (size_t)n); }
   {
     std::lock_guard<std::mutex> lk(q->mu);
     if (q->closed) {                                      // closed while copying: the worker may already be gone
       s.state = FREE;
       closed_late = true;
     } else {
-      s.n = n; s.tag = tag; s.rc = URF_OK;
+      s.n = n; s.fmt = fmt; s.tag = tag; s.rc = URF_OK;
       s.seq = q->next_seq++; s.gen = q->gen;
       s.state = PENDING;
       q->st.submitted++;

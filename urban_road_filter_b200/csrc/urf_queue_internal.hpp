@@ -1,5 +1,5 @@
 // urf_queue_internal.hpp — what urf_queue.cpp and urf_mq.cpp share (host code, C++ linkage, not part of include/urf.h):
-// the timed wait, the record format checks and the submit behind the creators and submits of both, the two halves of a
+// the timed wait, the scan kinds and the submit behind the submits of both, the two halves of a
 // delivery call, which urf_mq needs separately, the copy of a lent scan's labels and order, and the idle rule of the mq's
 // settings. urf_mq first asks every device queue how far its run of finished scans reaches, cuts
 // the global order at the first scan that is not done, and only then has each queue lend exactly its share.
@@ -21,13 +21,17 @@ bool wait_for(std::condition_variable& cv, std::unique_lock<std::mutex>& lk, int
   return cv.wait_for(lk, std::chrono::milliseconds(timeout_ms), pred);
 }
 
-// The record format checks of every record queue and record mq creator: URF_OK when point_step is in
-// [12, URF_MAX_POINT_STEP] and the FLOAT32 x / y / z (and intensity, when off_intensity >= 0) lie inside a record.
-int check_cloud2_format(int point_step, int off_x, int off_y, int off_z, int off_intensity);
+// What a queue's scans are, and which submits it takes: float4 points (urf_*_submit*), PointCloud2 records of one format
+// (urf_*_submit_cloud2*) or of the formats of a table (urf_*_submit_format*).
+enum class ScanKind { Float4, Records, Formats };
 
-// The submit of urf_queue_submit* without the check of the scan kind (float4 points or records), which the callers make:
-// data holds n points of the queue's format; by_reference as urf_queue_submit_ref, otherwise copied into the slot.
-int queue_submit(urf_queue* q, const void* data, int n, uint64_t tag, int timeout_ms, bool by_reference);
+// URF_OK when q takes scans of `kind` and fmt is the index of one of its formats (0 for the float4 and record kinds);
+// URF_ERR_INVALID otherwise.
+int queue_check_kind(const urf_queue* q, ScanKind kind, int fmt);
+
+// The submit behind urf_queue_submit* and urf_mq_submit*: queue_check_kind, then data holds n records of the queue's
+// format `fmt`; by_reference as urf_queue_submit_ref, otherwise copied into the slot.
+int queue_submit(urf_queue* q, ScanKind kind, int fmt, const void* data, int n, uint64_t tag, int timeout_ms, bool by_reference);
 
 // Gives back the slots lent by earlier delivery calls, waits up to timeout_ms (< 0: forever, 0: no wait) until the
 // oldest live scan is done, and returns how many consecutive scans from the oldest on are done (at most max_results).

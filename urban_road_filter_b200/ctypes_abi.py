@@ -118,6 +118,22 @@ class UrfCloud2User(C.Structure):
                 ("off_z", C.c_int32), ("off_intensity", C.c_int32)]
 
 
+URF_MAX_FORMATS = 8
+
+
+class UrfCloud2Format(C.Structure):
+    """urf_cloud2_format: one PointCloud2 record format (point_step and the byte offsets of x, y, z and intensity, -1: none)."""
+    _fields_ = [("point_step", C.c_int32), ("off_x", C.c_int32), ("off_y", C.c_int32), ("off_z", C.c_int32),
+                ("off_intensity", C.c_int32)]
+
+
+class UrfFormatsUser(C.Structure):
+    """urf_formats_user: what a formats stand-in's batch function and parameter hook get as `user` (the creator's user, the
+    format table, and during a batch call each scan's index into it)."""
+    _fields_ = [("user", C.c_void_p), ("formats", C.POINTER(UrfCloud2Format)), ("n_formats", C.c_int32),
+                ("fmt", C.POINTER(C.c_int32))]
+
+
 # cfg/LidarFilters.cfg:10-84 defaults
 DEFAULTS = dict(
     fixed_frame=b"left_os1/os1_lidar", topic_name=b"/left_os1/os1_cloud_node/points",
