@@ -147,3 +147,43 @@ def random_cloud(n: int, seed: int = 0, rings: int = 8, extent: float = 40.0) ->
     pts[:, 3] = rng.uniform(0, 255, n)
     _detie_radius(pts, seed)
     return pts
+
+
+# PointCloud2 layouts of drive_bag's sensors: (point_step, [(field, offset, datatype)]), datatype 7 = FLOAT32
+CLOUD2_LAYOUTS = {
+    "ouster": (48, [("x", 0, 7), ("y", 4, 7), ("z", 8, 7), ("intensity", 16, 7), ("t", 20, 6), ("reflectivity", 24, 4),
+                    ("ring", 26, 4), ("ambient", 28, 4), ("range", 32, 6)]),
+    "velodyne": (32, [("x", 0, 7), ("y", 4, 7), ("z", 8, 7), ("intensity", 16, 7), ("ring", 20, 4), ("time", 24, 7)]),
+}
+
+
+def drive_bag(path: str, sensors, scans_per_sensor: int, seed: int = 0, distinct: int = 4, compression: str = "none") -> int:
+    """Writes a seeded synthetic recorded drive to `path` as a ROS1 bag: sensors = [(topic, shape, layout)] with layout a
+    key of CLOUD2_LAYOUTS; each sensor publishes scans_per_sensor PointCloud2 messages 0.1 s apart (sensors offset by
+    10 ms), cycling through `distinct` make_scan scans of its shape; the bytes outside x / y / z / intensity are seeded
+    noise. Returns the number of messages."""
+    from .rosbag import POINTCLOUD2, BagWriter, Header, PointCloud2, PointField, Time, cloud2_parts
+
+    msgs = []
+    for i, (topic, shape, layout) in enumerate(sensors):
+        step, fields = CLOUD2_LAYOUTS[layout]
+        offs = {name: off for name, off, _ in fields}
+        recs = []
+        for k in range(distinct):
+            pts = make_scan(shape, seed + 97 * i + k)
+            rec = np.random.default_rng(seed + 1000 * i + k).integers(0, 256, (pts.shape[0], step), dtype=np.uint8)
+            for j, name in enumerate(("x", "y", "z", "intensity")):
+                rec[:, offs[name]: offs[name] + 4] = pts[:, j: j + 1].copy().view(np.uint8)
+            recs.append((pts.shape[0], rec.reshape(-1)))
+        pf = [PointField(name, off, dt, 1) for name, off, dt in fields]
+        for k in range(scans_per_sensor):
+            t = 1_000_000_000_000 + k * 100_000_000 + i * 10_000_000
+            stamp = Time(t // 1_000_000_000, t % 1_000_000_000)
+            n, rec = recs[k % distinct]
+            msgs.append((stamp, topic, PointCloud2(Header(k, stamp, topic.strip("/").split("/")[0]), 1, n, pf, False, step,
+                                                   n * step, rec, True)))
+    msgs.sort(key=lambda m: m[0])
+    with BagWriter(path, compression) as w:
+        for stamp, topic, msg in msgs:
+            w.write(topic, POINTCLOUD2, stamp, cloud2_parts(msg))
+    return len(msgs)
