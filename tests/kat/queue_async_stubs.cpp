@@ -4,7 +4,4 @@
 #include "../../include/urf.h"
 
 extern "C" int urf_enqueue_batch(urf_ctx*, const float* const*, const int*, int, urf_result*, int8_t* const*) { return URF_ERR_NO_DEVICE; }
-extern "C" int urf_enqueue_cloud2_batch(urf_ctx*, const void* const*, const int*, int, int, int, int, int, int, urf_result*, int8_t* const*) {
-  return URF_ERR_NO_DEVICE;
-}
 extern "C" int urf_finish_batch(urf_ctx*) { return URF_ERR_INVALID; }

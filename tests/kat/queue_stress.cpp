@@ -15,8 +15,6 @@
 // stand-ins for the CUDA side of liburf_b200.so (never reached: the queue is created with urf_queue_create_with)
 extern "C" void* urf_pinned_alloc(size_t) { return nullptr; }
 extern "C" void urf_pinned_free(void*) {}
-extern "C" int urf_process_batch(urf_ctx*, const float* const*, const int*, int, urf_result*) { return URF_ERR_NO_DEVICE; }
-extern "C" int urf_process_cloud2_batch(urf_ctx*, const void* const*, const int*, int, int, int, int, int, int, urf_result*, int8_t* const*) { return URF_ERR_NO_DEVICE; }
 extern "C" int urf_create(urf_ctx**, int, int, int) { return URF_ERR_NO_DEVICE; }
 extern "C" void urf_destroy(urf_ctx*) {}
 extern "C" int urf_set_params(urf_ctx*, const urf_params*) { return URF_ERR_NO_DEVICE; }

@@ -174,7 +174,13 @@ def test_mq_one_producer_every_delivery(label8):
     got = []
     cons = threading.Thread(target=lambda: got.extend(drain(mq, 48, 5)))
     cons.start()
-    keep = [submit(mq, k, 8 + k % 9, by_reference=k % 3 == 1) for k in range(48)]
+    # while the stand-ins wait at the gate nothing is delivered, so scans 0..8 are dealt round-robin, three to a device, and
+    # wait behind its first batch: each device runs its three in at most two batches, and one holds two of formats 0, 1, 3
+    # (device 0: scans 0, 3, 6)
+    fb.gate.clear()
+    keep = [submit(mq, k, 8 + k % 9, by_reference=k % 3 == 1) for k in range(9)]
+    fb.gate.set()
+    keep += [submit(mq, k, 8 + k % 9, by_reference=k % 3 == 1) for k in range(9, 48)]
     cons.join(30)
     assert not cons.is_alive() and len(keep) == 48
     assert [t for t, _ in got] == list(range(48))

@@ -636,31 +636,27 @@ int urf_process_batch_device(urf_ctx* ctx, const float* d_xyzi, int stride_point
 }
 
 namespace {
-// Shared body of the host-buffer batch entry points. step == 0: data[b] holds n[b] (x, y, z, intensity) float4 records that
-// are copied straight into the input buffer; step > 0: data[b] holds n[b] records of `step` bytes with FLOAT32 x / y / z /
-// intensity at the given byte offsets (oi < 0: none) — the raw bytes cross PCIe and are unpacked on the device.
-// fmt (or NULL): scan b's records have the format fmt[b] instead (step and the offsets are then ignored); a batch whose
-// formats are all equal runs as the one-format call.
+// Shared body of the host-buffer batch entry points. fmt == NULL: data[b] holds n[b] (x, y, z, intensity) float4 records
+// that are copied straight into the input buffer. Otherwise data[b] holds n[b] PointCloud2 records of the format fmt[0]
+// (per_scan: fmt[b]) — the raw bytes cross PCIe and are unpacked on the device; a table whose formats are all equal runs as
+// the one-format call.
 // label8 (or NULL): per scan an int8 HOST buffer for the labels (one byte per point instead of four).
 // clouds (or NULL, batch == 1 only): the four published clouds of the scan, packed on the device.
 // Enqueues the batch into the next free host slot and returns; finish_batch waits for it and fills outs.
-int enqueue_batch(urf_ctx* ctx, const void* const* data, const int* n, int batch, int step, int ox, int oy, int oz, int oi,
-                  const urf_cloud2_format* fmt, urf_result* outs, int8_t* const* label8, urf_clouds* clouds) {
-  if (!ctx || !data || !n || !outs || batch < 1) return URF_ERR_INVALID;
+int enqueue_batch(urf_ctx* ctx, const void* const* data, const int* n, int batch, const urf_cloud2_format* fmt, bool per_scan,
+                  urf_result* outs, int8_t* const* label8, urf_clouds* clouds) {
+  // a single format with point_step 0 is refused ahead of the capacity checks, every other bad format after them
+  if (!ctx || !data || !n || !outs || batch < 1 || (fmt && !per_scan && fmt->point_step == 0)) return URF_ERR_INVALID;
   if (batch > ctx->max_batch || ctx->hs_count == 2) return URF_ERR_CAPACITY;
-  if (fmt) {                                                  // step becomes the batch's largest point_step
-    bool mixed = false;
-    step = 0;
-    for (int b = 0; b < batch; b++) {
-      if (urf::check_cloud2_format(fmt[b]) != URF_OK) return URF_ERR_INVALID;
-      step = std::max(step, (int)fmt[b].point_step);
-      mixed |= std::memcmp(&fmt[b], &fmt[0], sizeof(urf_cloud2_format)) != 0;
-    }
-    ox = fmt[0].off_x; oy = fmt[0].off_y; oz = fmt[0].off_z; oi = fmt[0].off_intensity;
-    if (!mixed) fmt = nullptr;
-  } else if (step != 0 && urf::check_cloud2_format(step, ox, oy, oz, oi) != URF_OK) {
-    return URF_ERR_INVALID;
+  int step = 0;                                               // the batch's largest point_step; 0: float4 points
+  bool mixed = false;
+  for (int b = 0; fmt && b < (per_scan ? batch : 1); b++) {
+    if (urf::check_cloud2_format(fmt[b]) != URF_OK) return URF_ERR_INVALID;
+    step = std::max(step, (int)fmt[b].point_step);
+    mixed |= std::memcmp(&fmt[b], &fmt[0], sizeof(urf_cloud2_format)) != 0;
   }
+  const urf_cloud2_format one = fmt ? fmt[0] : urf_cloud2_format{};
+  if (!mixed) fmt = nullptr;
   CK(cudaSetDevice(ctx->device));
   const int slot = (ctx->hs_head + ctx->hs_count) % 2;
   urf_ctx::HostSlot& h = ctx->hs[slot];                       // free: its last batch was finished, its copies are done
@@ -754,8 +750,8 @@ int enqueue_batch(urf_ctx* ctx, const void* const* data, const int* n, int batch
     CK(cudaStreamWaitEvent(st, ctx->ev_in[c].get(), 0));
     const DevBuffers view = scan_view(bufv, b0, e);
     if (step != 0)
-      k_unpack_cloud2_batch<<<dim3((S + 255) / 256, nb), 256, 0, st>>>(h.rawb.get() + b0 * pts * step, view.in, view.n, S, step,
-                                                                        urf_cloud2_format{step, ox, oy, oz, oi}, fmt ? h.fmt.get() + b0 : nullptr);
+      k_unpack_cloud2_batch<<<dim3((S + 255) / 256, nb), 256, 0, st>>>(h.rawb.get() + b0 * pts * step, view.in, view.n, S, step, one,
+                                                                        fmt ? h.fmt.get() + b0 : nullptr);
     // ev0 / ev1 bracket the kernels of the whole call: before the first chunk's pipeline, after the last one's
     int L = graphed ? ctx->g_launches : 0;
     int rc = c == 0 ? cuda_rc(ctx, cudaEventRecord(h.ev0.get(), st), "cudaEventRecord(ev0)") : URF_OK;
@@ -856,70 +852,67 @@ int alloc_second_slot(urf_ctx* ctx) {
 }
 
 // The synchronous entry points: one enqueue and one finish, refused while asynchronous batches are in flight.
-int process_batch_impl(urf_ctx* ctx, const void* const* data, const int* n, int batch, int step, int ox, int oy, int oz, int oi,
-                       const urf_cloud2_format* fmt, urf_result* outs, int8_t* const* label8, urf_clouds* clouds) {
+int process_batch_impl(urf_ctx* ctx, const void* const* data, const int* n, int batch, const urf_cloud2_format* fmt, bool per_scan,
+                       urf_result* outs, int8_t* const* label8, urf_clouds* clouds) {
   if (ctx && ctx->hs_count) return URF_ERR_INVALID;
-  const int rc = enqueue_batch(ctx, data, n, batch, step, ox, oy, oz, oi, fmt, outs, label8, clouds);
+  const int rc = enqueue_batch(ctx, data, n, batch, fmt, per_scan, outs, label8, clouds);
   return rc != URF_OK ? rc : finish_batch(ctx);
 }
 
-int enqueue_async(urf_ctx* ctx, const void* const* data, const int* n, int batch, int step, int ox, int oy, int oz, int oi,
-                  const urf_cloud2_format* fmt, urf_result* outs, int8_t* const* label8) {
+int enqueue_async(urf_ctx* ctx, const void* const* data, const int* n, int batch, const urf_cloud2_format* fmt, bool per_scan,
+                  urf_result* outs, int8_t* const* label8) {
   if (!ctx) return URF_ERR_INVALID;
   const int rc = alloc_second_slot(ctx);
-  return rc != URF_OK ? rc : enqueue_batch(ctx, data, n, batch, step, ox, oy, oz, oi, fmt, outs, label8, nullptr);
+  return rc != URF_OK ? rc : enqueue_batch(ctx, data, n, batch, fmt, per_scan, outs, label8, nullptr);
 }
 }  // namespace
 
 int urf_enqueue_batch(urf_ctx* ctx, const float* const* xyzi, const int* n, int batch, urf_result* outs, int8_t* const* label8) {
-  return enqueue_async(ctx, reinterpret_cast<const void* const*>(xyzi), n, batch, 0, 0, 0, 0, -1, nullptr, outs, label8);
+  return enqueue_async(ctx, reinterpret_cast<const void* const*>(xyzi), n, batch, nullptr, false, outs, label8);
 }
 
 int urf_enqueue_cloud2_batch(urf_ctx* ctx, const void* const* data, const int* n_points, int batch, int point_step, int off_x, int off_y,
                              int off_z, int off_intensity, urf_result* outs, int8_t* const* label8) {
-  if (point_step == 0) return URF_ERR_INVALID;
-  return enqueue_async(ctx, data, n_points, batch, point_step, off_x, off_y, off_z, off_intensity, nullptr, outs, label8);
+  const urf_cloud2_format f{point_step, off_x, off_y, off_z, off_intensity};
+  return enqueue_async(ctx, data, n_points, batch, &f, false, outs, label8);
 }
 
-// the mixed entry points take their step and offsets from fmt; a batch of one format runs as the one-format call
 int urf_enqueue_cloud2_batch_mixed(urf_ctx* ctx, const void* const* data, const int* n_points, const urf_cloud2_format* fmt, int batch,
                                    urf_result* outs, int8_t* const* label8) {
-  if (!fmt) return URF_ERR_INVALID;
-  return enqueue_async(ctx, data, n_points, batch, 0, 0, 0, 0, -1, fmt, outs, label8);
+  return fmt ? enqueue_async(ctx, data, n_points, batch, fmt, true, outs, label8) : URF_ERR_INVALID;
 }
 
 int urf_process_cloud2_batch_mixed(urf_ctx* ctx, const void* const* data, const int* n_points, const urf_cloud2_format* fmt, int batch,
                                    urf_result* outs, int8_t* const* label8) {
-  if (!fmt) return URF_ERR_INVALID;
-  return process_batch_impl(ctx, data, n_points, batch, 0, 0, 0, 0, -1, fmt, outs, label8, nullptr);
+  return fmt ? process_batch_impl(ctx, data, n_points, batch, fmt, true, outs, label8, nullptr) : URF_ERR_INVALID;
 }
 
 int urf_finish_batch(urf_ctx* ctx) { return finish_batch(ctx); }
 
 int urf_process_batch(urf_ctx* ctx, const float* const* xyzi, const int* n, int batch, urf_result* outs) {
-  return process_batch_impl(ctx, reinterpret_cast<const void* const*>(xyzi), n, batch, 0, 0, 0, 0, -1, nullptr, outs, nullptr, nullptr);
+  return process_batch_impl(ctx, reinterpret_cast<const void* const*>(xyzi), n, batch, nullptr, false, outs, nullptr, nullptr);
 }
 
 int urf_process_batch_xyz(urf_ctx* ctx, const float* const* xyz, const int* n, int batch, urf_result* outs, int8_t* const* label8) {
-  return process_batch_impl(ctx, reinterpret_cast<const void* const*>(xyz), n, batch, 12, 0, 4, 8, -1, nullptr, outs, label8, nullptr);
+  const urf_cloud2_format f{12, 0, 4, 8, -1};
+  return process_batch_impl(ctx, reinterpret_cast<const void* const*>(xyz), n, batch, &f, false, outs, label8, nullptr);
 }
 
-// the record entry points reject point_step 0 themselves: the body reads step 0 as float4 input
 int urf_process_cloud2_batch(urf_ctx* ctx, const void* const* data, const int* n_points, int batch, int point_step, int off_x, int off_y,
                              int off_z, int off_intensity, urf_result* outs, int8_t* const* label8) {
-  if (point_step == 0) return URF_ERR_INVALID;
-  return process_batch_impl(ctx, data, n_points, batch, point_step, off_x, off_y, off_z, off_intensity, nullptr, outs, label8, nullptr);
+  const urf_cloud2_format f{point_step, off_x, off_y, off_z, off_intensity};
+  return process_batch_impl(ctx, data, n_points, batch, &f, false, outs, label8, nullptr);
 }
 
 int urf_process_cloud2(urf_ctx* ctx, const void* data, int n, int point_step, int off_x, int off_y, int off_z, urf_result* out) {
-  if (point_step == 0) return URF_ERR_INVALID;
-  return process_batch_impl(ctx, &data, &n, 1, point_step, off_x, off_y, off_z, -1, nullptr, out, nullptr, nullptr);
+  const urf_cloud2_format f{point_step, off_x, off_y, off_z, -1};
+  return process_batch_impl(ctx, &data, &n, 1, &f, false, out, nullptr, nullptr);
 }
 
 int urf_process_cloud2_packed(urf_ctx* ctx, const void* data, int n, int point_step, int off_x, int off_y, int off_z,
                               int off_intensity, urf_result* out, urf_clouds* clouds) {
-  if (!clouds || point_step == 0) return URF_ERR_INVALID;
-  return process_batch_impl(ctx, &data, &n, 1, point_step, off_x, off_y, off_z, off_intensity, nullptr, out, nullptr, clouds);
+  const urf_cloud2_format f{point_step, off_x, off_y, off_z, off_intensity};
+  return clouds ? process_batch_impl(ctx, &data, &n, 1, &f, false, out, nullptr, clouds) : URF_ERR_INVALID;
 }
 
 int urf_process(urf_ctx* ctx, const float* xyzi, int n, urf_result* out) {

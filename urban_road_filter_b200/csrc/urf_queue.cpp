@@ -12,14 +12,14 @@
 // takes the run of DONE slots that starts there through take_done_run and hands it out through hand_out.
 //
 // Label slots are int32, or int8 with URF_QUEUE_LABEL8: the worker then asks the batch body for one-byte labels (float4
-// queues go through urf_enqueue_cloud2_batch with 16-byte records, as the synchronous path went through
-// urf_process_cloud2_batch). With URF_QUEUE_ORDER a slot also holds the scan's emission order and ring_start: the worker
-// points the batch call's outs at them, the batch body fills them as it does for any caller, and delivery lends them with
-// the labels.
+// queues hand their scans over as 16-byte records, the format {16, 0, 4, 8, 12}). With URF_QUEUE_ORDER a slot also holds
+// the scan's emission order and ring_start: the worker points the batch call's outs at them, the batch body fills them as it
+// does for any caller, and delivery lends them with the labels.
 //
 // Scan kinds: float4 points, records of one format (urf_queue_create_cloud2), or records of the formats of a table, each
-// submit naming its scan's format (urf_queue_create_formats). A slot holds max_points records of the largest format, remembers
-// its scan's format, and a formats queue's run goes to urf_enqueue_cloud2_batch_mixed with each scan's format.
+// submit naming its scan's format (urf_queue_create_formats). A slot holds max_points records of the largest format and
+// remembers its scan's format. A run of float4 scans with int32 labels goes to urf_enqueue_batch; every other run goes to
+// urf_enqueue_cloud2_batch_mixed with each scan's format, and the batch body runs a run of one format as a one-format batch.
 //
 // The worker is one loop with a depth. On a real context it keeps two batches in flight (urf_enqueue_batch /
 // urf_finish_batch): it enqueues what is pending, enqueues the next pending run too if there is one, and only then waits
@@ -113,7 +113,7 @@ struct Run {
   std::vector<const float*> ptrs;
   std::vector<int> ns;
   std::vector<int32_t> fidx;             // per scan: its index into the queue's formats
-  std::vector<urf_cloud2_format> fmts;   // per scan: its format (a formats queue's mixed batch)
+  std::vector<urf_cloud2_format> fmts;   // per scan: its format (the batch call of every run but float4 with int32 labels)
   std::vector<urf_result> outs;
   std::vector<int8_t*> l8;
   int rc = URF_OK;             // synchronous stand-in: what the batch function returned, reported by finish_run
@@ -223,12 +223,9 @@ int enqueue_run(urf_queue* q, Run& r) {
     return URF_OK;
   }
   if (q->kind == ScanKind::Float4 && !q->label8) return urf_enqueue_batch(q->ctx, r.ptrs.data(), r.ns.data(), B, r.outs.data(), nullptr);
-  const auto data = reinterpret_cast<const void* const*>(r.ptrs.data());
   int8_t* const* l8 = q->label8 ? r.l8.data() : nullptr;
-  if (q->kind == ScanKind::Formats) return urf_enqueue_cloud2_batch_mixed(q->ctx, data, r.ns.data(), r.fmts.data(), B, r.outs.data(), l8);
-  // float4 scans with int8 labels are 16-byte records (x, y, z, intensity at 0, 4, 8, 12) to the record body
-  const urf_cloud2_format& f = q->formats[0];
-  return urf_enqueue_cloud2_batch(q->ctx, data, r.ns.data(), B, f.point_step, f.off_x, f.off_y, f.off_z, f.off_intensity, r.outs.data(), l8);
+  return urf_enqueue_cloud2_batch_mixed(q->ctx, reinterpret_cast<const void* const*>(r.ptrs.data()), r.ns.data(), r.fmts.data(), B,
+                                        r.outs.data(), l8);
 }
 
 // Waits for the oldest run in flight, r.
