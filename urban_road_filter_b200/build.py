@@ -138,6 +138,22 @@ def build_glue() -> str:
     return tgt
 
 
+def build_glue_ros2() -> str:
+    """ros2/urf_ros2_node.cpp (the ROS 2 node) compiled against the shim rclcpp headers of tests/ros2_shim + a C test entry."""
+    bdir = os.path.join(ROOT, "build")
+    os.makedirs(bdir, exist_ok=True)
+    tgt = os.path.join(bdir, "libglue_ros2.so")
+    shim = os.path.join(ROOT, "tests", "ros2_shim")
+    deps = [os.path.join(ROOT, "ros2", "urf_ros2_node.cpp"), os.path.join(ROOT, "tests", "kat", "ros2_glue_entry.cpp"),
+            os.path.join(ROOT, "include", "urf.h"), LIB]
+    deps += [os.path.join(d, f) for d, _, fs in os.walk(shim) for f in fs]
+    if _stale(tgt, deps):
+        subprocess.run(["g++", "-std=c++17", "-O2", "-Wall", "-fPIC", "-shared", "-I" + shim, "-I" + os.path.join(ROOT, "include"),
+                        "-o", tgt, os.path.join(ROOT, "tests", "kat", "ros2_glue_entry.cpp"),
+                        "-L" + PKG, "-l:liburf_b200.so", "-Wl,-rpath,$ORIGIN/../urban_road_filter_b200"], check=True)
+    return tgt
+
+
 if __name__ == "__main__":
     print(build_lib(force=True, verbose=True))
     build_oracle()
